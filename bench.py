@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — sliding-window continuous-time BA hot path (BASELINE.json metric) on B200.
+"""bench.py — sliding-window continuous-time BA hot path (BASELINE.json metric) on H100.
 
     python bench.py --gpus N --steps K --warmup W            # CUDA engine (this repo)
     python bench.py --impl reference --gpus N --steps K ...  # CPU restatement of the reference path
@@ -13,6 +13,9 @@ e2e    = the same metric through the C-ABI with HOST buffers: state + factors H2
 N > 1  = N independent replicas (one window per GPU, no data-path collective; "weak"); the
          landmark-sharded C4 run with its NCCL all-reduce is reported under "c4".
 One JSON line on stdout (rank 0).
+--dump-outputs DIR writes what the last timed resident solve returned to its caller (knots, biases, inverse depths,
+line delay, costs) as DIR/<name>.npy in float64; the window is generated from a fixed seed, so two builds can be
+compared output for output.
 """
 import argparse
 import importlib
@@ -38,7 +41,7 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
@@ -129,6 +132,21 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm), "source": "nvidia-smi"}
 
 
+def device_info(index):
+    """Name and power limit of the card the numbers were measured on (a power-capped card runs lower clocks)."""
+    import torch
+    out = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        vis = os.environ.get("CUDA_VISIBLE_DEVICES")
+        phys = vis.split(",")[index] if vis else str(index)
+        r = subprocess.run(["nvidia-smi", f"--id={phys}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=20)
+        out["power_limit_w"] = float(r.stdout.strip())
+    except Exception:
+        pass
+    return out
+
+
 def oracle_lib():
     so = os.path.join(ROOT, "oracle", "liboracle.so")
     if not os.path.exists(so):
@@ -173,9 +191,11 @@ VISUAL_KFLOP = 11.1  # SURVEY 8(d): ~6.0 kflop residual + analytic Jacobians (wi
 
 def roofline_k1_fp64(w_n_obs, visual_ms, fp64_tflops):
     """SURVEY 8(d) asks for K1's fp64 fraction next to its (by design tiny) HBM fraction: algorithmic flops of one
-    launch = 11.1 kflop per visual block, over the kernel's CUDA-event time, against the fp64 rate measured in-run."""
+    launch = 11.1 kflop per visual block, over the kernel's CUDA-event time, against the DFMA rate measured in-run (K1's
+    arithmetic is almost all DFMA; its few DMMA products are not counted separately)."""
     ach = VISUAL_KFLOP * 1e3 * w_n_obs / (visual_ms * 1e-3) / 1e12
     return {"bound": "fp64", "achieved": ach, "peak": fp64_tflops, "unit": "TFLOP/s", "frac": ach / fp64_tflops,
+            "peak_source": "fp64 DFMA rate measured in this run (ctvio_measure_fp64_tflops)",
             "algorithmic_flops": VISUAL_KFLOP * 1e3 * w_n_obs, "kernel_ms": visual_ms, "kernel": "visual_kernel<true> (K1)"}
 
 
@@ -377,6 +397,17 @@ def run_c5_streaming(lib, n_windows, device, cpu_windows):
     return out
 
 
+def dump_outputs(path, est, summary):
+    """What the resident solve hands its caller: the solved state and the summary's costs / counts (float64)."""
+    os.makedirs(path, exist_ok=True)
+    q, p = est.GetKnots()
+    arrays = {"knots_q": q, "knots_p": p, "biases": est.GetBiases(), "inv_depths": est.GetInvDepths(),
+              "line_delay": [est.GetLineDelay()],
+              "summary": [summary.iterations, summary.num_jacobian_evals, summary.initial_cost, summary.final_cost]}
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), np.asarray(a, dtype=np.float64))
+
+
 def run_reference(args, rank, world):
     if rank != 0:
         return
@@ -441,6 +472,8 @@ def main():
     ap.add_argument("--impl", default="ctvio", choices=["ctvio", "reference"])
     ap.add_argument("--cpu-budget-s", type=float, default=10.0)
     ap.add_argument("--no-c4", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed solve's outputs as DIR/<name>.npy (float64)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ctvio" else args.warmup
     rank = int(os.environ.get("RANK", "0"))
@@ -481,7 +514,7 @@ def main():
     # ---------------- resident path (value) ----------------
     est = pkg.setup_estimator(lib, w, device=local_rank)
     est.SaveState()
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
     sampler = ClockSampler(local_rank)
     per_ms, evals, iters, launches, wall = [], 0, 0, 0, 0.0
     for it in range(args.warmup + args.steps):
@@ -503,6 +536,8 @@ def main():
     clocks = sampler.stop()
     dev_s = sum(per_ms) * 1e-3
     summ = s
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, est, summ)
 
     # ---------------- e2e path: host buffers through the C-ABI ----------------
     e2e_est = pkg.Estimator(lib, pkg.make_config(device=local_rank, **w.config_kwargs()))
@@ -534,6 +569,8 @@ def main():
     # ---------------- kernel stage timings + roofline of the dominant kernel ----------------
     prof = est.ProfileKernels(reps=20, flush_l2=True) if rank == 0 else None
     fp64_tflops = est.MeasureFp64Tflops() if rank == 0 else None
+    # K5 runs its trailing updates on the fp64 tensor cores (DMMA m8n8k4), a separate pipe from DFMA
+    tensor_tflops = est.MeasureFp64TensorTflops() if rank == 0 else None
     if world > 1:  # every rank needs the measured fp64 rate for its shard's K1 fraction
         fp64_tflops = est.MeasureFp64Tflops()
     c4 = None
@@ -566,24 +603,15 @@ def main():
 
     if rank == 0:
         peaks, how = measured_peaks()
-        # dominant kernel of the step: the dense solve (K5, chol_dag_kernel; > 50 % of the LM iteration, see
-        # profiles/r1/e_launches_c2.csv).  It computes on the fp64 tensor/FMA pipe: algorithmic flops of one launch =
-        # n^3/3 (factor) + 2 n^2 (two triangular solves), n = n_p; the denominator is the fp64 rate measured in this run
-        # (MEASURED_PEAKS.json only has HBM and bf16 numbers).  K1's HBM-side roofline is reported next to it.
+        # dominant kernel of the step: the dense solve (K5, chol_dag_kernel; see "stage_ms").  Its updates run on the
+        # fp64 tensor cores: algorithmic flops of one launch = n^3/3 (factor) + 2 n^2 (two triangular solves), n = n_p,
+        # against the DMMA rate measured in this run (MEASURED_PEAKS.json only has HBM and bf16 numbers).  K1's
+        # HBM-side roofline is reported next to it.
         n_p = 6 * w.n_knots + 6 * len(w.kf_times) + 1
         chol_flops = n_p ** 3 / 3.0 + 2.0 * n_p ** 2
         ach_tf = chol_flops / (prof["cholesky_solve"] * 1e-3) / 1e12
         alg = algorithmic_bytes_visual(w)
         ach = alg / (prof["visual"] * 1e-3) / 1e9
-        traffic, traffic_k1, traffic_src = None, None, None
-        try:
-            with open(os.path.join(ROOT, "profiles", "kernel_traffic.json")) as f:
-                tj = json.load(f)
-                traffic, traffic_k1 = tj.get("c2_chol_dag_dram_bytes_per_launch"), tj.get("c2_visual_dram_bytes_per_launch")
-                traffic_src = "STATIC: dram__bytes_read+write per launch from the committed ncu --set full capture " + \
-                              str(tj.get("source", "profiles/kernel_traffic.json")) + " (not re-measured in this run)"
-        except Exception:
-            pass
         cpu1 = cpu_solve_rate(w, 1, args.cpu_budget_s) if world == 1 else None
         line = {
             "metric": "residual+Jacobian block evaluations per second (sliding-window LM solve)",
@@ -599,21 +627,23 @@ def main():
                     "d2h_bytes_per_step": int(d2h), "ms_per_step": 1e3 * e2e_s_max / args.steps},
             "gpu_launches": int(launches_all),
             "clocks": clocks,
-            "roofline": {"bound": "tensor", "achieved": ach_tf, "peak": fp64_tflops, "unit": "TFLOP/s",
-                         "frac": ach_tf / fp64_tflops, "traffic": traffic, "traffic_source": traffic_src,
+            "device": device_info(local_rank),
+            "roofline": {"bound": "tensor", "achieved": ach_tf, "peak": tensor_tflops, "unit": "TFLOP/s",
+                         "frac": ach_tf / tensor_tflops,
                          "kernel": "chol_dag_kernel (K5)",
-                         "peak_source": "fp64 DFMA/DMMA rate measured in this run (ctvio_measure_fp64_tflops); "
-                                        "MEASURED_PEAKS.json has no fp64 figure",
+                         "peak_source": "rate of the fp64 tensor-core instruction K5 issues (mma.sync.m8n8k4.f64), "
+                                        "measured in this run (ctvio_measure_fp64_tensor_tflops); not the data sheet's "
+                                        "fp64 tensor peak, which this shape does not reach",
                          "algorithmic_flops": chol_flops, "kernel_ms": prof["cholesky_solve"],
                          "note": "serial pivot chain of an n=%d factorisation: latency bound, not pipe bound "
-                                 "(floor ~126 cycles per column = %.1f us, see DESIGN.md)" % (n_p, n_p * 126 / 1.965e3)},
+                                 "(see DESIGN.md)" % n_p},
             "roofline_k1": {"bound": "hbm", "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                            "frac": ach / peaks["hbm_gbs"], "traffic": traffic_k1, "kernel": "visual_kernel<true> (K1)",
-                            "peak_source": how, "algorithmic_bytes": alg, "kernel_ms": prof["visual"],
-                            "traffic_source": traffic_src},
+                            "frac": ach / peaks["hbm_gbs"], "kernel": "visual_kernel<true> (K1)",
+                            "peak_source": how, "algorithmic_bytes": alg, "kernel_ms": prof["visual"]},
             "roofline_k1_fp64": roofline_k1_fp64(w.n_obs, prof["visual"], fp64_tflops),
             "stage_ms": prof,
             "fp64_peak_tflops_measured": fp64_tflops,
+            "fp64_tensor_peak_tflops_measured": tensor_tflops,
             "solver": {"iterations": summ.iterations, "jacobian_passes": summ.num_jacobian_evals,
                        "termination": summ.as_dict()["termination_name"], "final_cost": summ.final_cost},
         }

@@ -1,11 +1,11 @@
-"""ctrl-vio_b200 — B200-native sliding-window continuous-time bundle adjustment.
+"""ctrl-vio_b200 — H100-native sliding-window continuous-time bundle adjustment.
 
-The product is `csrc/libctvio_b200.so` (hand-written sm_100a CUDA behind the C-ABI
+The product is `csrc/libctvio_b200.so` (hand-written sm_90a CUDA behind the C-ABI
 of include/ctvio.h).  This Python package is only the host-side mirror used by
 tests and bench.py: ctypes binding (`binding.py`), the `Estimator` class with the
 reference's `TrajectoryEstimator` method names, and the synthetic window
 generator (`synthetic.py`).  There is no CPU fallback: `load()` raises when the
-CUDA library has not been built, and `ctvio_create` fails without a B200.
+CUDA library has not been built, and `ctvio_create` fails without an H100.
 
 The directory name contains a hyphen (it is the name the build contract asks
 for); import it with `importlib.import_module("ctrl-vio_b200")`.
@@ -31,7 +31,7 @@ _lib = None
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile the CUDA engine for sm_100a in-tree (csrc/build.sh)."""
+    """Compile the CUDA engine for sm_90a in-tree (csrc/build.sh)."""
     script = os.path.join(CSRC_DIR, "build.sh")
     env = dict(os.environ)
     if force:
@@ -49,7 +49,7 @@ def load() -> CtvioLib:
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise CtvioError(f"{LIB_PATH} is missing — run __graft_entry__.build() (nvcc, sm_100a). "
+            raise CtvioError(f"{LIB_PATH} is missing — run __graft_entry__.build() (nvcc, sm_90a). "
                              "There is no CPU fallback for the product path.")
         _lib = CtvioLib(LIB_PATH, "ctvio_")
     return _lib

@@ -102,7 +102,8 @@ ABI_SYMBOLS = [
     "eval_image_factors", "eval_imu_factors", "residual_summary", "eval_cost", "normal_equations",
     "query_trajectory", "triangulate",
     "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior", "ingest_feature_cloud", "add_image_features_from_slots",
-    "ingest_imu", "add_imu_from_table", "transfer_stats", "profile_kernels", "measure_fp64_tflops", "selfcheck_solver", "nccl_unique_id", "comm_init",
+    "ingest_imu", "add_imu_from_table", "transfer_stats", "profile_kernels", "measure_fp64_tflops", "measure_fp64_tensor_tflops",
+    "selfcheck_solver", "nccl_unique_id", "comm_init",
 ]
 
 
@@ -114,7 +115,7 @@ DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enab
 
 
 def _addr(a):
-    # (numpy's `.ctypes.data_as(...)` costs ~2.3 us per array; the raw address as a void pointer ~1.3 us: the host-buffer
+    # (numpy's `.ctypes.data_as(...)` costs more per array than the raw address as a void pointer: the host-buffer
     #  path passes ~25 arrays per window)
     return C.c_void_p(a.__array_interface__["data"][0]) if a is not None else None
 
@@ -468,6 +469,11 @@ class Estimator:
     def MeasureFp64Tflops(self):
         v = C.c_double()
         self.lib.call("measure_fp64_tflops", self.h, C.byref(v))
+        return v.value
+
+    def MeasureFp64TensorTflops(self):
+        v = C.c_double()
+        self.lib.call("measure_fp64_tensor_tflops", self.h, C.byref(v))
         return v.value
 
     # --- multi-GPU -----------------------------------------------------------------

@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# Build libctvio_b200.so in-tree for sm_100a (B200).  nvcc cross-compiles without a GPU.
+# Build libctvio_b200.so in-tree for sm_90a (H100).  nvcc cross-compiles without a GPU.
 # Every object is rebuilt when its source, ANY header of this directory, the public C-ABI header or this script is
 # newer than it (the header set is globbed, so a new .cuh / .h can not be forgotten in a dependency list).
 set -euo pipefail
@@ -9,7 +9,7 @@ SRCS="engine.cu kernels_residual.cu kernels_linear.cu chol_coop.cu chol_dag.cu m
 HDRS="$(ls *.h *.cuh) ../../include/ctvio.h build.sh"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 # NCCL: only <nccl.h> (types) is needed at build time; the library is dlopen'ed by comm.cu on first use.
-FLAGS="${CTVIO_EXTRA_NVCC_FLAGS:-} -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 --expt-relaxed-constexpr -Xcompiler -fPIC -Xptxas -v"
+FLAGS="${CTVIO_EXTRA_NVCC_FLAGS:-} -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 --expt-relaxed-constexpr -Xcompiler -fPIC -Xptxas -v"
 objs=""
 relink=0
 [[ -f "$OUT" ]] || relink=1
@@ -29,6 +29,6 @@ done
 for p in "${pids[@]:-}"; do [[ -n "$p" ]] && wait "$p"; done
 for f in $SRCS; do [[ "${f%.cu}.o" -nt "$OUT" ]] && relink=1; done
 if [[ $relink -eq 1 ]]; then
-  $NVCC -gencode arch=compute_100a,code=sm_100a -shared -o "$OUT" $objs -lcudart -ldl
+  $NVCC -gencode arch=compute_90a,code=sm_90a -shared -o "$OUT" $objs -lcudart -ldl
   echo "built $OUT"
 fi

@@ -3,7 +3,7 @@
 // this one is used when the window is so large that not every 64x64 tile can have its own SM (n_p > ~1000), when the
 // runtime refuses the DAG's cooperative launch, or on request (CTVIO_CHOL=coop, A/B measurements).
 // Replaces the factor/solve half of Ceres' SPARSE_NORMAL_CHOLESKY step (trajectory_estimator.cpp:374;
-// Ceres is not under /root/reference) on the Schur-reduced system.
+// Ceres is not part of the reference repository) on the Schur-reduced system.
 //
 //   per block column k (NB = 64):
 //     phase P  every CTA that owns a panel slab loads the (already updated) diagonal block, factors it
@@ -21,6 +21,7 @@
 
 #include "chol_tiles.cuh"
 #include "kernels.h"
+#include "marginalize.h"
 
 namespace ctvio {
 
@@ -249,55 +250,12 @@ __global__ void latency_probe_kernel(double seed, long long* out, double* sink) 
   }
   sink[threadIdx.x] = x;
 }
-// DMMA (fp64 tensor core, mma.sync.m8n8k4) throughput + dependent latency probe
-__device__ __forceinline__ void dmma(double& d0, double& d1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
-}
-__global__ void __launch_bounds__(256) dmma_peak_kernel(double* out, int iters, double seed, long long* lat) {
-  double c[8][2];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) { c[i][0] = seed + i; c[i][1] = seed - i; }
-  const double a = 1.0 + 1e-9 * threadIdx.x, b = 1e-3 + 1e-9 * threadIdx.x;
-  for (int i = 0; i < iters; ++i) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) dmma(c[j][0], c[j][1], a, b);
-  }
-  double s = 0.0;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) s += c[i][0] + c[i][1];
-  if (lat && blockIdx.x == 0 && threadIdx.x < 32) {  // dependent chain, one warp
-    double d0 = s, d1 = s + 1;
-    const long long t0 = clock64();
-#pragma unroll 1
-    for (int i = 0; i < 64; ++i) { dmma(d0, d1, a, b); dmma(d0, d1, a, b); dmma(d0, d1, a, b); dmma(d0, d1, a, b); }
-    const long long t1 = clock64();
-    s += d0 + d1;
-    if (threadIdx.x == 0) lat[0] = t1 - t0;
-  }
-  out[blockIdx.x * blockDim.x + threadIdx.x] = s;
-}
+// DMMA throughput + dependent latency: the fp64 tensor-core micro-benchmark of misc_kernels.cu at a chosen occupancy
 extern "C" int ctvio_debug_dmma(int ctas_per_sm, double* tflops, double* dep_latency_cycles) {
-  int dev = 0, n_sm = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-  const int ctas = n_sm * ctas_per_sm, iters = 1 << 13;
-  double* out; long long* lat;
-  cudaMalloc(&out, size_t(ctas) * 256 * 8); cudaMalloc(&lat, 8);
-  cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-  float best = 1e30f;
-  for (int rep = 0; rep < 4; ++rep) {
-    cudaEventRecord(e0);
-    dmma_peak_kernel<<<ctas, 256>>>(out, iters, 1.0 + rep, lat);
-    cudaEventRecord(e1); cudaEventSynchronize(e1);
-    float ms; cudaEventElapsedTime(&ms, e0, e1);
-    if (rep > 0 && ms < best) best = ms;
-  }
-  long long l = 0; cudaMemcpy(&l, lat, 8, cudaMemcpyDeviceToHost);
-  *dep_latency_cycles = double(l) / 256.0;
-  // per mma: 8x8x4 FMAs = 512 flop; per warp-iteration 8 mma; 8 warps per CTA
-  *tflops = 512.0 * 8.0 * 8.0 * double(iters) * ctas / (best * 1e-3) / 1e12;
-  cudaFree(out); cudaFree(lat);
-  return cudaGetLastError() == cudaSuccess ? 0 : -1;
+  const double v = measure_fp64_tensor_tflops(0, ctas_per_sm, dep_latency_cycles);
+  if (v < 0) return -1;
+  *tflops = v;
+  return 0;
 }
 extern "C" int ctvio_debug_latency(int nthreads, long long* out6) {
   long long* d; double* sink;
@@ -312,7 +270,7 @@ extern "C" int ctvio_debug_latency(int nthreads, long long* out6) {
 
 int launch_factor_solve(const LinearLaunch& a, cudaStream_t s) {
   // CTVIO_CHOL=coop forces the barrier kernel (A/B measurements, tests/...::test_barrier_cholesky_fallback_*); read on
-  // every call (a getenv costs nanoseconds against a 60 us kernel) so that one process can exercise both paths
+  // every call (a getenv costs nanoseconds against the kernel) so that one process can exercise both paths
   const char* env = std::getenv("CTVIO_CHOL");
   const int mode = (env && std::string(env) == "coop") ? 1 : 0;
   if (mode == 0 && a.chol_part && a.chol_flags && chol_dag_supported(a.npad, device_sm_count())) return launch_chol_dag(a, s);

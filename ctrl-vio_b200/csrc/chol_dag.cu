@@ -1,6 +1,6 @@
 // K5 (fast path): tile-DAG Cholesky + both triangular solves of the reduced camera system in ONE persistent
 // kernel WITHOUT grid-wide barriers.  Replaces the factor/solve half of Ceres' SPARSE_NORMAL_CHOLESKY step
-// (estimator/trajectory_estimator.cpp:374; Ceres itself is not under /root/reference) on the Schur-reduced system.
+// (estimator/trajectory_estimator.cpp:374; Ceres itself is not part of the reference repository) on the Schur-reduced system.
 //
 // Owner computes: every 64x64 tile (i, j), i >= j, of the lower triangle has ONE owner CTA that keeps the tile in
 // tensor-core fragments from the first to the last update, so the trailing matrix is never re-read or re-written in HBM.
@@ -11,7 +11,7 @@
 //     j IN STEP with its factorisation (one packet = 16 columns of L(i,j)); the sub-diagonal CTA (j+1, j) streams each
 //     finished 16-column slab to diagonal CTA j+1, which applies it as a rank-16 update: when the last pivot of column j
 //     is done, one 16x16 product, one slab hop and one rank-16 update separate it from the first pivot of column j+1.
-// r2 changes vs r1 (profiles/r2/README.md has the timelines): no 64x64 inverse on the chain (was ~half of the diagonal
+// r2 changes vs r1: no 64x64 inverse on the chain (was ~half of the diagonal
 // factor), solve pipelined with the factorisation, the chain's GEMM work split over two SMs per column (r1: one), and
 // the chain's messages are SELF-VALIDATING WORDS (sentinel = not yet written) instead of store + fence + flag + acquire.
 // Tiles that feed later GEMM updates still use release/acquire flags in global memory (epoch valued: never cleared).
@@ -51,7 +51,7 @@ constexpr unsigned long long kSentinel = 0xFFF8C0DEC0DE0001ull;
 // Chain positions p = 0, 1, 2, ... = diag 0, tile (1,0), diag 1, tile (2,1), ... are consecutive CTAs, so position p + 1
 // sits in the same cluster unless p + 1 is a multiple of the cluster size: the producer then writes its message words
 // straight into the consumer's shared memory (st.shared::cluster), the consumer spins on its OWN shared memory
-// (~30 cycles per poll instead of an L2 round trip of 600-1200, die-crossing dependent).  Same self-validating words:
+// (a poll of local shared memory instead of an L2 round trip).  Same self-validating words:
 // the consumer fills its receive area with sentinels, then arrives at the cluster barrier; a producer waits on that
 // barrier once, before its first remote store.
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return static_cast<unsigned>(__cvta_generic_to_shared(p)); }
@@ -189,7 +189,7 @@ __device__ __forceinline__ void tile_matvec(const double* Lrm, const double* v, 
 // f[mt][nt] -= A_frag(mt) B_frag(nt)' over nk4 k-steps of 4, for the (mt, nt) pairs of the COMPILE-TIME mask (bit 4 mt + nt).
 // Which fragments a warp has to touch is warp-uniform but only known at run time (it depends on the warp's position in
 // the folded fragment grid and on the 16-column step); a run-time predicate per mma.sync makes ptxas guard EVERY DMMA with
-// a WARPSYNC (measured: a 64x16x64 slab update took 2.3 us instead of 0.5).  So the run-time value selects one of a
+// a WARPSYNC (which made a 64x16x64 slab update several times slower).  So the run-time value selects one of a
 // handful of instantiations and the inner loop is branch free.
 template <unsigned MASK>
 __device__ __forceinline__ void mma_masked(Frag& f, const double* pa, int sa, const double* pb, int sb, const Lane& L, int nk4) {
@@ -506,7 +506,7 @@ __global__ void __launch_bounds__(256, 1) chol_dag_kernel(CholDagArgs a) {
       // The last update T -= L(i,j-1) L(j,j-1)' is STREAMED: both operand tiles arrive 16 columns (k) at a time, as
       // self-validating slabs, straight from the CTAs (i, j-1) and (j, j-1) that are still solving them, and are applied as
       // rank-16 updates.  (Waiting for the finished tiles - flag, 2 x 32 KB from L2, four lazy slab products inside the
-      // solve - left this CTA ~2 us behind the packets of column j at every column of the critical chain.)
+      // solve - left this CTA behind the packets of column j at every column of the critical chain.)
       const double* srcA = a.Spub + (size_t(i) * nb + (j - 1)) * 4096;
       const double* srcB = a.Spub + (size_t(j) * nb + (j - 1)) * 4096;
       const int r0 = tid >> 5, c0 = (tid & 31) * 2;  // thread's two double2 of a slab: rows r0, r0 + 8
@@ -683,7 +683,7 @@ __global__ void __launch_bounds__(256, 1) chol_dag_kernel(CholDagArgs a) {
   DSTAMP(j, 6);
   if (j == nb - 1) {
     // last block: the backward sweep starts here, with nothing to wait for - substitute straight from the packets
-    // (forming the explicit inverse first, as the other columns do off the chain, would put ~4 us ON it)
+    // (forming the explicit inverse first, as the other columns do off the chain, would put that work ON it)
     __syncthreads();
     block_solve_packets<false>(Pk, vec, x16, tid);  // vec = yf_j on entry (set above), x_j on exit
     if (tid < kCholNB) {

@@ -97,7 +97,7 @@ __device__ __forceinline__ bool chol4(const double a[4][4], double l[4][4], doub
 //       with P1 of the next step (warp 0 updates the next diagonal block first and starts its pivot chain at once).
 //
 // `side(s)` is called by the threads of warps 1..7 (tid >= 32) at the start of 16-column step s, i.e. while warp 0
-// runs the P1 chain and they would otherwise idle at the barrier: room for ~1 us of unrelated work per step.
+// runs the P1 chain and they would otherwise idle at the barrier: room for unrelated work per step.
 struct NoSideJob {
   __device__ __forceinline__ void operator()(int) const {}
 };
@@ -122,8 +122,7 @@ __device__ __forceinline__ void factor_p1_warp(double* D, double* L16t, double* 
   bool bad = false;
   // Software pipelined: the pivot of column j + 1 (shuffle, test, reciprocal square root: the long dependent part) is
   // issued BEFORE the 15 - j shared-memory loads and update FMAs of column j, which then execute in its shadow.  In
-  // program order "pivot, then updates" the in-order issue of the update block delayed every pivot by ~50 cycles
-  // (measured 180-190 cycles per column against ~125 for the dependent chain itself).
+  // program order "pivot, then updates" the in-order issue of the update block delayed every pivot.
   double ajj = __shfl_sync(0xffffffffu, d, 0);
   {
     // positive and normal <=> biased exponent in [1, 2046] and sign clear (integer test: off the fp64 pipe)
@@ -305,7 +304,7 @@ __device__ __forceinline__ bool factor_and_invert_64(double* D, double* Xi, doub
       } else {
         // fragment column = warp (warp 7 also takes column 0); fragment rows start at max(ct, rt0); the look-ahead
         // fragments (rt0, rt0), (rt0+1, rt0), (rt0+1, rt0+1) are warp 0's.  (Keeping warp 4 - same scheduler as the
-        // pivot warp - out of the tensor-core work was measured to change nothing: the pivot chain runs at ~0.3x
+        // pivot warp - out of the tensor-core work was measured to change nothing: the pivot chain runs slower
         // while the other warps' DMMAs are in flight whichever scheduler issues them, i.e. the fp64 pipe behaves as
         // one SM-wide resource; the overlap still hides about half of P3.)
         const int ct = warp;

@@ -1,5 +1,5 @@
 // NCCL communicator wrappers (multi-GPU landmark sharding: one sum-allreduce of the reduced camera
-// system per LM step over NVLink 5 / NVSwitch).
+// system per LM step over NVLink / NVSwitch).
 //
 // NCCL is bound at run time (dlopen) the first time a communicator is requested, not at link time:
 //  * single-GPU users do not need NCCL at all;

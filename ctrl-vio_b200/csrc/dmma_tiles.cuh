@@ -1,12 +1,13 @@
-// 64x64 fp64 tiles on the 5th-generation tensor cores' fp64 path (mma.sync.m8n8k4.f64; tcgen05 has no fp64 kind):
+// 64x64 fp64 tiles on the Hopper tensor cores' fp64 path (mma.sync.m8n8k4.f64; wgmma has no fp64 kind):
 // shared by the dense Cholesky (K5) and the Schur complement (K4).
 #pragma once
 #include "chol_tiles.cuh"
 
 namespace ctvio {
 
-// ---- fp64 tensor-core tiles (mma.sync.m8n8k4.f64, measured 37 TFLOP/s = the DFMA peak, at 1/5 of the
-// shared-memory operand traffic of a 4x4 register-tiled DFMA loop) ----
+// ---- fp64 tensor-core tiles (mma.sync.m8n8k4.f64: about the DFMA rate on H100, measured by
+// ctvio_measure_fp64_tensor_tflops, at a fraction of the shared-memory operand traffic of a 4x4 register-tiled DFMA
+// loop) ----
 // The 64x64 tile is an 8x8 grid of m8n8 fragments.  Warp (wm, wn) = (warp & 3, warp >> 2) owns the fragment rows
 // {wm, 7 - wm} and the fragment columns {0, 1, 6, 7} (wn = 0) / {2, 3, 4, 5} (wn = 1): with this folding every warp
 // has the same amount of work when only the lower triangle of the product is needed (SYRK of a diagonal tile: at most

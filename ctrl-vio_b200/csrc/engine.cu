@@ -6,7 +6,7 @@
 // Jacobi scaling fixed at iteration 0, D^2 = clamp(diag)/mu, rho = dcost/dmodel accepted above 1e-3,
 // mu <- mu / max(1/3, 1-(2rho-1)^3) on success, mu <- mu/f, f <- 2f on failure, function / parameter
 // tolerances, Armijo projected line search when the line delay has bounds.
-// B200-first differences from a port: every candidate point is evaluated with full Jacobians into a
+// GPU-first differences from a port: every candidate point is evaluated with full Jacobians into a
 // second normal-equation buffer (an accepted step costs no re-linearisation pass), all per-step
 // quantities are reduced on the device, and the host reads back ONE 96-byte scalar block per step.
 #include <cuda_runtime.h>
@@ -48,7 +48,7 @@ int fail(int code, const std::string& msg) {
 thread_local size_t g_upload_bytes = 0;  // bytes moved by DevBuf::upload (index tables etc.), see ctvio_transfer_stats
 
 // Pinned staging arena of one engine: every host -> device copy of a C-ABI call is staged here and issued as a truly
-// asynchronous copy (a cudaMemcpyAsync from pageable memory is a synchronous staged copy: ~15 us each, ~20 of them per
+// asynchronous copy (a cudaMemcpyAsync from pageable memory is a synchronous staged copy, and there are ~20 of them per
 // window).  The arena is rewound whenever the engine's stream is found idle at the start of a call (then every copy that
 // read from it has completed); a request that does not fit falls back to the pageable copy and grows the arena at the
 // next rewind.
@@ -146,7 +146,7 @@ struct ctvio_engine {
   cudaEvent_t ev_iter = nullptr;  // recorded behind the last kernel of every LM step (before anything speculative)
   bool speculate = true;       // CTVIO_NO_SPECULATION=1 switches the pipelined driver off
   bool staged_publish = false; // CTVIO_STAGED_PUBLISH=1: the scalar block reaches the host through a device staging copy
-                               // forwarded from stream2 (measured: C2 +2.5 %, C4 -0.7 % - off by default)
+                               // forwarded from stream2 (measured: no gain - off by default)
   DevState& state(int i) { return i < 2 ? x[i] : xs; }
   int cur = 0;
   bool table_valid = false;
@@ -912,7 +912,7 @@ void evaluate(ctvio_engine* e, int xb, int nb, bool full, bool reset_cost = true
     }
     return;
   }
-  // (streaming windows: K2 + K3 one after the other take 31 us against K1's 20 - they get a stream each)
+  // (streaming windows: K2 + K3 one after the other take longer than K1 - they get a stream each)
   const bool split = fork && !e->imu.empty() && (!e->biasf.empty() || (e->prior.n > 0 && e->prior_enabled));
   if (fork) {
     cudaEventRecord(e->ev_fork, st);
@@ -1006,7 +1006,9 @@ int ctvio_create(const ctvio_config* cfg, ctvio_handle* out) {
   CUDA_OK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   CUDA_OK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major < 10) return fail(CTVIO_ERR_NO_DEVICE, "libctvio_b200 is built for sm_100a (B200) only");
+  // sm_90a code runs on compute capability 9.0 only (arch-specific features: no forward compatibility)
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(CTVIO_ERR_NO_DEVICE, "libctvio_b200 is built for sm_90a (H100) only");
   ctvio_engine* e = new ctvio_engine();
   e->cfg = *cfg;
   std::memset(&e->opt, 0, sizeof(e->opt));
@@ -1368,15 +1370,15 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
   };
 
   // ---- pipelined driver (single GPU, no bounds, default flush mode) --------------------------------------------
-  // The host round trip between two LM steps (publish -> host decision -> launch: ~10 us of an ~100 us step at C2) is
+  // The host round trip between two LM steps (publish -> host decision -> launch: a noticeable part of a step at C2) is
   // taken off the critical path: gradient_norm_kernel also takes the accept / radius decision on the device, and the
   // linear solve of step i+1 is enqueued BEFORE the host has seen step i, assuming acceptance (the common case),
   // reading its radius from device memory and writing its candidate into a third state buffer.  When the host then
   // finds step i rejected / invalid / terminating, the speculated kernels' results are simply never used (they touch
   // only the step vectors, the free state buffer and per-step scalars that the next real step resets).
-  // Measured (profiles/r2/README.md): -2.5 % at C2 / C5 sizes, but +8 % per LM step at 100 k observations and more, with
-  // identical kernels and a host that is provably ahead (CTVIO_LM_TRACE) - cause not found; the round trip it hides is
-  // 1 % of such a step anyway.  CTVIO_SPECULATION=always / never overrides the size test.
+  // It pays at C2 / C5 sizes but was measured slower per LM step at 100 k observations and more, with identical kernels
+  // and a host that is provably ahead (CTVIO_LM_TRACE) - cause not found; the round trip it hides is a small part of
+  // such a step anyway.  CTVIO_SPECULATION=always / never overrides the size test.
   bool spec_size_ok = e->img.size() <= 20000;
   if (const char* sp = std::getenv("CTVIO_SPECULATION")) {
     if (std::strcmp(sp, "always") == 0) spec_size_ok = true;
@@ -2071,6 +2073,15 @@ int ctvio_measure_fp64_tflops(ctvio_handle e, double* tflops) {
   cudaSetDevice(e->cfg.device);
   const double v = ctvio::measure_fp64_tflops(e->stream);
   if (v < 0) return fail(CTVIO_ERR_CUDA, "fp64 micro-benchmark failed");
+  *tflops = v;
+  return CTVIO_OK;
+}
+
+int ctvio_measure_fp64_tensor_tflops(ctvio_handle e, double* tflops) {
+  if (!e || !tflops) return fail(CTVIO_ERR_INVALID, "null argument");
+  cudaSetDevice(e->cfg.device);
+  const double v = ctvio::measure_fp64_tensor_tflops(e->stream);
+  if (v < 0) return fail(CTVIO_ERR_CUDA, "fp64 tensor-core micro-benchmark failed");
   *tflops = v;
   return CTVIO_OK;
 }

@@ -2,7 +2,7 @@
 // Eigen::SelfAdjointEigenSolver calls of marginalization_factor.cpp:240-263 for those sizes.
 //
 // The element-wise parallel Jacobi (marginalize.cu) pays two block-wide barriers and a pass over the whole matrix for
-// every round of n/2 rotations (n - 1 rounds per sweep, ~1.5 us each at n = 85: bound by one SM's shared-memory
+// every round of n/2 rotations (n - 1 rounds per sweep, each bound by one SM's shared-memory
 // bandwidth).  Here the matrix is cut into 8-wide index blocks; a round pairs the blocks (round-robin tournament), ONE
 // WARP per pair runs 8 rounds of 8 disjoint rotations on its private 16x16 sub-matrix - every (p in I, q in J) pair
 // once - and accumulates them into a 16x16 orthogonal Q; then the whole matrix is updated ONCE per block round as

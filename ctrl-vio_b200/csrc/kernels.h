@@ -178,7 +178,7 @@ inline int device_sm_count() {
 // of a kernel perform their flush in BLOCK-INDEX ORDER (a ticket in global memory: CTA i flushes after CTA i-1 has
 // flushed and fenced), so every sum is accumulated in one fixed order and a solve is bit-reproducible run to run.
 // Blocks are dispatched in index order, so a waiting CTA's predecessors are always resident or done (no deadlock).
-// The serialised flush costs time (C2: K1 22 -> ~60 us); it is a verification / regression mode, off by default.
+// The serialised flush costs time (K1 runs several times longer at C2); it is a verification / regression mode, off by default.
 #if defined(__CUDACC__)
 __device__ __forceinline__ void det_ticket_wait(const int* ticket, int my) {
   if (!ticket) return;

@@ -1,8 +1,8 @@
-// Linear-algebra / LM-step kernels of the CUDA engine (sm_100a, fp64).
+// Linear-algebra / LM-step kernels of the CUDA engine (sm_90a, fp64).
 //
 // Replaces what Ceres does inside ceres::Solve for one trust-region step
 // (trajectory_estimator.cpp:367-408 -> Ceres 1.14 levenberg_marquardt_strategy.cc +
-// SPARSE_NORMAL_CHOLESKY; Ceres is not under /root/reference):
+// SPARSE_NORMAL_CHOLESKY; Ceres is not part of the reference repository):
 //   K4  scale_copy + schur     reduced camera system  M = S A S + D^2 - sum_l w_l w_l' / h_l
 //   K5  (chol_dag.cu, chol_coop.cu) dense Cholesky (NB = 64) + block triangular solves
 //   K6  backsub / quad / apply landmark back-substitution, model cost change, x (+) delta, norms
@@ -447,7 +447,7 @@ __global__ void __launch_bounds__(1024) gradient_norm_kernel(LinearLaunch a, Sta
           const double t3 = __dmul_rn(__dmul_rn(t, t), t);
           d.radius_next = fmin(da.max_radius, __ddiv_rn(da.radius, fmax(1.0 / 3.0, __dsub_rn(1.0, t3))));
           // the driver's termination tests (same order as the host): a speculated step behind a terminating or
-          // rejected one returns at once instead of running ~70 us (C2) / ~200 us (C4) for nothing
+          // rejected one returns at once instead of running for nothing
           const double step_norm = sqrt(sc.step_norm2), x_norm = sqrt(sc.x_norm2);
           const bool stop = step_norm <= __dmul_rn(da.parameter_tolerance, __dadd_rn(x_norm, da.parameter_tolerance)) ||
                             fabs(__dsub_rn(da.x_cost, sc.cost_eval)) <= __dmul_rn(da.function_tolerance, da.x_cost) ||

@@ -1,4 +1,4 @@
-// Residual / Jacobian / normal-equation kernels of the CUDA engine (sm_100a, fp64).
+// Residual / Jacobian / normal-equation kernels of the CUDA engine (sm_90a, fp64).
 //
 //   knot_table_kernel   K0  per linearisation point: d_k, |d_k|, Jr^-1(d_k) for every knot pair
 //   visual_kernel       K1  replaces ImageFeatureDelayFactor::Evaluate (image_feature_factor.h:63-269)
@@ -7,7 +7,7 @@
 //   small_factors_kernel K3 replaces BiasFactor::Evaluate (:45-99) and MarginalizationFactor::Evaluate
 //                           (marginalization_factor.cpp:326-373)
 //
-// K1 design (B200-first, not a translation of the reference's per-factor virtual calls):
+// K1 design (GPU-first, not a translation of the reference's per-factor virtual calls):
 //   * observations are pre-sorted by frame-pair group = (first knot of the padded anchor window,
 //     first knot of the padded observation window); one CTA owns a chunk of one group, so every
 //     Jacobian row of the chunk lives in the same 61-dim local space

@@ -308,7 +308,7 @@ __global__ void __launch_bounds__(1024) jacobi_eig_kernel(double* A, double* V, 
 
 // Same algorithm with A and V resident in shared memory (odd row stride: column accesses spread over the banks);
 // used whenever both fit (n <= ~117), i.e. for every prior of a TUM-RSVI-scale window: the three phases of a round
-// are then bound by shared-memory latency (~0.3 us per round) instead of L2 round trips (~4 us).
+// are then bound by shared-memory latency instead of L2 round trips.
 __global__ void __launch_bounds__(1024) jacobi_eig_smem_kernel(double* Ag, double* Vg, double* ev, int n, int max_sweeps) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int ld = n | 1;  // odd row stride (in doubles): a column walk visits 16 distinct bank pairs
@@ -444,7 +444,7 @@ __device__ __forceinline__ double rsqrt_fast(double x) {
 // transforms independently of the others (row r: (v_p, v_q) <- (c v_p - s v_q, s v_p + c v_q) for the pairs of the round),
 // so the eigenvalue kernel (one CTA, A only: half the shared-memory traffic and instructions per round) just logs
 // (p, q, c, s), and a second kernel with one CTA PER ROW of V replays the log on a row of the identity - n SMs instead of
-// one for the eigenvector half of the work, ~50 us for the n = 85 prior of a streaming window.
+// one for the eigenvector half of the work.
 struct JacobiRot {
   int p, q;
   double c, s;

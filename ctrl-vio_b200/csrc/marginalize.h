@@ -104,6 +104,9 @@ int launch_bias_abs_sums(const int2* ij, const double* sq, int n, const double* 
 
 // measured fp64 FMA throughput of the current device (TFLOP/s); < 0 on error
 double measure_fp64_tflops(cudaStream_t s);
+// measured fp64 tensor-core (mma.sync.m8n8k4.f64) throughput with `ctas_per_sm` CTAs of 256 threads per SM (TFLOP/s);
+// optionally the dependent latency of one mma in cycles; < 0 on error
+double measure_fp64_tensor_tflops(cudaStream_t s, int ctas_per_sm = 4, double* dep_latency_cycles = nullptr);
 
 int launch_flags_to_double(LmScalars* scal, cudaStream_t s);
 int launch_rho_pack(const double* rho, const uint8_t* owned, double* buf, int nL, cudaStream_t s);

@@ -108,6 +108,77 @@ double measure_fp64_tflops(cudaStream_t s) {
   return flops / (best * 1e-3) / 1e12;
 }
 
+// fp64 tensor-core micro-benchmark: every warp runs 8 independent mma.sync.m8n8k4.f64 accumulator chains (the fp64
+// tensor path this library uses; wgmma has no fp64 kind).  It is a different pipe from DFMA, so the kernels built on
+// DMMA (K4, K5) are measured against the rate of the instruction they issue, not against the DFMA loop above.  With
+// `lat`, warp 0 of CTA 0 also times a dependent chain of 256 mma.
+__device__ __forceinline__ void dmma(double& d0, double& d1, double a, double b) {
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
+}
+__global__ void __launch_bounds__(256) fp64_tensor_peak_kernel(double* out, int iters, double seed, long long* lat) {
+  double c[8][2];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) { c[i][0] = seed + i; c[i][1] = seed - i; }
+  const double a = 1.0 + 1e-9 * threadIdx.x, b = 1e-3 + 1e-9 * threadIdx.x;
+  for (int i = 0; i < iters; ++i) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) dmma(c[j][0], c[j][1], a, b);
+  }
+  double s = 0.0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) s += c[i][0] + c[i][1];
+  if (lat && blockIdx.x == 0 && threadIdx.x < 32) {
+    double d0 = s, d1 = s + 1;
+    const long long t0 = clock64();
+#pragma unroll 1
+    for (int i = 0; i < 64; ++i) { dmma(d0, d1, a, b); dmma(d0, d1, a, b); dmma(d0, d1, a, b); dmma(d0, d1, a, b); }
+    const long long t1 = clock64();
+    s += d0 + d1;
+    if (threadIdx.x == 0) lat[0] = t1 - t0;
+  }
+  out[blockIdx.x * blockDim.x + threadIdx.x] = s;
+}
+
+double measure_fp64_tensor_tflops(cudaStream_t s, int ctas_per_sm, double* dep_latency_cycles) {
+  int dev = 0, n_sm = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+  const int ctas = n_sm * ctas_per_sm, iters = 1 << 13;
+  double* out = nullptr;
+  long long* lat = nullptr;
+  if (cudaMalloc(&out, size_t(ctas) * 256 * sizeof(double)) != cudaSuccess) return -1.0;
+  if (dep_latency_cycles && cudaMalloc(&lat, sizeof(long long)) != cudaSuccess) {
+    cudaFree(out);
+    return -1.0;
+  }
+  cudaEvent_t e0, e1;
+  cudaEventCreate(&e0);
+  cudaEventCreate(&e1);
+  float best = 1e30f;
+  for (int rep = 0; rep < 5; ++rep) {
+    cudaEventRecord(e0, s);
+    fp64_tensor_peak_kernel<<<ctas, 256, 0, s>>>(out, iters, 1.0 + rep, lat);
+    cudaEventRecord(e1, s);
+    cudaEventSynchronize(e1);
+    float ms = 0;
+    cudaEventElapsedTime(&ms, e0, e1);
+    if (rep > 0 && ms < best) best = ms;
+  }
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  if (lat) {
+    long long l = 0;
+    cudaMemcpy(&l, lat, sizeof(l), cudaMemcpyDeviceToHost);
+    *dep_latency_cycles = double(l) / 256.0;
+    cudaFree(lat);
+  }
+  cudaFree(out);
+  if (cudaGetLastError() != cudaSuccess) return -1.0;
+  // one m8n8k4 = 256 FMAs = 512 flop; 8 per warp-iteration; 8 warps per CTA
+  const double flops = 512.0 * 8.0 * 8.0 * double(iters) * double(ctas);
+  return flops / (best * 1e-3) / 1e12;
+}
+
 
 // ---- sharded mode: packed all-reduce buffer (lower-triangular tiles only: half the bytes of the dense slab) ----
 size_t shard_pack_len(int npad) {

@@ -1,7 +1,7 @@
 // Step-size selection of the Armijo line search that Ceres 1.14 runs inside its trust-region loop
 // when a parameter has bounds (the camera line delay, trajectory_estimator.cpp:314-318):
 // interpolate cost (and directional derivative) samples with a polynomial and minimise it on
-// [x_min, x_max] (Ceres internal/ceres/polynomial.cc; Ceres is not under /root/reference).
+// [x_min, x_max] (Ceres internal/ceres/polynomial.cc; Ceres is not part of the reference repository).
 // Host-only, a few flops per LM step.
 #pragma once
 #include <algorithm>

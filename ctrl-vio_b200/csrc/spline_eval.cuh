@@ -2,7 +2,7 @@
 //
 // What the reference computes per factor with four separate View calls
 // (so3_spline_view.h:136-276,356-426; rd_spline_view.h:63-94;
-// split_spline_view.h:67-214) is reorganised here B200-first:
+// split_spline_view.h:67-214) is reorganised here GPU-first:
 //   * everything that depends only on the knots — d_k = log(R_k^-1 R_k+1),
 //     |d_k|, Jr^-1(d_k) — is computed ONCE per linearisation point into a
 //     "knot-pair table" (KnotPair, 128 B per pair) that the residual kernels stage

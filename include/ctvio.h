@@ -1,5 +1,5 @@
 /*
- * ctvio.h — C-ABI of the B200-native sliding-window continuous-time bundle
+ * ctvio.h — C-ABI of the H100-native sliding-window continuous-time bundle
  * adjustment engine (libctvio_b200.so).
  *
  * This is the drop-in boundary for the ONE hot path of APRIL-ZJU/Ctrl-VIO:
@@ -281,7 +281,7 @@ int ctvio_transfer_stats(ctvio_handle h, int64_t* h2d_bytes, int64_t* d2h_bytes,
 /* ---- measurement support (bench.py roofline) ----
  * Average CUDA-event duration (ms, on the engine stream) of one launch of each stage of an LM step at the
  * current state, over `reps` launches after 3 warm-up launches.  flush_l2 != 0 writes a 256 MiB scratch
- * buffer (> the 126 MB L2) between timed launches.
+ * buffer (> the 50 MB L2) between timed launches.
  *   out_ms[0] visual residual+Jacobian+accumulate kernel (K1)   out_ms[1] IMU kernel (K2)
  *   out_ms[2] bias + prior kernels (K3)                          out_ms[3] reduced system + landmark Schur (K4)
  *   out_ms[4] blocked Cholesky + triangular solves (K5)          out_ms[5] step vectors / back-substitution (K6)
@@ -290,6 +290,9 @@ int ctvio_profile_kernels(ctvio_handle h, int32_t reps, int32_t flush_l2, double
 /* fp64 FMA micro-benchmark (8 independent DFMA chains per thread, all SMs): measured TFLOP/s, the compute
  * roofline denominator of the fp64-bound kernels (MEASURED_PEAKS.json has only HBM and bf16). */
 int ctvio_measure_fp64_tflops(ctvio_handle h, double* tflops);
+/* fp64 tensor-core micro-benchmark (8 independent mma.sync.m8n8k4.f64 chains per warp, all SMs): measured TFLOP/s,
+ * the compute roofline denominator of the kernels built on DMMA (the dense solve K5, the Schur update K4). */
+int ctvio_measure_fp64_tensor_tflops(ctvio_handle h, double* tflops);
 /* Self-check of the dense solver (K5) on the reduced system of the current state: the system is built once, then
  * factored + solved `reps` times from the same input.  mismatches = number of repetitions whose solution differs
  * BITWISE from the first one (must be 0: the sharded mode relies on a reproducible replicated solve);

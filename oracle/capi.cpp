@@ -377,6 +377,10 @@ int ctvo_measure_fp64_tflops(void*, double* v) {
   *v = 0.0;
   return CTVIO_OK;
 }
+int ctvo_measure_fp64_tensor_tflops(void*, double* v) {
+  *v = 0.0;
+  return CTVIO_OK;
+}
 int ctvo_profile_kernels(void*, int32_t, int32_t, double* out) {
   for (int k = 0; k < 8; ++k) out[k] = 0.0;  // not meaningful for the CPU oracle
   return CTVIO_OK;

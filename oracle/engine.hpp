@@ -10,7 +10,7 @@
 //   factor/analytic_diff/marginalization_factor.cpp:85-265  marginalize()
 //   spline/se3_spline.h:463-503                  CaculateSplineMeta (padded knot windows)
 //   estimator/trajectory_manager.cpp:485-516     double2vector (4-DoF gauge re-alignment)
-//   Ceres-Solver 1.14 (NOT under /root/reference; pinned only by README.md:15):
+//   Ceres-Solver 1.14 (NOT part of the reference repository; pinned only by README.md:15):
 //     trust_region_minimizer.cc, levenberg_marquardt_strategy.cc, line_search.cc,
 //     polynomial.cc, corrector.cc, loss_function.cc, parameter_block.h  — restated
 //     from the published algorithm (SURVEY.md Appendix B).

@@ -7,7 +7,7 @@
 //   factor/analytic_diff/trajectory_value_factor.h:45-99    BiasFactor::Evaluate
 //   factor/analytic_diff/marginalization_factor.cpp:326-373 MarginalizationFactor::Evaluate
 //   marginalization_factor.cpp:39-67 + Ceres 1.14 corrector.cc / loss_function.cc
-//        (CauchyLoss + Corrector; Ceres itself is not under /root/reference)
+//        (CauchyLoss + Corrector; Ceres itself is not part of the reference repository)
 // Jacobians are returned per GLOBAL knot (start index + 4 blocks per side)
 // instead of the reference's padded parameter-block list; the unused padded
 // blocks are identically zero there (image_feature_factor.h:165-180).

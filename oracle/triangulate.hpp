@@ -1,8 +1,8 @@
 // ORACLE (test infrastructure, NOT product code).  Parity pinned for this file: tests/test_frontend_cpu.py checks it
 // against numpy.linalg.svd (LAPACK) on the same inputs.
 // Restates FeatureManager::triangulate(Rs, Ps, ric, tic) (visual_odometry/feature_manager.cpp:230-275; the
-// identity-extrinsic overload :173-223 is ric = I, tic = 0).  The reference's Eigen::JacobiSVD is not under
-// /root/reference (Eigen 3.3 is an external dependency, README.md:15-20); the smallest right singular vector is unique
+// identity-extrinsic overload :173-223 is ric = I, tic = 0).  The reference's Eigen::JacobiSVD is not part of
+// the reference repository (Eigen 3.3 is an external dependency, README.md:15-20); the smallest right singular vector is unique
 // up to sign and V(2)/V(3) is sign free, so any backward-stable SVD restates it: here a one-sided Jacobi (Hestenes)
 // sweep on the full 2m x 4 matrix.
 #pragma once

@@ -14,7 +14,7 @@ pkg = importlib.import_module("ctrl-vio_b200")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a)")
 
 
 @pytest.fixture(scope="session")

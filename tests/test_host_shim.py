@@ -1,7 +1,7 @@
 """The C++ host mirror of ctrlvio::TrajectoryEstimator (ctrl-vio_b200/host/trajectory_estimator.hpp):
 compiles against include/ctvio.h with plain g++ (no Eigen / Ceres / ROS), links the C-ABI library, and
  - without a GPU: fails loudly with CTVIO_ERR_NO_DEVICE (no CPU fallback),
- - on a B200 : reproduces the oracle's solve through the reference-shaped call sequence."""
+ - on an H100: reproduces the oracle's solve through the reference-shaped call sequence."""
 import os
 import subprocess
 

@@ -1,5 +1,5 @@
-import importlib, sys, numpy as np
-sys.path.insert(0, "/root/repo")
+import importlib, os, sys, numpy as np
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 pkg = importlib.import_module("ctrl-vio_b200"); st = importlib.import_module("ctrl-vio_b200.streaming")
 lib = pkg.load()
 seq = st.quantize_wire(st.config_c5_sequence(4))
