@@ -103,7 +103,7 @@ ABI_SYMBOLS = [
     "query_trajectory", "triangulate",
     "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior", "ingest_feature_cloud", "add_image_features_from_slots",
     "ingest_imu", "add_imu_from_table", "transfer_stats", "profile_kernels", "measure_fp64_tflops", "measure_fp64_tensor_tflops",
-    "selfcheck_solver", "nccl_unique_id", "comm_init",
+    "selfcheck_solver", "nccl_unique_id", "comm_init", "triangulate_window",
 ]
 
 
@@ -111,7 +111,7 @@ ABI_SYMBOLS = [
 # the device-residency / wire-format calls, which have no CPU meaning
 DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enable_prior", "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior",
                        "ingest_feature_cloud", "add_image_features_from_slots", "ingest_imu", "add_imu_from_table",
-                       "transfer_stats", "residual_summary")
+                       "transfer_stats", "residual_summary", "triangulate_window")
 
 
 def _addr(a):
@@ -425,6 +425,16 @@ class Estimator:
         n = a[0].shape[0]
         self.lib.call("add_image_features_from_slots", self.h, C.c_int32(n), *[_ip(x) for x in a], _ip(marg))
         self.n_img += n
+
+    def TriangulateWindow(self, obs_offset, obs_slot, obs_idx, init_depth=5.0):
+        """FeatureManager::triangulate of the resident window (feature_manager.cpp:226-338): DLT of every landmark whose
+        inverse depth is <= 0 from its observations (frame slot, feature index; the first one the anchor), camera poses
+        from the resident spline at each observation's row time.  Returns (n_triangulated, n_fallback)."""
+        obs_offset = _i32(obs_offset); obs_slot = _i32(obs_slot); obs_idx = _i32(obs_idx)
+        nt, nf = C.c_int32(), C.c_int32()
+        self.lib.call("triangulate_window", self.h, C.c_int32(max(obs_offset.shape[0] - 1, 0)), _ip(obs_offset), _ip(obs_slot),
+                      _ip(obs_idx), C.c_double(init_depth), C.byref(nt), C.byref(nf))
+        return nt.value, nf.value
 
     def IngestImu(self, records: np.ndarray, off_gyro, off_accel, drop_before_ns=0):
         """packed IMUData records (structured / byte array, one record per row)."""

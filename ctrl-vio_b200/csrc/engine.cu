@@ -240,7 +240,8 @@ struct ctvio_engine {
   size_t h2d_bytes = 0, d2h_bytes = 0;     // bytes moved by the C-ABI calls since ctvio_transfer_stats(reset)
 
   DevBuf<double> d_tmp;  // scratch (gauge inputs, probe outputs)
-  DevBuf<int32_t> d_tri_idx;  // ctvio_triangulate: start frames | observation offsets
+  DevBuf<int32_t> d_tri_idx;  // index uploads: ctvio_triangulate, ctvio_remap_landmarks, ctvio_triangulate_window
+  DevBuf<int32_t> d_tri_cnt;  // ctvio_triangulate_window: {triangulated, fallback}
   // marginalization workspace (K7), kept across windows: allocation / free costs more than the kernels
   struct MargWs {
     DevBuf<int32_t> pos_cam, pos_lm, prior_pos, marg_img, marg_imu;
@@ -2450,6 +2451,67 @@ int ctvio_remap_landmarks(ctvio_handle e, int32_t n_new, const int32_t* old_inde
   e->mirror_valid = false;
   e->nL = n_new;
   e->have_rho = true;
+  return CTVIO_OK;
+}
+
+int ctvio_triangulate_window(ctvio_handle e, int32_t nl, const int32_t* obs_offset, const int32_t* obs_slot, const int32_t* obs_idx,
+                             double init_depth, int32_t* n_triangulated, int32_t* n_fallback) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
+  if (!e->x[e->cur].ld.p) return fail(CTVIO_ERR_STATE, "the line delay has not been set");
+  if (nl != e->nL) return fail(CTVIO_ERR_INVALID, "n_landmarks differs from the engine's landmark count");
+  if (!(init_depth > 0.0) || !std::isfinite(init_depth)) return fail(CTVIO_ERR_INVALID, "init_depth must be positive");
+  if (nl > 0 && !obs_offset) return fail(CTVIO_ERR_INVALID, "null obs_offset");
+  if (nl > 0 && obs_offset[0] != 0) return fail(CTVIO_ERR_INVALID, "obs_offset[0] must be 0");
+  for (int l = 0; l < nl; ++l)
+    if (obs_offset[l + 1] < obs_offset[l]) return fail(CTVIO_ERR_INVALID, "obs_offset must be non-decreasing");
+  const int total = nl > 0 ? obs_offset[nl] : 0;
+  if (total > 0 && (!obs_slot || !obs_idx)) return fail(CTVIO_ERR_INVALID, "null observation array");
+  for (int k = 0; k < total; ++k) {
+    const int s = obs_slot[k];
+    if (s < 0 || s >= ctvio_engine::kFrameSlots || obs_idx[k] < 0 || obs_idx[k] >= e->h_frame_n[s])
+      return fail(CTVIO_ERR_INVALID, "feature slot / index out of range");
+  }
+  if (n_triangulated) *n_triangulated = 0;
+  if (n_fallback) *n_fallback = 0;
+  if (nl == 0) return CTVIO_OK;
+  cudaSetDevice(e->cfg.device);
+  ArenaScope arena(e);
+  cudaStream_t st = e->stream;
+  ensure_table(e);
+  const int other = e->cur ^ 1;
+  CUDA_OK(e->x[other].rho.reserve(size_t(nl) + 1));
+  CUDA_OK(e->d_tri_idx.reserve(size_t(nl) + 1 + 2 * size_t(total)));
+  CUDA_OK(e->d_tri_cnt.reserve(2));
+  int32_t* d_off = e->d_tri_idx.p;
+  int32_t* d_slot = d_off + nl + 1;
+  int32_t* d_idx = d_slot + total;
+  // only the three index arrays go up: bearings, rows, frame times, knots and the line delay are resident
+  CUDA_OK(staged_h2d(d_off, obs_offset, (size_t(nl) + 1) * sizeof(int32_t), st));
+  CUDA_OK(staged_h2d(d_slot, obs_slot, size_t(total) * sizeof(int32_t), st));
+  CUDA_OK(staged_h2d(d_idx, obs_idx, size_t(total) * sizeof(int32_t), st));
+  e->h2d_bytes += (size_t(nl) + 1 + 2 * size_t(total)) * sizeof(int32_t);
+  CUDA_OK(cudaMemsetAsync(e->d_tri_cnt.p, 0, 2 * sizeof(int32_t), st));
+  ctvio::TriangulateWindowArgs a;
+  a.n_landmarks = nl; a.obs_offset = d_off; a.obs_slot = d_slot; a.obs_idx = d_idx;
+  a.table = e->d_frames.p; a.frame_t = e->d_frame_t.p; a.frame_cap = ctvio_engine::kFrameCap;
+  a.st = e->x[e->cur].ptrs(); a.sp = e->sp; a.R_CI = e->rig.R_CI; a.p_CI = e->rig.p_CI;
+  a.init_depth = init_depth;
+  // written into the other state buffer's array and swapped in only on success: after CTVIO_ERR_TIME_RANGE the
+  // resident inverse depths are the ones before the call
+  a.rho_in = e->x[e->cur].rho.p; a.rho_out = e->x[other].rho.p;
+  a.counts = e->d_tri_cnt.p;
+  e->launches += ctvio::launch_triangulate_window(a, st);
+  int32_t cnt[2];
+  CUDA_OK(cudaMemcpyAsync(cnt, e->d_tri_cnt.p, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+  e->d2h_bytes += sizeof(cnt);
+  CUDA_OK(cudaStreamSynchronize(st));
+  if (cnt[0] < 0) return fail(CTVIO_ERR_TIME_RANGE, "an observation's row time falls outside the spline");
+  std::swap(e->x[e->cur].rho.p, e->x[other].rho.p);
+  std::swap(e->x[e->cur].rho.cap, e->x[other].rho.cap);
+  e->mirror_valid = false;
+  if (n_triangulated) *n_triangulated = cnt[0];
+  if (n_fallback) *n_fallback = cnt[1];
   return CTVIO_OK;
 }
 

@@ -3,6 +3,9 @@
 //   triangulate_kernel   replaces FeatureManager::triangulate (visual_odometry/feature_manager.cpp:173-223 and the
 //                        camera-extrinsic overload :230-275): per-landmark DLT, depth = V(2)/V(3) of the right singular
 //                        vector of the smallest singular value of the 2m x 4 system, INIT_DEPTH fallback below 0.1.
+//   triangulate_window_kernel  the same DLT for the landmarks of the resident window (AddImageToWindow,
+//                        visual_odometry.cpp:185-191), camera poses from the resident spline at each observation's row
+//                        time (the rolling-shutter variant triangulateRS, feature_manager.cpp:276-338, when ld > 0).
 //   unpack_cloud_kernel  replaces FeatureMsg2Image (visual_odometry/visual_struct.h:98-121) on the tracker's message
 //                        (visual_feature/feature_tracker_node.cpp:146-184): sensor_msgs::PointCloud arrives as packed
 //                        float32 triples + five float32 channels and is converted ON THE DEVICE into the resident
@@ -11,95 +14,16 @@
 //   gather_factors_kernel builds the sorted SoA image-factor arrays of K1 from the resident tables and an 8-byte
 //                        (slot_i, slot_j) descriptor per factor: the payload never passes through host marshalling.
 //
-// The reference runs Eigen::JacobiSVD on the tall matrix (QR preconditioner + two-sided Jacobi on R).  Here one thread
-// per landmark streams the rows through a Givens QR (R stays in registers, any number of frames) and then runs a
-// one-sided Jacobi SVD on the 4x4 R: same conditioning as the reference (no A'A squaring), no local-memory arrays.
+// The DLT itself (streaming Givens QR + 4x4 one-sided Jacobi SVD, one thread per landmark) is in dlt.cuh.
 #include "frontend.h"
 
 #include <algorithm>
 
+#include "dlt.cuh"
+
 namespace ctvio {
 
 namespace {
-
-struct R4 {
-  double r[4][4];  // upper triangular
-};
-
-// fold one row a[4] into R with 4 Givens rotations
-__device__ __forceinline__ void qr_push_row(R4& R, double a0, double a1, double a2, double a3) {
-  double a[4] = {a0, a1, a2, a3};
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    const double x = R.r[c][c], y = a[c];
-    if (y == 0.0) continue;
-    const double h = hypot(x, y);
-    const double cs = x / h, sn = y / h;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (k < c) continue;
-      const double rk = R.r[c][k], ak = a[k];
-      R.r[c][k] = cs * rk + sn * ak;
-      a[k] = -sn * rk + cs * ak;
-    }
-  }
-}
-
-// right singular vector of the smallest singular value of the upper triangular R (one-sided Jacobi, Hestenes)
-__device__ __forceinline__ void smallest_right_singular_vector(const R4& R, double v_out[4]) {
-  double G[4][4], V[4][4];  // column-major use: G[row][col]
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      G[i][j] = j >= i ? R.r[i][j] : 0.0;
-      V[i][j] = i == j ? 1.0 : 0.0;
-    }
-  for (int sweep = 0; sweep < 40; ++sweep) {
-    bool rotated = false;
-#pragma unroll
-    for (int p = 0; p < 3; ++p)
-#pragma unroll
-      for (int q = p + 1; q < 4; ++q) {
-        double al = 0, be = 0, ga = 0;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          al = fma(G[i][p], G[i][p], al);
-          be = fma(G[i][q], G[i][q], be);
-          ga = fma(G[i][p], G[i][q], ga);
-        }
-        if (ga == 0.0 || fabs(ga) <= 1e-300 || fabs(ga) <= 2.3e-16 * sqrt(al * be)) continue;
-        rotated = true;
-        const double zeta = (be - al) / (2.0 * ga);
-        const double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
-        const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const double gp = G[i][p], gq = G[i][q];
-          G[i][p] = c * gp - s * gq;
-          G[i][q] = s * gp + c * gq;
-          const double vp = V[i][p], vq = V[i][q];
-          V[i][p] = c * vp - s * vq;
-          V[i][q] = s * vp + c * vq;
-        }
-      }
-    if (!rotated) break;
-  }
-  int best = 0;
-  double best_n = 1e300;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    double nj = 0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) nj = fma(G[i][j], G[i][j], nj);
-    if (nj < best_n) { best_n = nj; best = j; }
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    // select without dynamic register indexing
-    v_out[i] = best == 0 ? V[i][0] : best == 1 ? V[i][1] : best == 2 ? V[i][2] : V[i][3];
-  }
-}
 
 __global__ void triangulate_kernel(TriangulateArgs a) {
   const int l = blockIdx.x * blockDim.x + threadIdx.x;
@@ -130,21 +54,8 @@ __global__ void triangulate_kernel(TriangulateArgs a) {
     M3 R1;
     V3 t1;
     cam_pose(start + k, R1, t1);
-    const V3 t = m3_tvec(R0, t1 - t0);
-    const M3 R = m3_mul(m3_transpose(R0), R1);
-    // P = [R' | -R' t]   (:255-257)
-    const M3 Rt = m3_transpose(R);
-    const V3 pt = neg(m3_vec(Rt, t));
-    V3 f{a.obs_point[3 * (o0 + k)], a.obs_point[3 * (o0 + k) + 1], a.obs_point[3 * (o0 + k) + 2]};
-    const double fn = sqrt(f.x * f.x + f.y * f.y + f.z * f.z);
-    f = (1.0 / fn) * f;
-    const double P0[4] = {Rt.m[0], Rt.m[1], Rt.m[2], pt.x};
-    const double P1[4] = {Rt.m[3], Rt.m[4], Rt.m[5], pt.y};
-    const double P2[4] = {Rt.m[6], Rt.m[7], Rt.m[8], pt.z};
-    qr_push_row(Rq, f.x * P2[0] - f.z * P0[0], f.x * P2[1] - f.z * P0[1], f.x * P2[2] - f.z * P0[2],
-                f.x * P2[3] - f.z * P0[3]);
-    qr_push_row(Rq, f.y * P2[0] - f.z * P1[0], f.y * P2[1] - f.z * P1[1], f.y * P2[2] - f.z * P1[2],
-                f.y * P2[3] - f.z * P1[3]);
+    const V3 f{a.obs_point[3 * (o0 + k)], a.obs_point[3 * (o0 + k) + 1], a.obs_point[3 * (o0 + k) + 2]};
+    dlt_push_observation(Rq, R0, t0, R1, t1, f);
   }
   double v[4];
   smallest_right_singular_vector(Rq, v);
@@ -152,6 +63,101 @@ __global__ void triangulate_kernel(TriangulateArgs a) {
   if (!(d >= 0.1)) d = a.init_depth;  // :268-271 (NaN / inf from v[3] == 0 also fall back)
   if (!isfinite(d)) d = a.init_depth;
   a.depth[l] = d;
+}
+
+// ---- DLT of the resident window (triangulate at the row time, feature_manager.cpp:226-274 / :276-338) ----------------
+// One CTA per kTriLmPerCta consecutive landmarks.  Their observations are processed in chunks of kTriObsChunk: every
+// thread evaluates observation poses (the ~11 spline evaluations per landmark are the bulk of the work) into shared
+// memory, then the thread of each landmark folds the rows of its observations in that chunk into its R (registers,
+// kept across chunks, so a landmark may have any number of observations).  Rows enter in observation order, the SVD
+// runs once per landmark: no atomics on the result, bitwise reproducible.
+constexpr int kTriThreads = 128;
+constexpr int kTriLmPerCta = 32;
+constexpr int kTriObsChunk = 256;
+constexpr int kTriPoseWords = 14;  // camera R (9) | camera t (3) | bearing x, y
+
+__global__ void __launch_bounds__(kTriThreads) triangulate_window_kernel(TriangulateWindowArgs a) {
+  __shared__ double s_pose[kTriObsChunk][kTriPoseWords];
+  __shared__ int32_t s_off[kTriLmPerCta + 1];
+  __shared__ uint8_t s_todo[kTriLmPerCta];
+  const int tid = threadIdx.x;
+  const int l0 = blockIdx.x * kTriLmPerCta;
+  const int nl = min(kTriLmPerCta, a.n_landmarks - l0);
+  const int l = l0 + tid;
+  const bool owner = tid < nl;
+  const double rho_old = owner ? a.rho_in[l] : 0.0;
+  // feature_manager.cpp:239-240: an initialised depth (> 0) is kept; NaN is not > 0 and is re-triangulated
+  const bool want = owner && !(rho_old > 0.0);
+  if (tid <= nl) s_off[tid] = a.obs_offset[l0 + tid];
+  if (owner) s_todo[tid] = want && a.obs_offset[l + 1] - a.obs_offset[l] >= 2;
+  __syncthreads();
+  const int o_begin = s_off[0], o_end = s_off[nl];
+  const int lo = owner ? s_off[tid] : 0, hi = owner ? s_off[tid + 1] : 0;
+  const bool dlt = owner && s_todo[tid];
+  const int64_t ld_ns = int64_t(*a.st.ld * 1e9);  // image_feature_factor.h:72 (truncation), as K1
+  bool out_of_range = false;
+  R4 Rq = {};
+  M3 R0{};
+  V3 t0{0.0, 0.0, 0.0};
+  for (int c0 = o_begin; c0 < o_end; c0 += kTriObsChunk) {
+    const int c1 = min(c0 + kTriObsChunk, o_end);
+    for (int k = c0 + tid; k < c1; k += kTriThreads) {
+      const int slot = a.obs_slot[k];
+      const FrameFeature f = a.table[size_t(slot) * a.frame_cap + a.obs_idx[k]];
+      int32_t s;
+      double u;
+      // every observation's time is checked; poses are evaluated only for the landmarks that are triangulated
+      if (!spline_index(a.sp, a.frame_t[slot] + int64_t(f.row) * ld_ns, s, u)) { out_of_range = true; continue; }
+      int j = 0;  // landmark of observation k: last j with s_off[j] <= k
+      for (int step = kTriLmPerCta / 2; step > 0; step >>= 1)
+        if (j + step < nl && s_off[j + step] <= k) j += step;
+      if (!s_todo[j]) continue;
+      SideEval ev;
+      eval_side<false, kPStride>(a.sp, a.st.q, a.st.p, a.st.tab, s, u, ev);
+      const M3 Rc = m3_mul(ev.R, a.R_CI);        // R_c = R * R_CI         (:246)
+      const V3 tc = ev.p + m3_vec(ev.R, a.p_CI);  // t_c = p + R * p_CI     (:245)
+      double* w = s_pose[k - c0];
+#pragma unroll
+      for (int e = 0; e < 9; ++e) w[e] = Rc.m[e];
+      w[9] = tc.x; w[10] = tc.y; w[11] = tc.z;
+      w[12] = f.x; w[13] = f.y;
+    }
+    __syncthreads();
+    if (dlt) {
+      const int k1 = min(hi, c1);
+      for (int k = max(lo, c0); k < k1; ++k) {
+        const double* w = s_pose[k - c0];
+        M3 R1;
+#pragma unroll
+        for (int e = 0; e < 9; ++e) R1.m[e] = w[e];
+        const V3 t1{w[9], w[10], w[11]};
+        if (k == lo) { R0 = R1; t0 = t1; }  // the anchor
+        dlt_push_observation(Rq, R0, t0, R1, t1, V3{w[12], w[13], 1.0});
+      }
+    }
+    __syncthreads();
+  }
+  bool triangulated = false;
+  if (want) {
+    double d = a.init_depth;  // fewer than 2 observations: INIT_DEPTH
+    if (dlt) {
+      double v[4];
+      smallest_right_singular_vector(Rq, v);
+      const double dd = v[2] / v[3];
+      if (dd >= 0.1 && isfinite(dd)) { d = dd; triangulated = true; }  // :266-271 (NaN / inf fall back as well)
+    }
+    a.rho_out[l] = 1.0 / d;
+  } else if (owner) {
+    a.rho_out[l] = rho_old;
+  }
+  const int n_tri = __syncthreads_count(triangulated);
+  const int n_fb = __syncthreads_count(want && !triangulated);
+  const int bad = __syncthreads_or(out_of_range);
+  if (tid == 0) {
+    if (n_tri) atomicAdd(&a.counts[0], n_tri);
+    if (n_fb) atomicAdd(&a.counts[1], n_fb);
+    if (bad) atomicOr(&a.counts[0], int(0x80000000u));
+  }
 }
 
 // ---- wire formats -> resident tables ----------------------------------------------------------------
@@ -285,6 +291,11 @@ __global__ void prior_x0_kernel(StatePtrs st, const int32_t* type, const int32_t
 int launch_triangulate(const TriangulateArgs& a, cudaStream_t s) {
   if (a.n_landmarks <= 0) return 0;
   triangulate_kernel<<<(a.n_landmarks + 127) / 128, 128, 0, s>>>(a);
+  return 1;
+}
+int launch_triangulate_window(const TriangulateWindowArgs& a, cudaStream_t s) {
+  if (a.n_landmarks <= 0) return 0;
+  triangulate_window_kernel<<<(a.n_landmarks + kTriLmPerCta - 1) / kTriLmPerCta, kTriThreads, 0, s>>>(a);
   return 1;
 }
 int launch_unpack_cloud(const UnpackCloudArgs& a, cudaStream_t s) {

@@ -1,5 +1,6 @@
-// Front-end data formats either side of the hot path (frontend.cu): DLT triangulation, wire-format unpacking,
-// device-side construction of the sorted image-factor arrays from the resident per-frame feature tables.
+// Front-end data formats either side of the hot path (frontend.cu): DLT triangulation (from caller poses, and of the
+// resident window from the resident spline), wire-format unpacking, device-side construction of the sorted image-factor
+// arrays from the resident per-frame feature tables.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -69,6 +70,29 @@ struct GatherFactorsArgs {
   int4* meta;
 };
 int launch_gather_factors(const GatherFactorsArgs& a, cudaStream_t s);
+
+// DLT of the resident window's landmarks: observation k of landmark l (obs_offset[l] <= k < obs_offset[l+1], the first
+// one the anchor) is feature obs_idx[k] of frame slot obs_slot[k]; its camera pose is the resident spline at the row
+// time frame_t[slot] + row * int64(ld * 1e9) composed with the extrinsic.  Only landmarks with rho_in <= 0 get a new
+// value; rho_out receives every landmark (kept ones bitwise).
+struct TriangulateWindowArgs {
+  int32_t n_landmarks;
+  const int32_t* obs_offset;  // [n_landmarks + 1], obs_offset[0] == 0
+  const int32_t* obs_slot;    // [total]
+  const int32_t* obs_idx;     // [total]
+  const FrameFeature* table;  // [n_slots][frame_cap]
+  const int64_t* frame_t;     // [n_slots]
+  int32_t frame_cap;
+  StatePtrs st;               // knots, knot-pair table (valid), line delay
+  SplineParams sp;
+  M3 R_CI;                    // camera -> IMU rotation
+  V3 p_CI;
+  double init_depth;          // INIT_DEPTH
+  const double* rho_in;       // [n_landmarks]
+  double* rho_out;            // [n_landmarks] (must not alias rho_in)
+  int32_t* counts;            // [2] zeroed by the caller: {triangulated, fallback}; sign bit of [0] = a time left the spline
+};
+int launch_triangulate_window(const TriangulateWindowArgs& a, cudaStream_t s);
 
 // device-resident window bookkeeping (all on the device)
 int launch_extend_knots(const StatePtrs& st, int old_n, int new_n, cudaStream_t s);

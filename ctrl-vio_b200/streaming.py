@@ -356,11 +356,21 @@ class ResidentRunner(StreamingRunner):
     """The same per-image cycle with the window living in HBM: the new image's PointCloud and the new IMUData records go
     up as they are, control points are extended / dropped on the device, inverse depths are re-indexed on the device,
     the prior is handed over device-to-device, and the factor payload is gathered from the resident tables (only index
-    tables cross the boundary).  MARGIN_OLD only (every frame a keyframe, the C5 configuration)."""
+    tables cross the boundary).  MARGIN_OLD only (every frame a keyframe, the C5 configuration).
 
-    def __init__(self, lib, seq, **kw):
+    triangulate=True: new landmarks enter with inverse depth -1 and get their initial depth from TriangulateWindow (the
+    reference's FeatureManager::triangulate in AddImageToWindow, visual_odometry.cpp:185-191) on the device, after the
+    predictor solve, from the resident spline at each observation's row time.  The reference takes the newest frame's
+    pose from its own IMU propagation (RI_, PI_, :189-190); here it is the predictor-solved spline, which carries the same
+    IMU information.  Default (False): new landmarks take the sequence's initial guess rho0, as before.
+    triangulate_probe (tests): called as probe(runner, obs_offset, obs_slot, obs_idx, rho_before) right after
+    TriangulateWindow, on the engine state the call used."""
+
+    def __init__(self, lib, seq, triangulate=False, **kw):
         assert not kw.get("second_new_every"), "the resident runner implements the MARGIN_OLD slide only"
         super().__init__(lib, seq, **kw)
+        self.triangulate = triangulate
+        self.triangulate_probe = None
         self.clouds = FrameClouds(seq)
         self.n_slots = 16
         self.imu_sent = 0          # samples of the source sequence already ingested
@@ -422,7 +432,8 @@ class ResidentRunner(StreamingRunner):
             pos = np.searchsorted(self.prev_lm_global, lm_global)
             pos = np.clip(pos, 0, len(self.prev_lm_global) - 1)
             old_index = np.where(self.prev_lm_global[pos] == lm_global, pos, -1).astype(np.int32)
-        init_rho = s.rho0[lm_global]
+        # new landmarks (old_index < 0): the sequence's initial guess, or -1 (not initialised) when triangulated below
+        init_rho = np.full(len(lm_global), -1.0) if self.triangulate else s.rho0[lm_global]
         img_marg = (w.anchor_frame[w.lm] == 0).astype(np.int32)  # (inverse depths are positive in the synthetic sequences)
         bias_marg = np.zeros(len(w.bf_i), np.int32); bias_marg[0] = 1
         # factor -> (frame slot, index in that frame's cloud) of its two observations
@@ -432,6 +443,8 @@ class ResidentRunner(StreamingRunner):
         idx_i = self.clouds.anchor_idx[g_lm]
         slot_j = (frames[w.obs_frame] % self.n_slots).astype(np.int32)
         idx_j = self.clouds.obs_idx[sel]
+        if self.triangulate:
+            tri_csr = self._observation_csr(frames, w, lm_global, slot_j, idx_j)
         R0 = t0_ = None
         if self.readback is not None:
             qn, pn = self.readback[0][ks - self.prev_ks], self.readback[1][ks - self.prev_ks]
@@ -451,6 +464,14 @@ class ResidentRunner(StreamingRunner):
             n_init = e.AddImuFromTable(max_bef_ns, max_t, fixed_node=len(frames) - 1)
             if n_init > 0:
                 init_summary = e.Solve(self.init_iters)
+        n_tri = n_fb = None
+        if self.triangulate:
+            # FeatureManager::triangulate on the predictor-solved spline (window 0: the initializer's), before the
+            # image factors that read the depths
+            rho_before = e.GetInvDepths() if self.triangulate_probe is not None else None
+            n_tri, n_fb = e.TriangulateWindow(*tri_csr)
+            if self.triangulate_probe is not None:
+                self.triangulate_probe(self, *tri_csr, rho_before)
         e.SetOptions(self._make_options(fix_ld=False, ld_lower=0.0, ld_upper=syn.LD_UPPER, is_marg_state=True,
                                         ctrl_to_be_opt_now=nowk, ctrl_to_be_opt_later=later))
         e.ClearFactors()
@@ -488,9 +509,28 @@ class ResidentRunner(StreamingRunner):
                    init_iterations=None if init_summary is None else init_summary.iterations, init_n_imu=0,
                    init_device_ms=0.0 if init_summary is None else init_summary.device_ms, prior_dim=n_out.value,
                    h2d_bytes=h2d, d2h_bytes=d2h)
+        if self.triangulate:
+            rec.update(n_triangulated=n_tri, n_fallback=n_fb, n_new_lm=int(np.sum(old_index < 0)))
         self.records.append(rec)
         self.step_index += 1
         return rec
+
+    def _observation_csr(self, frames, w, lm_global, slot_j, idx_j):
+        """(obs_offset, obs_slot, obs_idx) of TriangulateWindow: per window landmark its anchor, then its observations
+        in frame order (the factors are landmark-major and frame-ordered within a landmark)."""
+        assert np.all(np.diff(w.lm) >= 0)
+        n_lm = len(lm_global)
+        counts = np.bincount(w.lm, minlength=n_lm)
+        obs_offset = np.concatenate([[0], np.cumsum(counts + 1)]).astype(np.int32)
+        first_factor = np.cumsum(counts) - counts
+        obs_slot = np.empty(obs_offset[-1], np.int32)
+        obs_idx = np.empty(obs_offset[-1], np.int32)
+        obs_slot[obs_offset[:-1]] = frames[w.anchor_frame] % self.n_slots
+        obs_idx[obs_offset[:-1]] = self.clouds.anchor_idx[lm_global]
+        pos = obs_offset[w.lm] + 1 + np.arange(len(w.lm)) - first_factor[w.lm]
+        obs_slot[pos] = slot_j
+        obs_idx[pos] = idx_j
+        return obs_offset, obs_slot, obs_idx
 
     def _factor_selection(self, frames, lm_global):
         """indices (into the source sequence's observation arrays) of the window's factors, in subwindow_frames order"""

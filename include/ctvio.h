@@ -245,6 +245,29 @@ int ctvio_slide_window(ctvio_handle h, int32_t n_drop_knots, int32_t n_drop_bias
 /* replaces FeatureManager::getDepthVector / setDepth re-indexing (visual_odometry/feature_manager.cpp:139-170): landmark l
  * of the new window takes the inverse depth of old landmark old_index[l] (>= 0), else init_inv_depth[l]. */
 int ctvio_remap_landmarks(ctvio_handle h, int32_t n_landmarks, const int32_t* old_index, const double* init_inv_depth);
+/* replaces FeatureManager::triangulate(Rs, Ps, ric, tic) as VisualOdometry::AddImageToWindow calls it for every new image
+ * (visual_odometry.cpp:185-191, feature_manager.cpp:226-274), with the camera poses taken from the RESIDENT spline and the
+ * bearings / rows from the resident frame table: only index arrays go up, only the two counts come back.
+ *   Landmark l is numbered as ctvio_remap_landmarks / ctvio_set_inv_depths number it; n_landmarks must equal the engine's
+ *   landmark count.  Its observations are k = obs_offset[l] .. obs_offset[l+1]-1 (obs_offset[0] == 0, non-decreasing):
+ *   feature obs_idx[k] of resident frame slot obs_slot[k]; the first one is the anchor.
+ *   Camera pose of an observation: the spline at frame_t[slot] + row * floor(ld * 1e9) (the current line delay, truncated
+ *   to int64 like the image factor), composed with the configured extrinsic: R_c = R * R(q_CtoI), t_c = p + R * p_CinI.
+ *   With ld == 0 this is the reference's triangulate at the frame poses; with ld > 0 it is its rolling-shutter variant
+ *   triangulateRS (feature_manager.cpp:276-338, compiled out there) with the factor's row time and the configured
+ *   extrinsic.  There is no mode flag: the line delay of the state decides.
+ *   Only landmarks whose resident inverse depth is <= 0 (or NaN) are written (estimated_depth > 0 -> continue, :239-240);
+ *   all others stay bitwise untouched.  Fewer than 2 observations -> 1 / init_depth; otherwise the DLT depth V(2)/V(3)
+ *   of the smallest right singular vector, replaced by init_depth (INIT_DEPTH, parameters.cpp:44) when below 0.1 or not
+ *   finite; written as an inverse depth.
+ *   n_triangulated (may be NULL): landmarks written from a DLT depth; n_fallback (may be NULL): landmarks given init_depth.
+ *   Errors: CTVIO_ERR_INVALID for a landmark-count mismatch, a bad obs_offset, a slot outside 0..15, an index >= the
+ *   feature count ingested in that slot or init_depth <= 0; CTVIO_ERR_STATE before the knots / line delay are set;
+ *   CTVIO_ERR_TIME_RANGE when an observation's time falls outside the spline - the resident inverse depths are then
+ *   unchanged.  One kernel launch (plus the knot-pair table when stale), one stream synchronisation; bitwise
+ *   reproducible (no atomics on the depths). */
+int ctvio_triangulate_window(ctvio_handle h, int32_t n_landmarks, const int32_t* obs_offset, const int32_t* obs_slot,
+                             const int32_t* obs_idx, double init_depth, int32_t* n_triangulated, int32_t* n_fallback);
 /* The reference builds a fresh TrajectoryEstimator without the prior for InitTrajectory (trajectory_manager.cpp:297);
  * here the resident prior is switched off / on instead of being cleared and re-uploaded. */
 int ctvio_enable_prior(ctvio_handle h, int32_t on);
