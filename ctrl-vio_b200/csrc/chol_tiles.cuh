@@ -59,28 +59,6 @@ __device__ __forceinline__ double rsqrt_pos(double x) {
   return fma(p, ye, y);
 }
 
-// 4x4 lower Cholesky of a (registers), reciprocal pivots rd.  Returns false on a bad pivot.
-__device__ __forceinline__ bool chol4(const double a[4][4], double l[4][4], double rd[4]) {
-  bool ok = true;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    double v = a[j][j];
-#pragma unroll
-    for (int k = 0; k < j; ++k) v = fma(-l[j][k], l[j][k], v);
-    if (!(v > 0.0) || !isfinite(v)) { ok = false; v = 1.0; }
-    rd[j] = rsqrt(v);
-    l[j][j] = v * rd[j];
-#pragma unroll
-    for (int i = j + 1; i < 4; ++i) {
-      double w = a[i][j];
-#pragma unroll
-      for (int k = 0; k < j; ++k) w = fma(-l[i][k], l[j][k], w);
-      l[i][j] = w * rd[j];
-    }
-  }
-  return ok;
-}
-
 // Lower Cholesky of the 64x64 block D (row-major, row stride kTS; destroyed) by 256 threads, producing the inverse
 // factor Xi = L^-1 (lower triangular, row-major) and XiT = Xi^T.  T is scratch (>= 256 + 16 * kTS + 16 * kX16Stride doubles),
 // rdiag[64] receives 1 / L_jj.  Returns false on a non-positive pivot (the pivot is replaced by 1 so that the

@@ -96,20 +96,12 @@ __device__ __forceinline__ void frag_load_global(Frag& f, const double* tile, in
       f.c[mt][nt][0] = v.x; f.c[mt][nt][1] = v.y;
     }
 }
-// fragments -> smem row-major (dst[r][c]) / transposed (dst[c][r])
+// fragments -> smem row-major (dst[r][c])
 __device__ __forceinline__ void frag_store(double* dst, const Frag& f, const Lane& L) {
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
     for (int nt = 0; nt < 4; ++nt)
       *reinterpret_cast<double2*>(dst + L.row(mt) * kTS + L.col(nt)) = make_double2(f.c[mt][nt][0], f.c[mt][nt][1]);
-}
-__device__ __forceinline__ void frag_store_t(double* dst, const Frag& f, const Lane& L) {
-#pragma unroll
-  for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) dst[(L.col(nt) + e) * kTS + L.row(mt)] = f.c[mt][nt][e];
 }
 }  // namespace ctvio

@@ -13,7 +13,6 @@
 
 #include <algorithm>
 #include <atomic>
-#include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -130,7 +129,6 @@ struct ctvio_engine {
   bool masks_dirty = true;
   SplineParams sp;
   RigParams rig;
-  bool use_tma = true;
   bool deterministic = false;   // ctvio_set_deterministic: ordered flushes, single stream (kernels.h)
   DevBuf<int32_t> d_ticket;     // [0] kernel flush ticket, [1] scalar flush ticket
 
@@ -141,12 +139,8 @@ struct ctvio_engine {
   // state: two buffers (current / candidate) + snapshot
   DevState x[2], snap;
   DevState xs;                 // third state buffer of the pipelined LM driver (swapped into x[] when it ends up current)
-  DevBuf<LmPublished> d_pubstage;  // device staging copy of the published block (forwarded to h_pub from stream2)
   DevBuf<LmDecision> d_dec;    // device-side step decision (accept, next radius) read by the speculated linear solve
   cudaEvent_t ev_iter = nullptr;  // recorded behind the last kernel of every LM step (before anything speculative)
-  bool speculate = true;       // CTVIO_NO_SPECULATION=1 switches the pipelined driver off
-  bool staged_publish = false; // CTVIO_STAGED_PUBLISH=1: the scalar block reaches the host through a device staging copy
-                               // forwarded from stream2 (measured: no gain - off by default)
   DevState& state(int i) { return i < 2 ? x[i] : xs; }
   int cur = 0;
   bool table_valid = false;
@@ -340,14 +334,6 @@ int fetch_new_prior(ctvio_engine* e);
 int prepare(ctvio_engine* e) {
   if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
   ArenaScope arena(e);
-  static const bool prep_timing = std::getenv("CTVIO_PREP_TIMING") != nullptr;
-  auto tp0 = std::chrono::steady_clock::now();
-  auto lap = [&](const char* what) {
-    if (!prep_timing) return;
-    auto t = std::chrono::steady_clock::now();
-    std::fprintf(stderr, "[prepare] %-22s %7.1f us\n", what, std::chrono::duration<double, std::micro>(t - tp0).count());
-    tp0 = t;
-  };
   if (e->nK < 4) return fail(CTVIO_ERR_STATE, "need at least 4 knots");
   if (!e->have_bias) { e->nB = 0; }
   cudaStream_t st = e->stream;
@@ -423,14 +409,11 @@ int prepare(ctvio_engine* e) {
       hpj[k] = make_double2(o.pj[0], o.pj[1]);
       hm[k] = make_int4(o.rowi, o.rowj, o.lm, o.marg);
     }
-    lap("image windows + sort");
     // work items: chunks of one group; chunk size adapts so that small problems still spread over the SMs
-    // (a group is split into equal chunks of at most `cap` observations, cap a multiple of the 128-observation round)
     // one evaluation round (<= 128 observations, a lane pair each) per CTA: the round is latency bound whatever its
     // fill, so a group is cut into EQUAL chunks of at most one round (263 observations -> 3 x 88, not 128 + 128 + 7)
-    // and every chunk gets its own CTA; CTVIO_VIS_CAP overrides (multiples of 128) for experiments
-    int cap = kVisObsPerRound;
-    if (const char* env = std::getenv("CTVIO_VIS_CAP")) cap = std::max(kVisObsPerRound, std::atoi(env) / kVisObsPerRound * kVisObsPerRound);
+    // and every chunk gets its own CTA
+    constexpr int cap = kVisObsPerRound;
     std::vector<VisualItem>& items = e->h_items;
     items.clear();
     for (int k = 0; k < n;) {
@@ -466,7 +449,6 @@ int prepare(ctvio_engine* e) {
     CUDA_OK(e->d_img_orig.upload(e->img_order, st));
     CUDA_OK(e->d_items.upload(items, st));
 
-    lap("image arrays + upload");
     // ---- landmark layout ----
     e->h_woff.assign(e->nL + 1, 0);
     for (int l = 0; l < e->nL; ++l) {
@@ -476,7 +458,6 @@ int prepare(ctvio_engine* e) {
     CUDA_OK(e->d_lo.upload(e->h_lo, st));
     CUDA_OK(e->d_hi.upload(e->h_hi, st));
     CUDA_OK(e->d_woff.upload(e->h_woff, st));
-    lap("landmark layout");
     // ---- imu / bias factors ----
     const int ni = int(e->imu.size());
     std::vector<longlong2> it(ni);
@@ -536,7 +517,6 @@ int prepare(ctvio_engine* e) {
     CUDA_OK(e->d_bf_ij.upload(bij, st));
     CUDA_OK(e->d_bf_s.upload(bs, st));
 
-    lap("imu / bias");
     // ---- buffers ----
     const size_t np = size_t(d.np);
     e->off_gc = np * np;
@@ -555,7 +535,6 @@ int prepare(ctvio_engine* e) {
       e->linv_npad = e->npad;
       e->chol_seq = 0;
     }
-    lap("buffers");
     {
       // ---- K4 work items: per 64x64 tile (ti >= tj) of the reduced system the landmarks whose knot-dim range
       // [lo, hi) touches both blocks, cut into parts of `part` landmarks so that about two waves of CTAs exist
@@ -598,7 +577,6 @@ int prepare(ctvio_engine* e) {
       CUDA_OK(e->d_lis.reserve(e->nL));
       CUDA_OK(e->d_lc.reserve(e->nL));
     }
-    lap("schur lists");
     if (chol_dag_flags_len(e->npad) > e->d_chol_flags.cap) {
       CUDA_OK(e->d_chol_flags.reserve(chol_dag_flags_len(e->npad)));
       CUDA_OK(cudaMemsetAsync(e->d_chol_flags.p, 0, e->d_chol_flags.cap * sizeof(int32_t), e->stream));
@@ -612,7 +590,6 @@ int prepare(ctvio_engine* e) {
     if (e->nL > 0) CUDA_OK(cudaMemsetAsync(e->d_hh.p, 0, sizeof(double) * e->nL, st));
     e->prior_dirty = true;
   }
-  lap("reserves");
   // ---- masks (depend on options + structure) ----
   if (e->structure_dirty || e->masks_dirty) {
     e->h_cmask.assign(d.np, 0);
@@ -666,7 +643,6 @@ int prepare(ctvio_engine* e) {
     CUDA_OK(e->d_active.upload(e->h_active, st));
     e->masks_dirty = false;
   }
-  lap("masks");
   e->structure_dirty = false;
   if (e->prior_dirty) {
     const int rc = prepare_prior(e);
@@ -751,7 +727,6 @@ VisualLaunch visual_launch(ctvio_engine* e, int xb, int nb, double cauchy) {
   v.cauchy = cauchy;
   v.cmask = e->d_cmask.p;
   v.scal = e->d_scal.p;
-  v.use_tma = e->use_tma;
   v.det_ticket = e->deterministic ? e->d_ticket.p : nullptr;
   return v;
 }
@@ -951,7 +926,7 @@ int read_scalars(ctvio_engine* e, bool published = false) {
       if ((++spins & 0xfffu) == 0 && cudaStreamQuery(e->stream) != cudaErrorNotReady) {
         if (*seq == e->pub_seq) break;
         CUDA_OK(cudaStreamSynchronize(e->stream));
-        CUDA_OK(cudaStreamSynchronize(e->stream2));  // (pipelined driver: the publication is forwarded from stream2)
+        CUDA_OK(cudaStreamSynchronize(e->stream2));  // (the factor kernels forked onto stream2 are settled too)
         if (*seq != e->pub_seq) return fail(CTVIO_ERR_CUDA, "LM step finished without publishing its scalars");
       }
     }
@@ -1022,10 +997,6 @@ int ctvio_create(const ctvio_config* cfg, ctvio_handle* out) {
   e->rig.gravity = V3{cfg->gravity[0], cfg->gravity[1], cfg->gravity[2]};
   for (int k = 0; k < 6; ++k) e->rig.imu_info[k] = cfg->imu_info[k];
   if (const char* det = std::getenv("CTVIO_DETERMINISTIC")) e->deterministic = det[0] == '1';
-  if (const char* ns = std::getenv("CTVIO_NO_SPECULATION")) e->speculate = ns[0] != '1';
-  if (const char* dp = std::getenv("CTVIO_STAGED_PUBLISH")) e->staged_publish = dp[0] == '1';
-  const char* no_tma = std::getenv("CTVIO_NO_TMA");
-  e->use_tma = !(no_tma && no_tma[0] == '1');
   if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess ||
       cudaStreamCreateWithFlags(&e->stream2, cudaStreamNonBlocking) != cudaSuccess ||
       cudaStreamCreateWithFlags(&e->stream3, cudaStreamNonBlocking) != cudaSuccess ||
@@ -1034,7 +1005,7 @@ int ctvio_create(const ctvio_config* cfg, ctvio_handle* out) {
       cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&e->ev_zero, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreate(&e->ev_iter) != cudaSuccess || e->d_dec.reserve(1) != cudaSuccess || e->d_pubstage.reserve(1) != cudaSuccess ||
+      cudaEventCreate(&e->ev_iter) != cudaSuccess || e->d_dec.reserve(1) != cudaSuccess ||
       cudaHostAlloc(&e->h_pub, sizeof(LmPublished), cudaHostAllocMapped) != cudaSuccess ||
       cudaMallocHost(&e->h_scal, sizeof(LmScalars)) != cudaSuccess || e->d_scal.reserve(1) != cudaSuccess ||
       e->d_ticket.reserve(4) != cudaSuccess) {
@@ -1378,14 +1349,14 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
   // finds step i rejected / invalid / terminating, the speculated kernels' results are simply never used (they touch
   // only the step vectors, the free state buffer and per-step scalars that the next real step resets).
   // It pays at C2 / C5 sizes but was measured slower per LM step at 100 k observations and more, with identical kernels
-  // and a host that is provably ahead (CTVIO_LM_TRACE) - cause not found; the round trip it hides is a small part of
-  // such a step anyway.  CTVIO_SPECULATION=always / never overrides the size test.
+  // while host timestamps showed the host ahead of the device - cause not found; the round trip it hides is a small
+  // part of such a step anyway.  CTVIO_SPECULATION=always / never overrides the size test.
   bool spec_size_ok = e->img.size() <= 20000;
   if (const char* sp = std::getenv("CTVIO_SPECULATION")) {
     if (std::strcmp(sp, "always") == 0) spec_size_ok = true;
     if (std::strcmp(sp, "never") == 0) spec_size_ok = false;
   }
-  const bool pipelined = e->speculate && spec_size_ok && !sharded && !is_constrained && !e->deterministic;
+  const bool pipelined = spec_size_ok && !sharded && !is_constrained && !e->deterministic;
   int cur_ne = cur;  // normal-equation buffer of the current point (state and normal equations flip separately here)
   if (pipelined) {
     rc = alloc_state(e, e->xs);
@@ -1394,8 +1365,6 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
     bool spec_in_flight = false; // speculated kernels that read ne_slab[cur_ne ^ 1] may still be running
     int spec_out = -1;
     unsigned spec_chol_seq0 = e->chol_seq;
-    double host_spec_us = 0, host_wait_us = 0;
-    static const bool lm_trace = std::getenv("CTVIO_LM_TRACE") != nullptr;  // host-side timing of the driver
     cudaEventRecord(e->ev_iter, st);
     while (true) {
       if (iter >= max_iterations) { term = CTVIO_TERM_NO_CONVERGENCE; break; }
@@ -1423,14 +1392,8 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
       const LmDecideArgs da{e->d_dec.p, x_cost, radius, min_relative_decrease, max_radius,
                             parameter_tolerance, function_tolerance, gradient_tolerance, min_radius};
       e->launches += launch_gradient_norm(linear_launch(e, cand_ne), e->state(cand).ptrs(), e->opt.fix_ld, e->opt.ld_lower,
-                                          e->opt.ld_upper, st, false, e->staged_publish ? e->d_pubstage.p : e->h_pub, ++e->pub_seq,
-                                          &da);
+                                          e->opt.ld_upper, st, false, e->h_pub, ++e->pub_seq, &da);
       cudaEventRecord(e->ev_iter, st);
-      if (e->staged_publish) {
-        // the block goes to the host from the second stream: its PCIe round trip overlaps the speculated linear solve
-        cudaStreamWaitEvent(e->stream2, e->ev_iter, 0);
-        e->launches += launch_publish(e->d_pubstage.p, e->h_pub, e->stream2);
-      }
       // ---- speculate: step iter + 1 from (cand, cand_ne), radius from the device-side decision ----
       spec_ready = false;
       if (iter < max_iterations) {
@@ -1438,16 +1401,12 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
         while (spec_out == cur || spec_out == cand) ++spec_out;
         const ApplyLaunch spec_step = make_apply(cand, spec_out, 1.0);
         spec_chol_seq0 = e->chol_seq;
-        const auto th0 = std::chrono::steady_clock::now();
         rc = lm_step(e, cand_ne, 0.0, &spec_step, &e->d_dec.p->radius_next, &e->d_dec.p->go);
         if (rc) return rc;
         spec_ready = true;
         spec_in_flight = true;
-        host_spec_us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - th0).count();
       }
-      const auto th1 = std::chrono::steady_clock::now();
       rc = read_scalars(e, true);
-      host_wait_us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - th1).count();
       if (rc) return rc;
       const LmScalars sc = *e->h_scal;
       const LmDecision dec = const_cast<const LmPublished*>(e->h_pub)->dec;
@@ -1515,7 +1474,6 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
     CUDA_OK(cudaStreamSynchronize(e->stream2));
     float ms = 0;
     cudaEventElapsedTime(&ms, e->ev0, e->ev_iter);
-    if (lm_trace) std::fprintf(stderr, "[lm] iters %d device %.3f ms host: spec enqueue %.1f us/iter, wait %.1f us/iter\n", iter, ms, host_spec_us / std::max(iter, 1), host_wait_us / std::max(iter, 1));
     sum.iterations = iter;
     sum.termination = term;
     sum.final_cost = x_cost;

@@ -212,7 +212,6 @@ struct VisualLaunch {
   double cauchy;
   const uint8_t* cmask;   // [np] 1 = constant
   LmScalars* scal;
-  bool use_tma;
   int* det_ticket = nullptr;  // deterministic mode: flush in block order
 };
 int launch_visual(const VisualLaunch& a, bool full, cudaStream_t s);
@@ -290,7 +289,6 @@ int launch_lm_step(const LinearLaunch& a, double radius, cudaStream_t s);
 // the three stages of launch_lm_step, separately launchable for measurement
 // radius_dev != null: the radius is read from device memory (first double of an LmDecision)
 int launch_reduced_system(const LinearLaunch& a, double radius, cudaStream_t s, const double* radius_dev = nullptr);
-int launch_publish(const LmPublished* stage, LmPublished* pub, cudaStream_t s);
 int launch_factor_solve(const LinearLaunch& a, cudaStream_t s);
 // tile-DAG variant (chol_dag.cu): usable when every tile gets its own SM
 bool chol_dag_supported(int npad, int n_sm);
@@ -301,9 +299,8 @@ int launch_chol_dag_init(double* linv_buf, double* part_buf, int npad, cudaStrea
 int launch_chol_dag(const LinearLaunch& a, cudaStream_t s);
 int launch_chol_coop(const LinearLaunch& a, cudaStream_t s);
 int launch_step_vectors(const LinearLaunch& a, cudaStream_t s);
-// sharded mode: after the all-reduce of [M | rhs | diagA] add the LM damping, identity rows of constant /
-// padding dims; and the iteration-0 Jacobi scale from the all-reduced diagonal
-int launch_add_damping(const LinearLaunch& a, double radius, cudaStream_t s);
+// sharded mode: the iteration-0 Jacobi scale from the all-reduced camera diagonal (the LM damping and identity rows
+// of constant / padding dims are added after the all-reduce by launch_shard_unpack, marginalize.h)
 int launch_extract_diag(const LinearLaunch& a, cudaStream_t s);
 int launch_jacobi_scale_from_diag(const LinearLaunch& a, cudaStream_t s);
 // reset = false: the accumulator was already zeroed by scale_copy_kernel of the same LM step

@@ -316,22 +316,6 @@ __global__ void __launch_bounds__(256) step_vectors_kernel(LinearLaunch a, int n
   else landmark_step_block(a, blockIdx.x - ncb, nullptr);
 }
 
-__global__ void add_damping_kernel(LinearLaunch a, double radius) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= a.npad) return;
-  double* d = a.M + size_t(i) * a.npad + i;
-  if (i < a.dims.np && !a.cmask[i]) {
-    const double sd = a.sc[i] * a.sc[i] * a.diagA[i];
-    *d += fmin(fmax(sd, kMinLmDiag), kMaxLmDiag) / radius;
-  } else {
-    *d = 1.0;
-    a.rhs[i] = 0.0;
-  }
-}
-int launch_add_damping(const LinearLaunch& a, double radius, cudaStream_t s) {
-  add_damping_kernel<<<(a.npad + 255) / 256, 256, 0, s>>>(a, radius);
-  return 1;
-}
 __global__ void extract_diag_kernel(LinearLaunch a) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.npad) return;
@@ -376,9 +360,7 @@ int launch_lm_step(const LinearLaunch& a, double radius, cudaStream_t s) {
 
 // max-norm of the (bounds-projected) gradient over the active parameters; a few CTAs (one per 1024 entries, at most
 // 16), combined with an integer atomicMax on the bit pattern (the values are non-negative); the CTA that arrives
-// last hands the finished scalar block of the LM step to `pub`: mapped host memory, or a device staging block that
-// publish_kernel forwards from a second stream (pipelined driver: the PCIe write round trip of the publication then
-// overlaps the next step's linear solve instead of delaying it)
+// last hands the finished scalar block of the LM step to `pub` (mapped host memory)
 __global__ void __launch_bounds__(1024) gradient_norm_kernel(LinearLaunch a, StatePtrs st, int fix_ld, double ld_lower,
                                                              double ld_upper, LmPublished* pub, unsigned long long seq,
                                                              LmDecideArgs da) {
@@ -471,29 +453,6 @@ int launch_gradient_norm(const LinearLaunch& a, const StatePtrs& st, int fix_ld,
   const int n = a.dims.np + a.dims.nL;
   const int grid = std::min(16, std::max(1, (n + 1023) / 1024));
   gradient_norm_kernel<<<grid, 1024, 0, s>>>(a, st, fix_ld, ld_lower, ld_upper, pub, seq, da);
-  return 1;
-}
-
-// staging block (device) -> mapped host memory, on a stream of its own
-__global__ void publish_kernel(const LmPublished* __restrict__ stage, LmPublished* pub) {
-  if (threadIdx.x == 0) {
-    static_assert(sizeof(LmPublished) % 16 == 0, "copied as 16-byte words");
-    constexpr int kWords = int(offsetof(LmPublished, seq) / 16);
-    static_assert(offsetof(LmPublished, seq) % 16 == 0, "payload is a whole number of 16-byte words");
-    const uint4* src = reinterpret_cast<const uint4*>(stage);
-    uint4* dst = reinterpret_cast<uint4*>(pub);
-    uint4 w[kWords];
-#pragma unroll
-    for (int k = 0; k < kWords; ++k) w[k] = __ldcg(src + k);
-    const unsigned long long seq = __ldcg(&stage->seq);
-#pragma unroll
-    for (int k = 0; k < kWords; ++k) dst[k] = w[k];
-    __threadfence_system();
-    *reinterpret_cast<volatile unsigned long long*>(&pub->seq) = seq;
-  }
-}
-int launch_publish(const LmPublished* stage, LmPublished* pub, cudaStream_t s) {
-  publish_kernel<<<1, 32, 0, s>>>(stage, pub);
   return 1;
 }
 

@@ -37,7 +37,6 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -99,7 +98,6 @@ struct VisArgs {
   double cauchy;
   const uint8_t* cmask;
   LmScalars* scal;
-  int use_tma;
   int* det_ticket;
 };
 
@@ -217,52 +215,34 @@ __global__ void __launch_bounds__(kVisThreads, 1) visual_kernel(const __grid_con
 
   // ---- stage the 10 active knots + 8 knot-pair entries (TMA bulk copies, one mbarrier) ----
   const int w0[2] = {item.wi0, item.wj0};
-  if (a.use_tma) {
-    if (tid == 0) {
-      sm.err = 0;
-      mbar_init(reinterpret_cast<uint64_t*>(&sm.bar), 1);
-      fence_mbar_init();
-    }
-    __syncthreads();
-    if (tid == 0) {
-      uint32_t bytes = 0;
+  if (tid == 0) {
+    sm.err = 0;
+    mbar_init(reinterpret_cast<uint64_t*>(&sm.bar), 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    uint32_t bytes = 0;
 #pragma unroll
-      for (int sd = 0; sd < 2; ++sd) {
-        const int nk = min(kWinKnots, nK - w0[sd]);
-        const int npair = min(4, nK - 1 - w0[sd]);
-        bytes += uint32_t(nk) * 64u + uint32_t(npair) * uint32_t(sizeof(KnotPair));
-      }
-      mbar_expect_tx(reinterpret_cast<uint64_t*>(&sm.bar), bytes);
+    for (int sd = 0; sd < 2; ++sd) {
+      const int nk = min(kWinKnots, nK - w0[sd]);
+      const int npair = min(4, nK - 1 - w0[sd]);
+      bytes += uint32_t(nk) * 64u + uint32_t(npair) * uint32_t(sizeof(KnotPair));
+    }
+    mbar_expect_tx(reinterpret_cast<uint64_t*>(&sm.bar), bytes);
 #pragma unroll
-      for (int sd = 0; sd < 2; ++sd) {
-        const int nk = min(kWinKnots, nK - w0[sd]);
-        const int npair = min(4, nK - 1 - w0[sd]);
-        tma_bulk_g2s(&sm.q[sd][0][0], a.st.q + 4 * w0[sd], uint32_t(nk) * 32u, reinterpret_cast<uint64_t*>(&sm.bar));
-        tma_bulk_g2s(&sm.p[sd][0][0], a.st.p + 4 * w0[sd], uint32_t(nk) * 32u, reinterpret_cast<uint64_t*>(&sm.bar));
-        tma_bulk_g2s(&sm.tab[sd][0], a.st.tab + w0[sd], uint32_t(npair) * uint32_t(sizeof(KnotPair)),
-                     reinterpret_cast<uint64_t*>(&sm.bar));
-      }
-    }
-  } else {
-    if (tid == 0) sm.err = 0;
-    // plain cooperative loads (debug path, CTVIO_NO_TMA=1)
-    for (int i = tid; i < 2 * kWinKnots * 4; i += kVisThreads) {
-      const int sd = i / (kWinKnots * 4), r = i % (kWinKnots * 4);
-      const int k = w0[sd] + r / 4;
-      (&sm.q[sd][0][0])[r] = k < nK ? a.st.q[4 * k + (r & 3)] : 0.0;
-      (&sm.p[sd][0][0])[r] = k < nK ? a.st.p[4 * k + (r & 3)] : 0.0;
-    }
-    for (int i = tid; i < 2 * 4 * 16; i += kVisThreads) {
-      const int sd = i / 64, r = i % 64;
-      const int k = w0[sd] + r / 16;
-      reinterpret_cast<double*>(&sm.tab[sd][0])[r] = k < nK - 1 ? reinterpret_cast<const double*>(a.st.tab + k)[r & 15] : 0.0;
+    for (int sd = 0; sd < 2; ++sd) {
+      const int nk = min(kWinKnots, nK - w0[sd]);
+      const int npair = min(4, nK - 1 - w0[sd]);
+      tma_bulk_g2s(&sm.q[sd][0][0], a.st.q + 4 * w0[sd], uint32_t(nk) * 32u, reinterpret_cast<uint64_t*>(&sm.bar));
+      tma_bulk_g2s(&sm.p[sd][0][0], a.st.p + 4 * w0[sd], uint32_t(nk) * 32u, reinterpret_cast<uint64_t*>(&sm.bar));
+      tma_bulk_g2s(&sm.tab[sd][0], a.st.tab + w0[sd], uint32_t(npair) * uint32_t(sizeof(KnotPair)),
+                   reinterpret_cast<uint64_t*>(&sm.bar));
     }
   }
   if (FULL)
     for (int i = tid; i < 36 * 64; i += kVisThreads) accs[i] = 0.0;
-  if (a.use_tma) {
-    while (!mbar_try_wait(reinterpret_cast<uint64_t*>(&sm.bar), 0)) {
-    }
+  while (!mbar_try_wait(reinterpret_cast<uint64_t*>(&sm.bar), 0)) {
   }
   __syncthreads();
 
@@ -353,12 +333,10 @@ __global__ void __launch_bounds__(kVisThreads, 1) visual_kernel(const __grid_con
               const double p0v = mp ? 0.0 : ck * cm.JvR[c], p1v = mp ? 0.0 : ck * cm.JvR[3 + c];
               row0[col + c] = r0v; row1[col + c] = r1v;
               row0[col + 3 + c] = p0v; row1[col + 3 + c] = p1v;
-#ifndef CTVIO_EXPERIMENT_NO_W_ATOMICS
               if (!a.det_ticket) {  // (deterministic mode: recomputed from the shared tile inside the ordered flush)
                 if (!mr) atomicAdd(Wl + gd + c, r0v * jrho[0] + r1v * jrho[1]);
                 if (!mp) atomicAdd(Wl + gd + 3 + c, p0v * jrho[0] + p1v * jrho[1]);
               }
-#endif
             }
           });
           if (side == 0) {
@@ -496,7 +474,7 @@ __global__ void __launch_bounds__(kVisThreads, 1) visual_kernel(const __grid_con
 
 int launch_visual(const VisualLaunch& l, bool full, cudaStream_t s) {
   if (l.n_items <= 0) return 0;
-  VisArgs a{l.obs, l.items, l.st, l.ne, l.lm, l.dims, l.sp, l.rig, l.cauchy, l.cmask, l.scal, l.use_tma ? 1 : 0, l.det_ticket};
+  VisArgs a{l.obs, l.items, l.st, l.ne, l.lm, l.dims, l.sp, l.rig, l.cauchy, l.cmask, l.scal, l.det_ticket};
   static PerDeviceOnce once;
   if (once.first()) {
     cudaFuncSetAttribute(visual_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(visual_smem_bytes()));
@@ -831,7 +809,7 @@ __global__ void probe_image_kernel(VisArgs a, const int32_t* orig_index, int wan
 int launch_probe_image(const VisualLaunch& l, const int32_t* orig_index, bool want_jac, double* r, int32_t* s,
                        double* J, cudaStream_t st) {
   if (l.obs.n <= 0) return 0;
-  VisArgs a{l.obs, l.items, l.st, l.ne, l.lm, l.dims, l.sp, l.rig, l.cauchy, l.cmask, l.scal, 0, nullptr};
+  VisArgs a{l.obs, l.items, l.st, l.ne, l.lm, l.dims, l.sp, l.rig, l.cauchy, l.cmask, l.scal, nullptr};
   probe_image_kernel<<<(l.obs.n + 63) / 64, 64, 0, st>>>(a, orig_index, want_jac ? 1 : 0, r, s, J);
   return 1;
 }

@@ -243,8 +243,6 @@ __global__ void __launch_bounds__(1024) jacobi_eig_kernel(double* A, double* V, 
     if ((tid & 31) == 0) { atomicAdd(&s_off, off); atomicAdd(&s_diag, dg); }
     __syncthreads();
     // converged, or stagnating at the rounding floor (the off-diagonal mass no longer halves per sweep once it is
-    // below ~(n eps)^2 of the diagonal mass): more sweeps only shuffle noise
-    // converged, or stagnating at the rounding floor (the off-diagonal mass no longer halves per sweep once it is
     // below ~(n eps)^2 of the diagonal mass): more sweeps only shuffle noise.  (Stopping earlier, e.g. one sweep after
     // 1e-20, is NOT an option: the eps = 1e-30 pseudo-inverse of the reference inverts the smallest eigenvalues, so
     // their RELATIVE accuracy matters - measured: 5e-3 cost drift over a few windows.)
@@ -306,115 +304,10 @@ __global__ void __launch_bounds__(1024) jacobi_eig_kernel(double* A, double* V, 
   for (int i = tid; i < n; i += nt) ev[i] = A[size_t(i) * n + i];
 }
 
-// Same algorithm with A and V resident in shared memory (odd row stride: column accesses spread over the banks);
-// used whenever both fit (n <= ~117), i.e. for every prior of a TUM-RSVI-scale window: the three phases of a round
-// are then bound by shared-memory latency instead of L2 round trips.
-__global__ void __launch_bounds__(1024) jacobi_eig_smem_kernel(double* Ag, double* Vg, double* ev, int n, int max_sweeps) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int ld = n | 1;  // odd row stride (in doubles): a column walk visits 16 distinct bank pairs
-  double* A = reinterpret_cast<double*>(smem_raw);
-  double* V = A + size_t(n) * ld;
-  double* cs = V + size_t(n) * ld;                             // [npairs][2]
-  int* pp = reinterpret_cast<int*>(cs + 2 * ((n + 1) / 2));   // [npairs][2]
-  __shared__ double s_off, s_diag, s_prev;
-  const int tid = threadIdx.x, nt = blockDim.x;
-  const int ne = (n + 1) & ~1;
-  const int npairs = ne / 2;
-  for (int e = tid; e < n * n; e += nt) {
-    const int i = e / n, j = e % n;
-    A[i * ld + j] = Ag[e];
-    V[i * ld + j] = (i == j) ? 1.0 : 0.0;
-  }
-  __syncthreads();
-  for (int sweep = 0; sweep < max_sweeps; ++sweep) {
-    if (tid == 0) { s_off = 0.0; s_diag = 0.0; }
-    __syncthreads();
-    double off = 0, dg = 0;
-    for (int e = tid; e < n * n; e += nt) {
-      const int i = e / n, j = e % n;
-      const double v = A[i * ld + j];
-      if (i == j) dg += v * v; else off += v * v;
-    }
-    for (int o = 16; o > 0; o >>= 1) {
-      off += __shfl_xor_sync(0xffffffffu, off, o);
-      dg += __shfl_xor_sync(0xffffffffu, dg, o);
-    }
-    if ((tid & 31) == 0) { atomicAdd(&s_off, off); atomicAdd(&s_diag, dg); }
-    __syncthreads();
-    // converged, or stagnating at the rounding floor (the off-diagonal mass no longer halves per sweep once it is
-    // below ~(n eps)^2 of the diagonal mass): more sweeps only shuffle noise
-    // converged, or stagnating at the rounding floor (the off-diagonal mass no longer halves per sweep once it is
-    // below ~(n eps)^2 of the diagonal mass): more sweeps only shuffle noise.  (Stopping earlier, e.g. one sweep after
-    // 1e-20, is NOT an option: the eps = 1e-30 pseudo-inverse of the reference inverts the smallest eigenvalues, so
-    // their RELATIVE accuracy matters - measured: 5e-3 cost drift over a few windows.)
-    const double prev = sweep > 0 ? s_prev : 1e300;
-    if (s_off <= 1e-60 || s_off <= 1e-30 * s_diag || (s_off <= 1e-24 * s_diag && s_off > 0.5 * prev)) break;
-    __syncthreads();
-    if (tid == 0) s_prev = s_off;
-    for (int round = 0; round < ne - 1; ++round) {
-      for (int k = tid; k < npairs; k += nt) {
-        int p, q;
-        if (k == 0) { p = ne - 1; q = round % (ne - 1); }
-        else { p = (round + k) % (ne - 1); q = (round + ne - 1 - k) % (ne - 1); }
-        if (p > q) { const int t = p; p = q; q = t; }
-        double c = 1.0, s = 0.0;
-        if (q < n) {
-          const double apq = A[p * ld + q];
-          if (apq != 0.0) {
-            const double app = A[p * ld + p], aqq = A[q * ld + q];
-            const double theta = (aqq - app) / (2.0 * apq);
-            const double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-            c = 1.0 / sqrt(t * t + 1.0);
-            s = t * c;
-          }
-        }
-        cs[2 * k] = c; cs[2 * k + 1] = s;
-        pp[2 * k] = p; pp[2 * k + 1] = q;
-      }
-      __syncthreads();
-      // warp = pair (k, k + 32, ...), lanes stride over the rows / columns: no integer divisions in the hot loops
-      const int warp = tid >> 5, lane = tid & 31, nwarps = nt >> 5;
-      for (int k = warp; k < npairs; k += nwarps) {
-        const int p = pp[2 * k], q = pp[2 * k + 1];
-        if (q >= n) continue;
-        const double c = cs[2 * k], s = cs[2 * k + 1];
-        if (s == 0.0) continue;
-        for (int r = lane; r < n; r += 32) {
-          const double ap = A[r * ld + p], aq = A[r * ld + q];
-          A[r * ld + p] = c * ap - s * aq;
-          A[r * ld + q] = s * ap + c * aq;
-          const double vp = V[r * ld + p], vq = V[r * ld + q];
-          V[r * ld + p] = c * vp - s * vq;
-          V[r * ld + q] = s * vp + c * vq;
-        }
-      }
-      __syncthreads();
-      for (int k = warp; k < npairs; k += nwarps) {
-        const int p = pp[2 * k], q = pp[2 * k + 1];
-        if (q >= n) continue;
-        const double c = cs[2 * k], s = cs[2 * k + 1];
-        if (s == 0.0) continue;
-        for (int col = lane; col < n; col += 32) {
-          const double ap = A[p * ld + col], aq = A[q * ld + col];
-          A[p * ld + col] = c * ap - s * aq;
-          A[q * ld + col] = s * ap + c * aq;
-        }
-      }
-      __syncthreads();
-    }
-  }
-  for (int e = tid; e < n * n; e += nt) {
-    const int i = e / n, j = e % n;
-    Ag[e] = A[i * ld + j];
-    Vg[e] = V[i * ld + j];
-  }
-  for (int i = tid; i < n; i += nt) ev[i] = A[i * ld + i];
-}
-
 // Two-sided parallel Jacobi, block form.  The n/2 disjoint rotations of a round act on A as  A <- J' A J : the 2x2
 // block of rows {p_k, q_k} and columns {p_l, q_l} becomes  R_k' B R_l  and depends on NO other entry, so one thread
 // owns one (k, l) block for the whole round, in place, rows and columns in ONE phase: 2 barriers per round
-// (rotations | update) instead of the 3 + separate row pass of the kernels above, and 4 loads / 4 stores per 12 FMAs.
+// (rotations | update) instead of the 3 + separate row pass of the kernel above, and 4 loads / 4 stores per 12 FMAs.
 // V <- V J rides in the same phase.  The (k, l) -> thread assignment does not depend on the round, so the index
 // arithmetic is hoisted out of the sweep loop.  Rotation sequence and every sum are fixed: bit-reproducible.
 // A_SMEM / V_SMEM: the matrix / the eigenvectors live in shared memory (odd row stride) or stay in global memory (L2).

@@ -108,7 +108,6 @@ double measure_fp64_tflops(cudaStream_t s);
 // optionally the dependent latency of one mma in cycles; < 0 on error
 double measure_fp64_tensor_tflops(cudaStream_t s, int ctas_per_sm = 4, double* dep_latency_cycles = nullptr);
 
-int launch_flags_to_double(LmScalars* scal, cudaStream_t s);
 int launch_rho_pack(const double* rho, const uint8_t* owned, double* buf, int nL, cudaStream_t s);
 int launch_rho_unpack(double* rho, const double* buf, int nL, cudaStream_t s);
 
@@ -123,7 +122,7 @@ bool comm_allgather(void* comm, const double* send, double* recv, size_t n_per_r
 // sharded mode: lower-triangular 64x64 tiles of M + rhs + diagA <-> one contiguous all-reduce buffer
 size_t shard_pack_len(int npad);
 int launch_shard_pack(const LinearLaunch& a, double* packed, cudaStream_t s);
-// after the all-reduce: scatter back, add the LM damping / identity rows (replaces add_damping_kernel)
+// after the all-reduce: scatter back, add the LM damping / identity rows
 int launch_shard_unpack(const LinearLaunch& a, const double* packed, double radius, cudaStream_t s);
 // sharded mode: per-rank scalar blocks (all-gathered, [world][8]) -> the common scalar block: sums of cost / g'd / d'Hd /
 // |dx|^2 / |x|^2 / error flag, maxima of the gradient / step max-norms; identical on every rank, published to the mapped

@@ -42,12 +42,7 @@ int launch_dot_gradient(const LinearLaunch& a, cudaStream_t s) {
 }
 
 // sharded mode helpers
-__global__ void flags_to_double_kernel(LmScalars* scal) { scal->err_sum = (scal->error_flags != 0) ? 1.0 : 0.0; }
-int launch_flags_to_double(LmScalars* scal, cudaStream_t s) {
-  flags_to_double_kernel<<<1, 1, 0, s>>>(scal);
-  return 1;
-}
-// buf = [rho masked by ownership (nL) | owned (nL)] before the all-reduce, rho <- sum / count afterwards
+// buf =[rho masked by ownership (nL) | owned (nL)] before the all-reduce, rho <- sum / count afterwards
 __global__ void rho_pack_kernel(const double* rho, const uint8_t* owned, double* buf, int nL) {
   const int l = blockIdx.x * blockDim.x + threadIdx.x;
   if (l >= nL) return;

@@ -1,5 +1,4 @@
-"""Host-side cost of the host-buffer path at C2: per-call wall clock of one e2e step (Set* / Add* / Solve / Get*), and the
-laps of prepare() when CTVIO_PREP_TIMING=1 is set."""
+"""Host-side cost of the host-buffer path at C2: per-call wall clock of one e2e step (Set* / Add* / Solve / Get*)."""
 import importlib, os, sys, time
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -11,7 +10,6 @@ est.SetOptions(pkg.make_options(fix_ld=w.fix_ld, ld_lower=w.ld_lower, ld_upper=w
 names = ["SetKnots", "SetBiases", "SetInvDepths", "SetLineDelay", "ClearFactors", "AddImage", "AddIMU", "AddBias", "Solve", "GetKnots", "GetBiases", "GetInvDepths", "GetLineDelay"]
 acc = np.zeros(len(names)); n = 0
 for it in range(30):
-    if it == 29: os.environ["CTVIO_PREP_TIMING_NOW"] = "1"
     ts = [time.perf_counter()]
     est.SetKnots(w.q0, w.p0); ts.append(time.perf_counter())
     est.SetBiases(w.bias0); ts.append(time.perf_counter())
