@@ -103,7 +103,7 @@ ABI_SYMBOLS = [
     "query_trajectory", "triangulate",
     "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior", "ingest_feature_cloud", "add_image_features_from_slots",
     "ingest_imu", "add_imu_from_table", "transfer_stats", "profile_kernels", "measure_fp64_tflops", "measure_fp64_tensor_tflops",
-    "selfcheck_solver", "nccl_unique_id", "comm_init", "triangulate_window",
+    "selfcheck_solver", "nccl_unique_id", "comm_init", "triangulate_window", "check_keyframe", "slide_window_second_new",
 ]
 
 
@@ -111,7 +111,8 @@ ABI_SYMBOLS = [
 # the device-residency / wire-format calls, which have no CPU meaning
 DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enable_prior", "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior",
                        "ingest_feature_cloud", "add_image_features_from_slots", "ingest_imu", "add_imu_from_table",
-                       "transfer_stats", "residual_summary", "triangulate_window")
+                       "transfer_stats", "residual_summary", "triangulate_window", "check_keyframe",
+                       "slide_window_second_new")
 
 
 def _addr(a):
@@ -401,6 +402,21 @@ class Estimator:
         self.lib.call("slide_window", self.h, C.c_int32(n_drop_knots), C.c_int32(n_drop_bias), C.c_int32(n_new_bias))
         self.n_knots -= n_drop_knots
         self.n_bias += n_new_bias - n_drop_bias
+
+    def SlideWindowSecondNew(self):
+        """the MARGIN_SECOND_NEW slide (visual_odometry.cpp:253-278): bias node n-2 takes node n-1's value; knots and
+        prior stay."""
+        self.lib.call("slide_window_second_new", self.h)
+
+    def CheckKeyframe(self, frame_slots, min_parallax):
+        """FeatureManager::addFeatureCheckParallax (feature_manager.cpp:28-87) over resident frame slots, oldest to
+        newest, the new image last.  Returns (is_keyframe, n_tracked, parallax_num, parallax_sum)."""
+        slots = _i32(frame_slots)
+        kf, nt, num = C.c_int32(), C.c_int32(), C.c_int32()
+        s = C.c_double()
+        self.lib.call("check_keyframe", self.h, C.c_int32(slots.shape[0]), _ip(slots), C.c_double(min_parallax),
+                      C.byref(kf), C.byref(nt), C.byref(num), C.byref(s))
+        return bool(kf.value), nt.value, num.value, s.value
 
     def EnablePrior(self, on: bool):
         self.lib.call("enable_prior", self.h, C.c_int32(int(on)))

@@ -236,6 +236,7 @@ struct ctvio_engine {
   DevBuf<double> d_tmp;  // scratch (gauge inputs, probe outputs)
   DevBuf<int32_t> d_tri_idx;  // index uploads: ctvio_triangulate, ctvio_remap_landmarks, ctvio_triangulate_window
   DevBuf<int32_t> d_tri_cnt;  // ctvio_triangulate_window: {triangulated, fallback}
+  DevBuf<ctvio::KeyframeResult> d_kf_result;  // ctvio_check_keyframe
   // marginalization workspace (K7), kept across windows: allocation / free costs more than the kernels
   struct MargWs {
     DevBuf<int32_t> pos_cam, pos_lm, prior_pos, marg_img, marg_imu;
@@ -2470,6 +2471,64 @@ int ctvio_triangulate_window(ctvio_handle e, int32_t nl, const int32_t* obs_offs
   e->mirror_valid = false;
   if (n_triangulated) *n_triangulated = cnt[0];
   if (n_fallback) *n_fallback = cnt[1];
+  return CTVIO_OK;
+}
+
+int ctvio_check_keyframe(ctvio_handle e, int32_t n_frames, const int32_t* frame_slots, double min_parallax,
+                         int32_t* is_keyframe, int32_t* n_tracked, int32_t* parallax_num, double* parallax_sum) {
+  static_assert(ctvio_engine::kFrameSlots == ctvio::kKeyframeMaxSlots && ctvio_engine::kFrameCap == ctvio::kKeyframeMaxFeatures,
+                "the keyframe kernel covers the whole frame table");
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (!frame_slots || !is_keyframe) return fail(CTVIO_ERR_INVALID, "null argument");
+  if (n_frames < 1 || n_frames > ctvio_engine::kFrameSlots) return fail(CTVIO_ERR_INVALID, "n_frames must be 1..16");
+  if (!(min_parallax >= 0.0) || !std::isfinite(min_parallax)) return fail(CTVIO_ERR_INVALID, "min_parallax must be finite and >= 0");
+  ctvio::KeyframeArgs a;
+  uint32_t listed = 0;
+  for (int k = 0; k < n_frames; ++k) {
+    const int s = frame_slots[k];
+    if (s < 0 || s >= ctvio_engine::kFrameSlots) return fail(CTVIO_ERR_INVALID, "frame slot out of range");
+    if (listed & (1u << s)) return fail(CTVIO_ERR_INVALID, "a frame slot is listed twice");
+    listed |= 1u << s;
+    a.slot[k] = s;
+    a.count[k] = e->h_frame_n[s];  // 0 for a slot that never received a cloud
+  }
+  cudaSetDevice(e->cfg.device);
+  cudaStream_t st = e->stream;
+  CUDA_OK(e->d_frames.reserve(size_t(ctvio_engine::kFrameSlots) * ctvio_engine::kFrameCap));
+  CUDA_OK(e->d_kf_result.reserve(1));
+  a.table = e->d_frames.p; a.frame_cap = ctvio_engine::kFrameCap; a.n_frames = n_frames;
+  a.min_parallax = min_parallax; a.out = e->d_kf_result.p;
+  // the slot list goes up with the launch; ids and bearings are resident
+  e->h2d_bytes += size_t(n_frames) * sizeof(int32_t);
+  e->launches += ctvio::launch_keyframe_parallax(a, st);
+  ctvio::KeyframeResult r;
+  CUDA_OK(cudaMemcpyAsync(&r, e->d_kf_result.p, sizeof(r), cudaMemcpyDeviceToHost, st));
+  e->d2h_bytes += sizeof(r);
+  CUDA_OK(cudaStreamSynchronize(st));
+  *is_keyframe = r.is_keyframe;
+  if (n_tracked) *n_tracked = r.n_tracked;
+  if (parallax_num) *parallax_num = r.parallax_num;
+  if (parallax_sum) *parallax_sum = r.parallax_sum;
+  return CTVIO_OK;
+}
+
+int ctvio_slide_window_second_new(ctvio_handle e) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (e->nB < 2) return fail(CTVIO_ERR_STATE, "the window has fewer than 2 bias nodes");
+  const int gone = e->nB - 2;
+  // the prior is kept as it is (trajectory_manager.cpp:270-280), so none of its blocks may belong to the leaving node
+  for (size_t b = 0; b < e->prior.type.size(); ++b) {
+    const int t = e->prior.type[b];
+    if ((t == CTVIO_BLK_BG || t == CTVIO_BLK_BA) && e->prior.index[b] == gone)
+      return fail(CTVIO_ERR_STATE, "the active prior holds a block of the second-newest bias node");
+  }
+  cudaSetDevice(e->cfg.device);
+  // Bgs_/Bas_[WINDOW_SIZE - 1] = [WINDOW_SIZE] (visual_odometry.cpp:253-278); node nB-1 keeps its value and stands for the
+  // next image, as the node ctvio_slide_window appends does.  Knots, time origin and prior block indices do not move.
+  double* bias = e->x[e->cur].bias.p;
+  CUDA_OK(cudaMemcpyAsync(bias + 6 * size_t(gone), bias + 6 * size_t(gone + 1), 6 * sizeof(double), cudaMemcpyDeviceToDevice,
+                          e->stream));
+  e->mirror_valid = false;
   return CTVIO_OK;
 }
 

@@ -6,6 +6,9 @@
 //   triangulate_window_kernel  the same DLT for the landmarks of the resident window (AddImageToWindow,
 //                        visual_odometry.cpp:185-191), camera poses from the resident spline at each observation's row
 //                        time (the rolling-shutter variant triangulateRS, feature_manager.cpp:276-338, when ld > 0).
+//   keyframe_parallax_kernel  replaces FeatureManager::addFeatureCheckParallax (feature_manager.cpp:28-87) as
+//                        VisualOdometry::AddImageToWindow uses it (visual_odometry.cpp:180-183), on the resident frame
+//                        slots: tracked count of the new image and mean parallax between the two frames before it.
 //   unpack_cloud_kernel  replaces FeatureMsg2Image (visual_odometry/visual_struct.h:98-121) on the tracker's message
 //                        (visual_feature/feature_tracker_node.cpp:146-184): sensor_msgs::PointCloud arrives as packed
 //                        float32 triples + five float32 channels and is converted ON THE DEVICE into the resident
@@ -160,6 +163,100 @@ __global__ void __launch_bounds__(kTriThreads) triangulate_window_kernel(Triangu
   }
 }
 
+// ---- keyframe decision (addFeatureCheckParallax + compensatedParallax2, feature_manager.cpp:28-87 / :424-456) ------------
+// One CTA, one thread per feature index.  The (id, index) keys of the new slot and of slot fc-2 are sorted in shared
+// memory (bitonic, both arrays at once); the features of the other listed slots binary-search the new slot's keys and
+// mark the hits (an idempotent store), the features of slot fc-1 search slot fc-2's keys and store their parallax at
+// their own index.  The counts come from __syncthreads_count, the parallax sum from a fixed tree over the feature
+// indices: no atomics, bitwise reproducible.
+constexpr int kKfThreads = kKeyframeMaxFeatures;
+
+// sort key of (id, index): the signed id ordered as unsigned in the high word, the index in the low word
+__device__ __forceinline__ uint64_t kf_key(int32_t id, int i) {
+  return (uint64_t(uint32_t(id) ^ 0x80000000u) << 32) | uint32_t(i);
+}
+// index (in its slot) of the feature with this id among the n sorted keys, or -1
+__device__ __forceinline__ int kf_find(const uint64_t* keys, int n, int32_t id) {
+  const uint64_t lo = kf_key(id, 0);
+  int a = 0, b = n;  // first key >= lo
+  while (a < b) {
+    const int m = (a + b) >> 1;
+    if (keys[m] < lo) a = m + 1; else b = m;
+  }
+  return (a < n && (keys[a] >> 32) == (lo >> 32)) ? int(uint32_t(keys[a])) : -1;
+}
+
+__global__ void __launch_bounds__(kKfThreads) keyframe_parallax_kernel(KeyframeArgs a) {
+  __shared__ uint64_t s_key[2][kKeyframeMaxFeatures];  // [0]: the new slot, [1]: slot fc-2
+  __shared__ double s_par[kKeyframeMaxFeatures];       // parallax of feature i of slot fc-1 (0: not a parallax feature)
+  __shared__ uint8_t s_tracked[kKeyframeMaxFeatures];  // feature i of the new slot occurs in another listed slot
+  const int tid = threadIdx.x;
+  const int fc = a.n_frames - 1;  // frame_count
+  const int n_new = a.count[fc];
+  const int n_old = fc >= 2 ? a.count[fc - 2] : 0;
+  const FrameFeature* t_new = a.table + size_t(a.slot[fc]) * a.frame_cap;
+  const FrameFeature* t_old = fc >= 2 ? a.table + size_t(a.slot[fc - 2]) * a.frame_cap : nullptr;
+  s_key[0][tid] = tid < n_new ? kf_key(t_new[tid].id, tid) : ~0ull;
+  s_key[1][tid] = tid < n_old ? kf_key(t_old[tid].id, tid) : ~0ull;
+  s_par[tid] = 0.0;
+  s_tracked[tid] = 0;
+  __syncthreads();
+  // bitonic sort of both key arrays: threads [0, N/2) work on s_key[0], [N/2, N) on s_key[1]
+  {
+    constexpr int N = kKeyframeMaxFeatures;
+    uint64_t* keys = s_key[tid / (N / 2)];
+    const int p = tid % (N / 2);
+    for (int k = 2; k <= N; k <<= 1)
+      for (int j = k >> 1; j > 0; j >>= 1) {
+        const int i = 2 * j * (p / j) + p % j;
+        const uint64_t x = keys[i], y = keys[i + j];
+        if ((x > y) == ((i & k) == 0)) { keys[i] = y; keys[i + j] = x; }
+        __syncthreads();
+      }
+  }
+  // last_track_num (:38-57): the new image's features whose id is already in the window
+  for (int f = 0; f < fc; ++f) {
+    const FrameFeature* t = a.table + size_t(a.slot[f]) * a.frame_cap;
+    for (int i = tid; i < a.count[f]; i += kKfThreads) {
+      const int hit = kf_find(s_key[0], n_new, t[i].id);
+      if (hit >= 0) s_tracked[hit] = 1;
+    }
+  }
+  // parallax features (:62-72): start_frame <= fc-2 && endFrame() >= fc-1, i.e. seen in slots fc-2 and fc-1
+  bool parallax_feature = false;
+  if (fc >= 2 && tid < a.count[fc - 1]) {
+    const FrameFeature fj = a.table[size_t(a.slot[fc - 1]) * a.frame_cap + tid];
+    const int i = kf_find(s_key[1], n_old, fj.id);
+    if (i >= 0) {
+      // compensatedParallax2 (:424-456) with z == 1: the compensated and the plain distance coincide.  The products are
+      // rounded separately (no FMA) so that every per-feature value is the one a host restatement computes.
+      const FrameFeature fi = t_old[i];
+      const double du = fi.x - fj.x, dv = fi.y - fj.y;
+      s_par[tid] = sqrt(__dadd_rn(__dmul_rn(du, du), __dmul_rn(dv, dv)));
+      parallax_feature = true;
+    }
+  }
+  __syncthreads();
+  const int n_tracked = __syncthreads_count(tid < n_new && s_tracked[tid]);
+  const int parallax_num = __syncthreads_count(parallax_feature);
+  for (int stride = kKfThreads / 2; stride > 0; stride >>= 1) {
+    if (tid < stride) s_par[tid] += s_par[tid + stride];
+    __syncthreads();
+  }
+  if (tid == 0) {
+    const double sum = s_par[0];
+    KeyframeResult r;
+    r.n_tracked = n_tracked;
+    r.parallax_num = parallax_num;
+    r.parallax_sum = sum;
+    r.pad = 0;
+    // :59-60 and :74-86
+    if (fc < 2 || n_tracked < 20 || parallax_num == 0) r.is_keyframe = 1;
+    else r.is_keyframe = sum / parallax_num >= a.min_parallax;
+    *a.out = r;
+  }
+}
+
 // ---- wire formats -> resident tables ----------------------------------------------------------------
 
 __global__ void unpack_cloud_kernel(UnpackCloudArgs a) {
@@ -296,6 +393,10 @@ int launch_triangulate(const TriangulateArgs& a, cudaStream_t s) {
 int launch_triangulate_window(const TriangulateWindowArgs& a, cudaStream_t s) {
   if (a.n_landmarks <= 0) return 0;
   triangulate_window_kernel<<<(a.n_landmarks + kTriLmPerCta - 1) / kTriLmPerCta, kTriThreads, 0, s>>>(a);
+  return 1;
+}
+int launch_keyframe_parallax(const KeyframeArgs& a, cudaStream_t s) {
+  keyframe_parallax_kernel<<<1, kKfThreads, 0, s>>>(a);
   return 1;
 }
 int launch_unpack_cloud(const UnpackCloudArgs& a, cudaStream_t s) {

@@ -1,6 +1,6 @@
 // Front-end data formats either side of the hot path (frontend.cu): DLT triangulation (from caller poses, and of the
-// resident window from the resident spline), wire-format unpacking, device-side construction of the sorted image-factor
-// arrays from the resident per-frame feature tables.
+// resident window from the resident spline), the keyframe decision over the resident frame slots, wire-format unpacking,
+// device-side construction of the sorted image-factor arrays from the resident per-frame feature tables.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -93,6 +93,28 @@ struct TriangulateWindowArgs {
   int32_t* counts;            // [2] zeroed by the caller: {triangulated, fallback}; sign bit of [0] = a time left the spline
 };
 int launch_triangulate_window(const TriangulateWindowArgs& a, cudaStream_t s);
+
+// Keyframe decision of the new image (addFeatureCheckParallax, feature_manager.cpp:28-87) over resident frame slots:
+// slot[0 .. n_frames-1] lists the window oldest to newest, the last one the new image.  One CTA of
+// kKeyframeMaxFeatures threads; every slot holds at most kKeyframeMaxFeatures features.
+constexpr int kKeyframeMaxSlots = 16, kKeyframeMaxFeatures = 1024;
+struct KeyframeResult {
+  int32_t is_keyframe;
+  int32_t n_tracked;     // features of the new slot whose id occurs in another listed slot (last_track_num)
+  int32_t parallax_num;  // features of slot fc-1 whose id occurs in slot fc-2 (0 when fc < 2)
+  int32_t pad;
+  double parallax_sum;   // sum of their bearing distances, summed in a fixed order
+};
+struct KeyframeArgs {
+  const FrameFeature* table;  // [n_slots][frame_cap]
+  int32_t frame_cap;
+  int32_t n_frames;           // 1 .. kKeyframeMaxSlots
+  int32_t slot[kKeyframeMaxSlots];
+  int32_t count[kKeyframeMaxSlots];  // features ingested in slot[k] (<= kKeyframeMaxFeatures)
+  double min_parallax;        // MIN_PARALLAX
+  KeyframeResult* out;
+};
+int launch_keyframe_parallax(const KeyframeArgs& a, cudaStream_t s);
 
 // device-resident window bookkeeping (all on the device)
 int launch_extend_knots(const StatePtrs& st, int old_n, int new_n, cudaStream_t s);

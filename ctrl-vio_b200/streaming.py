@@ -53,14 +53,19 @@ class StreamingRunner:
     oracle) -- used by the sensitivity tests; the window problem is mathematically unchanged.
     second_new_every: every N-th frame is treated as a non-keyframe: when it is the second-newest frame of the window
     the step takes the MARGIN_SECOND_NEW branch (no marginalization, the frame is dropped instead of the oldest).
+    min_parallax: when set, the branch of every step (the first one included) comes from the features instead:
+    keyframe_decision over the window's tracker messages (the reference's addFeatureCheckParallax), MARGIN_OLD for a
+    keyframe.  The record then also carries n_tracked and mean_parallax (None without parallax features).
     """
 
     def __init__(self, lib, seq: "syn.Window", iters=15, init_iters=8, device=0, second_new_every=0, perm_seed=None,
-                 predictor=True):
+                 predictor=True, min_parallax=None):
         from . import make_config, make_options
         self.lib, self.seq, self.iters, self.init_iters = lib, seq, iters, init_iters
         self.predictor = predictor
         self.second_new_every = second_new_every
+        self.min_parallax = min_parallax
+        self.clouds = FrameClouds(seq) if min_parallax is not None else None
         self.rng = None if perm_seed is None else np.random.default_rng(perm_seed)
         s = seq
         self.frames = list(range(WIN_KF))                       # source keyframe ids in the window
@@ -92,6 +97,15 @@ class StreamingRunner:
 
     def _perm(self, n):
         return np.arange(n) if self.rng is None else self.rng.permutation(n)
+
+    def _second_new_rule(self):
+        """the second_new_every rule: MARGIN_SECOND_NEW when the second-newest frame is an N-th frame"""
+        n = self.second_new_every
+        return MARGIN_SECOND_NEW if n and (self.frames[-2] % n) == n - 1 else MARGIN_OLD
+
+    @staticmethod
+    def _decision_record(n_tracked, parallax_num, parallax_sum):
+        return dict(n_tracked=n_tracked, mean_parallax=parallax_sum / parallax_num if parallax_num else None)
 
     # -- prior re-indexing (index identity <-> window-relative indices) -----------------------------
     def _prior_to_window(self, ks, frames, lm_global):
@@ -153,9 +167,14 @@ class StreamingRunner:
         ks = self._knot_of(int(kf[0]))                # min_idx of UpdateTrajectory = first control point of the window
         nloc = self.ncp - ks
         nowk, later = 0, self._knot_of(int(kf[1])) - ks
-        marg_flag = MARGIN_OLD
-        if self.second_new_every and (self.frames[-2] % self.second_new_every) == self.second_new_every - 1:
-            marg_flag = MARGIN_SECOND_NEW
+        decision = None
+        if self.min_parallax is not None:
+            # the feature manager's keyframe decision (visual_odometry.cpp:180-183), over the tracker's messages
+            is_kf, n_tracked, num, psum = keyframe_decision([self.clouds.message(f) for f in self.frames], self.min_parallax)
+            marg_flag = MARGIN_OLD if is_kf else MARGIN_SECOND_NEW
+            decision = self._decision_record(n_tracked, num, psum)
+        else:
+            marg_flag = self._second_new_rule()
 
         # ---- host-side "tracker / feature manager": slice the sequence (not timed) ----
         w = syn.subwindow_frames(s, frames, imu_max_ns=min(max_t, t_newest + 1), window_size=WINDOW_SIZE)
@@ -249,6 +268,8 @@ class StreamingRunner:
                    init_n_imu=0 if init_sel is None else len(init_sel),
                    init_device_ms=0.0 if init_summary is None else init_summary.device_ms,
                    prior_dim=0 if self.prior is None else self.prior.n, h2d_bytes=h2d, d2h_bytes=d2h)
+        if decision is not None:
+            rec.update(decision)
         self.records.append(rec)
         self.step_index += 1
         return rec
@@ -352,11 +373,50 @@ class FrameClouds:
         return pts, ids, (syn.FX * xy[:, 0] + syn.U0).astype(np.float32) if hasattr(syn, "FX") else z, row.astype(np.float32), z, z
 
 
+def keyframe_decision(messages, min_parallax):
+    """FeatureManager::addFeatureCheckParallax + compensatedParallax2 (feature_manager.cpp:28-87, :424-456) over the
+    window's tracker messages (FrameClouds.message tuples), oldest to newest, the new image last: the host-buffer
+    path's feature manager and the reference of ctvio_check_keyframe.  Ids and bearings are read as the wire carries
+    them (float32; id = int(id + 0.5) as FeatureMsg2Image), ids are unique within a message.
+    Returns (is_keyframe, n_tracked, parallax_num, parallax_sum):
+      n_tracked     features of the new image whose id occurs in any other message (last_track_num);
+      parallax_num  features of message fc-1 whose id also occurs in message fc-2 (fc = len(messages) - 1), 0 if fc < 2;
+      parallax_sum  the sum of their bearing distances sqrt(du^2 + dv^2) (z == 1: compensated == plain);
+      is_keyframe   fc < 2, n_tracked < 20 or no parallax feature, else parallax_sum / parallax_num >= min_parallax."""
+    fc = len(messages) - 1
+    ids = [(np.asarray(m[1], np.float32).astype(np.float64) + 0.5).astype(np.int64) for m in messages]
+    others = np.concatenate(ids[:fc]) if fc > 0 else np.zeros(0, np.int64)
+    n_tracked = int(np.isin(ids[fc], others).sum())
+    parallax_num, parallax_sum = 0, 0.0
+    if fc >= 2:
+        id_i, id_j = ids[fc - 2], ids[fc - 1]
+        xy_i = np.asarray(messages[fc - 2][0], np.float32)[:, :2].astype(np.float64)
+        xy_j = np.asarray(messages[fc - 1][0], np.float32)[:, :2].astype(np.float64)
+        order = np.argsort(id_i, kind="stable")
+        pos = np.clip(np.searchsorted(id_i[order], id_j), 0, max(len(id_i) - 1, 0))
+        hit = (id_i[order][pos] == id_j) if len(id_i) else np.zeros(len(id_j), bool)
+        i = order[pos[hit]]
+        du = xy_i[i, 0] - xy_j[hit, 0]
+        dv = xy_i[i, 1] - xy_j[hit, 1]
+        parallax_num = int(hit.sum())
+        parallax_sum = float(np.sum(np.sqrt(du * du + dv * dv)))
+    if fc < 2 or n_tracked < 20 or parallax_num == 0:
+        return True, n_tracked, parallax_num, parallax_sum
+    return bool(parallax_sum / parallax_num >= min_parallax), n_tracked, parallax_num, parallax_sum
+
+
 class ResidentRunner(StreamingRunner):
     """The same per-image cycle with the window living in HBM: the new image's PointCloud and the new IMUData records go
     up as they are, control points are extended / dropped on the device, inverse depths are re-indexed on the device,
     the prior is handed over device-to-device, and the factor payload is gathered from the resident tables (only index
-    tables cross the boundary).  MARGIN_OLD only (every frame a keyframe, the C5 configuration).
+    tables cross the boundary).
+
+    Both branches of the reference's slide: by default every frame is a keyframe (MARGIN_OLD, the C5 configuration);
+    second_new_every takes the base class's rule; min_parallax takes the decision on the device (CheckKeyframe over the
+    window's frame slots, right after the new cloud is ingested).  MARGIN_SECOND_NEW solves without marginalization
+    flags, keeps the prior and drops the second-newest frame (SlideWindowSecondNew).  Frame slots come from a small
+    allocator (a window that skipped frames can span more than 16 source frames): frame f takes slot f % 16 when that
+    slot is free, else the lowest free one, so a MARGIN_OLD-only run uses exactly the slots f % 16.
 
     triangulate=True: new landmarks enter with inverse depth -1 and get their initial depth from TriangulateWindow (the
     reference's FeatureManager::triangulate in AddImageToWindow, visual_odometry.cpp:185-191) on the device, after the
@@ -367,16 +427,27 @@ class ResidentRunner(StreamingRunner):
     TriangulateWindow, on the engine state the call used."""
 
     def __init__(self, lib, seq, triangulate=False, **kw):
-        assert not kw.get("second_new_every"), "the resident runner implements the MARGIN_OLD slide only"
         super().__init__(lib, seq, **kw)
         self.triangulate = triangulate
         self.triangulate_probe = None
-        self.clouds = FrameClouds(seq)
+        if self.clouds is None:
+            self.clouds = FrameClouds(seq)
         self.n_slots = 16
+        self.slot_of = {}          # source frame -> frame slot, for the frames in the engine's table
         self.imu_sent = 0          # samples of the source sequence already ingested
         self.prev_lm_global = None
         self.prev_ks = None
         self.readback = None
+        self.prior_dim = 0         # dimension of the engine's active prior
+
+    def _assign_slot(self, f):
+        """frame slot of a new frame: f % n_slots when free, else the lowest free slot"""
+        used = set(self.slot_of.values())
+        s = f % self.n_slots
+        if s in used:
+            s = min(set(range(self.n_slots)) - used)
+        self.slot_of[f] = s
+        return s
 
     def _imu_records(self, lo, hi):
         s = self.seq
@@ -395,19 +466,31 @@ class ResidentRunner(StreamingRunner):
             e.SetTimeOrigin(s.t0_ns)
             e.SetKnots(self.q[:self.ncp], self.p[:self.ncp]); e.SetBiases(self.bias[self.frames]); e.SetLineDelay(self.ld)
             for f in self.frames:
-                e.IngestFeatureCloud(f % self.n_slots, int(s.kf_times[f]), *self.clouds.message(f))
+                e.IngestFeatureCloud(self._assign_slot(f), int(s.kf_times[f]), *self.clouds.message(f))
             self.base_knot = 0      # global index of the engine's knot 0
         else:
             self.frames.append(self.next_frame)
+            self._assign_slot(self.next_frame)
             self.next_frame += 1
         frames = np.asarray(self.frames, np.int64)
+        frame_slots = np.array([self.slot_of[f] for f in self.frames], np.int32)   # window position -> frame slot
         kf = s.kf_times[frames]
         t_newest = int(kf[-1])
         t0 = time.perf_counter()
         max_bef_ns = max_bef_idx = None
         if not first:
             f = self.frames[-1]
-            e.IngestFeatureCloud(f % self.n_slots, t_newest, *self.clouds.message(f))
+            e.IngestFeatureCloud(int(frame_slots[-1]), t_newest, *self.clouds.message(f))
+        decision = None
+        if self.min_parallax is not None:
+            # addFeatureCheckParallax on the device, over the clouds already in the frame table
+            is_kf, n_tracked, num, psum = e.CheckKeyframe(frame_slots, self.min_parallax)
+            marg_flag = MARGIN_OLD if is_kf else MARGIN_SECOND_NEW
+            decision = self._decision_record(n_tracked, num, psum)
+        else:
+            marg_flag = self._second_new_rule()
+        marg = marg_flag == MARGIN_OLD
+        if not first:
             max_bef_ns = s.t0_ns + (self.ncp - 3) * s.dt_ns
             max_bef_idx = self.ncp - 1
             self.ncp = e.ExtendKnotsTo(t_newest + EXTEND_NS) + self.base_knot
@@ -436,15 +519,17 @@ class ResidentRunner(StreamingRunner):
         init_rho = np.full(len(lm_global), -1.0) if self.triangulate else s.rho0[lm_global]
         img_marg = (w.anchor_frame[w.lm] == 0).astype(np.int32)  # (inverse depths are positive in the synthetic sequences)
         bias_marg = np.zeros(len(w.bf_i), np.int32); bias_marg[0] = 1
+        if not marg:
+            img_marg[:] = 0; bias_marg[:] = 0
         # factor -> (frame slot, index in that frame's cloud) of its two observations
         sel = self._factor_selection(frames, lm_global)
         g_lm = lm_global[w.lm]
-        slot_i = (frames[w.anchor_frame[w.lm]] % self.n_slots).astype(np.int32)
+        slot_i = frame_slots[w.anchor_frame[w.lm]]
         idx_i = self.clouds.anchor_idx[g_lm]
-        slot_j = (frames[w.obs_frame] % self.n_slots).astype(np.int32)
+        slot_j = frame_slots[w.obs_frame]
         idx_j = self.clouds.obs_idx[sel]
         if self.triangulate:
-            tri_csr = self._observation_csr(frames, w, lm_global, slot_j, idx_j)
+            tri_csr = self._observation_csr(frames, w, lm_global, slot_j, idx_j, frame_slots)
         R0 = t0_ = None
         if self.readback is not None:
             qn, pn = self.readback[0][ks - self.prev_ks], self.readback[1][ks - self.prev_ks]
@@ -472,60 +557,74 @@ class ResidentRunner(StreamingRunner):
             n_tri, n_fb = e.TriangulateWindow(*tri_csr)
             if self.triangulate_probe is not None:
                 self.triangulate_probe(self, *tri_csr, rho_before)
-        e.SetOptions(self._make_options(fix_ld=False, ld_lower=0.0, ld_upper=syn.LD_UPPER, is_marg_state=True,
+        e.SetOptions(self._make_options(fix_ld=False, ld_lower=0.0, ld_upper=syn.LD_UPPER, is_marg_state=marg,
                                         ctrl_to_be_opt_now=nowk, ctrl_to_be_opt_later=later))
         e.ClearFactors()
         e.EnablePrior(True)
         e.AddImageFeaturesFromSlots(slot_i, idx_i, slot_j, idx_j, w.lm, img_marg)
         opt_min = s.t0_ns + ks * s.dt_ns
-        e.AddImuFromTable(opt_min, min(max_t, t_newest + 1), kf_times=kf, marg_before_ns=int(kf[1]))
+        if marg:
+            e.AddImuFromTable(opt_min, min(max_t, t_newest + 1), kf_times=kf, marg_before_ns=int(kf[1]))
+        else:
+            e.AddImuFromTable(opt_min, min(max_t, t_newest + 1), kf_times=kf)
         e.AddBiasFactor(w.bf_i, w.bf_j, w.bf_sqrt_info, bias_marg)
         t_built = time.perf_counter()
         summ = e.Solve(self.iters)
         t_solved = time.perf_counter()
         e.GaugeRealign(nowk, R0, t0_)
-        n_out = C_int32(); nb_out = C_int32()
-        e.lib.call("marginalize", e.h, byref(n_out), byref(nb_out))
-        if n_out.value > 0:
-            e.AdoptPrior()           # device-to-device
+        if marg:
+            n_out = C_int32(); nb_out = C_int32()
+            e.lib.call("marginalize", e.h, byref(n_out), byref(nb_out))
+            if n_out.value > 0:
+                e.AdoptPrior()           # device-to-device
+            self.prior_dim = n_out.value
         t_marged = time.perf_counter()
         qs, ps = e.GetKnots(); ld = e.GetLineDelay()   # the trajectory is the product the caller publishes
-        drop_knots = later
-        e.SlideWindow(drop_knots, 1, 1)                # slideWindowOld: oldest frame's control points and bias node leave
+        if marg:
+            drop_knots = later
+            e.SlideWindow(drop_knots, 1, 1)            # slideWindowOld: oldest frame's control points and bias node leave
+        else:
+            drop_knots = 0
+            e.SlideWindowSecondNew()                   # slideWindowNew: the second-newest frame leaves, the prior stays
         t_wall = time.perf_counter() - t_start
         h2d, d2h = (0, 0) if first else e.TransferStats(reset=True)
 
+        del self.slot_of[self.frames.pop(0 if marg else -2)]
         self.q[ks:self.ncp] = qs; self.p[ks:self.ncp] = ps
         self.ld = ld
         self.readback, self.prev_ks, self.prev_lm_global = (qs, ps), ks, lm_global
         self.base_knot = ks + drop_knots
-        self.frames.pop(0)
         rec = dict(window=self.step_index, ms=1e3 * (t_wall + t_push), prior_const=0.0,
                    ms_build_and_predict=1e3 * (t_built - t_start + t_push), ms_solve=1e3 * (t_solved - t_built),
                    ms_realign_marginalize=1e3 * (t_marged - t_solved), ms_readback=1e3 * (t_start + t_wall - t_marged),
                    iterations=summ.iterations, final_cost=summ.final_cost, initial_cost=summ.initial_cost,
                    termination=summ.termination, n_obs=w.n_obs, n_imu=len(w.imu_t), n_knots=nloc, n_lm=len(lm_global),
-                   device_ms=summ.device_ms, marg_flag=MARGIN_OLD,
+                   device_ms=summ.device_ms, marg_flag=marg_flag,
                    init_iterations=None if init_summary is None else init_summary.iterations, init_n_imu=0,
-                   init_device_ms=0.0 if init_summary is None else init_summary.device_ms, prior_dim=n_out.value,
+                   init_device_ms=0.0 if init_summary is None else init_summary.device_ms, prior_dim=self.prior_dim,
                    h2d_bytes=h2d, d2h_bytes=d2h)
+        if decision is not None:
+            rec.update(decision)
         if self.triangulate:
             rec.update(n_triangulated=n_tri, n_fallback=n_fb, n_new_lm=int(np.sum(old_index < 0)))
         self.records.append(rec)
         self.step_index += 1
         return rec
 
-    def _observation_csr(self, frames, w, lm_global, slot_j, idx_j):
+    def _observation_csr(self, frames, w, lm_global, slot_j, idx_j, frame_slots=None):
         """(obs_offset, obs_slot, obs_idx) of TriangulateWindow: per window landmark its anchor, then its observations
-        in frame order (the factors are landmark-major and frame-ordered within a landmark)."""
+        in frame order (the factors are landmark-major and frame-ordered within a landmark).  frame_slots: the frame
+        slot of each window position (default: frame % n_slots, the slots of a MARGIN_OLD-only run)."""
         assert np.all(np.diff(w.lm) >= 0)
+        if frame_slots is None:
+            frame_slots = frames % self.n_slots
         n_lm = len(lm_global)
         counts = np.bincount(w.lm, minlength=n_lm)
         obs_offset = np.concatenate([[0], np.cumsum(counts + 1)]).astype(np.int32)
         first_factor = np.cumsum(counts) - counts
         obs_slot = np.empty(obs_offset[-1], np.int32)
         obs_idx = np.empty(obs_offset[-1], np.int32)
-        obs_slot[obs_offset[:-1]] = frames[w.anchor_frame] % self.n_slots
+        obs_slot[obs_offset[:-1]] = frame_slots[w.anchor_frame]
         obs_idx[obs_offset[:-1]] = self.clouds.anchor_idx[lm_global]
         pos = obs_offset[w.lm] + 1 + np.arange(len(w.lm)) - first_factor[w.lm]
         obs_slot[pos] = slot_j

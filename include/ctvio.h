@@ -242,6 +242,35 @@ int ctvio_extend_knots_to(ctvio_handle h, int64_t t_ns, int32_t* n_knots_out);
  * n_drop_bias bias nodes leave the window (device-side shift, time origin advanced), n_new_bias nodes are appended as
  * copies of the newest one (Bgs_/Bas_[WINDOW_SIZE]); the ACTIVE prior's knot / bias block indices are re-based. */
 int ctvio_slide_window(ctvio_handle h, int32_t n_drop_knots, int32_t n_drop_bias, int32_t n_new_bias);
+/* replaces the MARGIN_SECOND_NEW half of VisualOdometry::SlideWindow (visual_odometry.cpp:253-278): bias node nB-2 takes
+ * the value of node nB-1 (Bgs_/Bas_[WINDOW_SIZE-1] = [WINDOW_SIZE]); node nB-1 keeps its value and stands for the next
+ * image.  Knots, time origin and prior are untouched; prior blocks keep their indices.  Use it after a solve without
+ * marginalization (no ctvio_marginalize / ctvio_adopt_prior), when ctvio_check_keyframe decided against the image
+ * before the new one.
+ *   Errors: CTVIO_ERR_STATE with fewer than 2 bias nodes, or when the active prior holds a block of bias node nB-2 -
+ *   nothing changes then. */
+int ctvio_slide_window_second_new(ctvio_handle h);
+/* replaces FeatureManager::addFeatureCheckParallax as VisualOdometry::AddImageToWindow uses it
+ * (feature_manager.cpp:28-87, visual_odometry.cpp:180-183) on the resident frame table: no knots or state are needed,
+ * only clouds ingested with ctvio_ingest_feature_cloud.
+ *   frame_slots[0 .. n_frames-1] lists the window's slots oldest to newest, the last one the new image; fc = n_frames-1
+ *   is the reference's frame_count.  An empty cloud is a valid slot.
+ *   n_tracked (last_track_num): features of the new slot whose id occurs in any other listed slot.
+ *   parallax_num / parallax_sum: the features of slot fc-1 whose id also occurs in slot fc-2 (tracks are contiguous in
+ *   window positions, so this is start_frame <= fc-2 && endFrame() >= fc-1), and the sum of their parallaxes
+ *   sqrt(du^2 + dv^2) between the two bearings (compensatedParallax2, :424-456; with z == 1 the compensated and the plain
+ *   term coincide).  Both are 0 when fc < 2; they are computed whenever fc >= 2, also when n_tracked < 20.
+ *   is_keyframe = 1 when fc < 2, n_tracked < 20 or parallax_num == 0, else parallax_sum / parallax_num >= min_parallax
+ *   (MIN_PARALLAX, focal-length normalised).  0 means MARGIN_SECOND_NEW.
+ *   Contract: ids are unique within a cloud, as the tracker guarantees.
+ *   Difference from the reference: its feature list also forgets landmarks removed by removeFailures (depth < 0); here
+ *   membership is only "the id occurs in a listed slot".
+ *   Outputs other than is_keyframe may be NULL.  The sum runs in a fixed order: bitwise reproducible.  One kernel launch,
+ *   the slot list up, one 24-byte result back, one stream synchronisation.
+ *   Errors: CTVIO_ERR_INVALID for n_frames outside 1..16, a slot outside 0..15, a slot listed twice, or a min_parallax
+ *   that is negative or not finite. */
+int ctvio_check_keyframe(ctvio_handle h, int32_t n_frames, const int32_t* frame_slots, double min_parallax,
+                         int32_t* is_keyframe, int32_t* n_tracked, int32_t* parallax_num, double* parallax_sum);
 /* replaces FeatureManager::getDepthVector / setDepth re-indexing (visual_odometry/feature_manager.cpp:139-170): landmark l
  * of the new window takes the inverse depth of old landmark old_index[l] (>= 0), else init_inv_depth[l]. */
 int ctvio_remap_landmarks(ctvio_handle h, int32_t n_landmarks, const int32_t* old_index, const double* init_inv_depth);
