@@ -104,6 +104,8 @@ ABI_SYMBOLS = [
     "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior", "ingest_feature_cloud", "add_image_features_from_slots",
     "ingest_imu", "add_imu_from_table", "transfer_stats", "profile_kernels", "measure_fp64_tflops", "measure_fp64_tensor_tflops",
     "selfcheck_solver", "nccl_unique_id", "comm_init", "triangulate_window", "check_keyframe", "slide_window_second_new",
+    "feature_table_add", "feature_table_window", "triangulate_window_from_table", "add_image_features_from_table",
+    "feature_table_slide", "feature_table_landmarks",
 ]
 
 
@@ -112,7 +114,8 @@ ABI_SYMBOLS = [
 DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enable_prior", "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior",
                        "ingest_feature_cloud", "add_image_features_from_slots", "ingest_imu", "add_imu_from_table",
                        "transfer_stats", "residual_summary", "triangulate_window", "check_keyframe",
-                       "slide_window_second_new")
+                       "slide_window_second_new", "feature_table_add", "feature_table_window", "triangulate_window_from_table",
+                       "add_image_features_from_table", "feature_table_slide", "feature_table_landmarks")
 
 
 def _addr(a):
@@ -451,6 +454,50 @@ class Estimator:
         self.lib.call("triangulate_window", self.h, C.c_int32(max(obs_offset.shape[0] - 1, 0)), _ip(obs_offset), _ip(obs_slot),
                       _ip(obs_idx), C.c_double(init_depth), C.byref(nt), C.byref(nf))
         return nt.value, nf.value
+
+    # --- resident feature table (FeatureManager's feature list on the device) --------------------------------
+    def FeatureTableAdd(self, frame_slot):
+        """addFeatureCheckParallax's insertion (feature_manager.cpp:28-59) for the cloud ingested into frame_slot.
+        Returns (n_tracked, n_new)."""
+        nt, nn = C.c_int32(), C.c_int32()
+        self.lib.call("feature_table_add", self.h, C.c_int32(frame_slot), C.byref(nt), C.byref(nn))
+        return nt.value, nn.value
+
+    def FeatureTableWindow(self, frame_slots, window_size):
+        """setDepth + getDepthVector's numbering over the window's frame slots, oldest to newest; re-lays out the resident
+        inverse depths to it.  Returns n_landmarks."""
+        slots = _i32(frame_slots)
+        n = C.c_int32()
+        self.lib.call("feature_table_window", self.h, C.c_int32(slots.shape[0]), _ip(slots), C.c_int32(window_size),
+                      C.byref(n))
+        self.n_lm = n.value
+        return n.value
+
+    def TriangulateWindowFromTable(self, init_depth=5.0):
+        """TriangulateWindow over the last FeatureTableWindow's landmarks.  Returns (n_triangulated, n_fallback)."""
+        nt, nf = C.c_int32(), C.c_int32()
+        self.lib.call("triangulate_window_from_table", self.h, C.c_double(init_depth), C.byref(nt), C.byref(nf))
+        return nt.value, nf.value
+
+    def AddImageFeaturesFromTable(self, marg_oldest):
+        """one image factor per (landmark, non-anchor observation) of the last window.  Returns n_factors."""
+        n = C.c_int32()
+        self.lib.call("add_image_features_from_table", self.h, C.c_int32(int(marg_oldest)), C.byref(n))
+        self.n_img += n.value
+        return n.value
+
+    def FeatureTableSlide(self, frame_slot):
+        """removeFailures, then the leaving slot's landmarks and observations leave.  Returns n_removed."""
+        n = C.c_int32()
+        self.lib.call("feature_table_slide", self.h, C.c_int32(frame_slot), C.byref(n))
+        return n.value
+
+    def FeatureTableLandmarks(self, n_landmarks=None):
+        """(feature id, anchor slot, used_num) of each landmark of the last window"""
+        n = self.n_lm if n_landmarks is None else n_landmarks
+        ids, anchor, used = (np.zeros(max(n, 0), np.int32) for _ in range(3))
+        self.lib.call("feature_table_landmarks", self.h, C.c_int32(n), _ip(ids), _ip(anchor), _ip(used))
+        return ids, anchor, used
 
     def IngestImu(self, records: np.ndarray, off_gyro, off_accel, drop_before_ns=0):
         """packed IMUData records (structured / byte array, one record per row)."""

@@ -237,6 +237,24 @@ struct ctvio_engine {
   DevBuf<int32_t> d_tri_idx;  // index uploads: ctvio_triangulate, ctvio_remap_landmarks, ctvio_triangulate_window
   DevBuf<int32_t> d_tri_cnt;  // ctvio_triangulate_window: {triangulated, fallback}
   DevBuf<ctvio::KeyframeResult> d_kf_result;  // ctvio_check_keyframe
+  uint32_t h_frame_ingested = 0;  // frame slots holding a cloud from ctvio_ingest_feature_cloud (cleared when the table slides it)
+  // resident feature table (ctvio_feature_table_*), allocated at full size on first use
+  struct FeatureTable {
+    DevBuf<int32_t> id, anchor, lm, idx, new_index;
+    DevBuf<uint32_t> mask;
+    DevBuf<double> rho;
+    DevBuf<uint64_t> key[2];  // sorted (id, entry) keys, ping-pong
+    int cur_key = 0;
+    DevBuf<int32_t> obs_offset, obs_slot, obs_idx, lm_id, lm_anchor, lm_used, result;
+    DevBuf<ctvio::FactorDesc> desc;
+    int n_entries = 0;
+    uint32_t held = 0;            // frame slots whose cloud the table holds
+    int n_lm = -1;                // landmarks of the last window (-1: none yet); the resident inverse depths follow it
+    int n_obs = 0;
+    bool window_current = false;  // the CSR and records describe the table as it is (no add / slide since the window)
+    int32_t oldest_slot = 0;
+    ctvio::FeatureTablePtrs ptrs() { return ctvio::FeatureTablePtrs{id.p, anchor.p, mask.p, lm.p, rho.p, idx.p}; }
+  } ft;
   // marginalization workspace (K7), kept across windows: allocation / free costs more than the kernels
   struct MargWs {
     DevBuf<int32_t> pos_cam, pos_lm, prior_pos, marg_img, marg_imu;
@@ -959,6 +977,55 @@ int alloc_state(ctvio_engine* e, DevState& s) {
   CUDA_OK(s.bias.reserve(6 * size_t(std::max(e->nB, 1))));
   CUDA_OK(s.rho.reserve(size_t(std::max(e->nL, 1))));
   CUDA_OK(s.ld.reserve(1));
+  return CTVIO_OK;
+}
+
+// DLT of the resident window (ctvio_triangulate_window, ctvio_triangulate_window_from_table) from a device-resident
+// observation CSR
+int triangulate_window_device(ctvio_engine* e, int nl, const int32_t* d_off, const int32_t* d_slot, const int32_t* d_idx,
+                              double init_depth, int32_t* n_triangulated, int32_t* n_fallback) {
+  cudaStream_t st = e->stream;
+  ensure_table(e);
+  const int other = e->cur ^ 1;
+  CUDA_OK(e->x[other].rho.reserve(size_t(nl) + 1));
+  CUDA_OK(e->d_tri_cnt.reserve(2));
+  CUDA_OK(cudaMemsetAsync(e->d_tri_cnt.p, 0, 2 * sizeof(int32_t), st));
+  ctvio::TriangulateWindowArgs a;
+  a.n_landmarks = nl; a.obs_offset = d_off; a.obs_slot = d_slot; a.obs_idx = d_idx;
+  a.table = e->d_frames.p; a.frame_t = e->d_frame_t.p; a.frame_cap = ctvio_engine::kFrameCap;
+  a.st = e->x[e->cur].ptrs(); a.sp = e->sp; a.R_CI = e->rig.R_CI; a.p_CI = e->rig.p_CI;
+  a.init_depth = init_depth;
+  // written into the other state buffer's array and swapped in only on success: after CTVIO_ERR_TIME_RANGE the
+  // resident inverse depths are the ones before the call
+  a.rho_in = e->x[e->cur].rho.p; a.rho_out = e->x[other].rho.p;
+  a.counts = e->d_tri_cnt.p;
+  e->launches += ctvio::launch_triangulate_window(a, st);
+  int32_t cnt[2];
+  CUDA_OK(cudaMemcpyAsync(cnt, e->d_tri_cnt.p, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+  e->d2h_bytes += sizeof(cnt);
+  CUDA_OK(cudaStreamSynchronize(st));
+  if (cnt[0] < 0) return fail(CTVIO_ERR_TIME_RANGE, "an observation's row time falls outside the spline");
+  std::swap(e->x[e->cur].rho.p, e->x[other].rho.p);
+  std::swap(e->x[e->cur].rho.cap, e->x[other].rho.cap);
+  e->mirror_valid = false;
+  if (n_triangulated) *n_triangulated = cnt[0];
+  if (n_fallback) *n_fallback = cnt[1];
+  return CTVIO_OK;
+}
+
+// the resident feature table's arrays, at full size (kFeatureTableMaxEntries entries), on first use
+int ensure_feature_table(ctvio_engine* e) {
+  auto& t = e->ft;
+  if (t.id.p) return CTVIO_OK;
+  const size_t cap = ctvio::kFeatureTableMaxEntries, slots = ctvio_engine::kFrameSlots;
+  CUDA_OK(e->d_frames.reserve(slots * ctvio_engine::kFrameCap));
+  CUDA_OK(t.id.reserve(cap)); CUDA_OK(t.anchor.reserve(cap)); CUDA_OK(t.lm.reserve(cap)); CUDA_OK(t.mask.reserve(cap));
+  CUDA_OK(t.rho.reserve(cap)); CUDA_OK(t.idx.reserve(slots * cap)); CUDA_OK(t.new_index.reserve(cap));
+  CUDA_OK(t.key[0].reserve(cap)); CUDA_OK(t.key[1].reserve(cap));
+  CUDA_OK(t.obs_offset.reserve(cap + 1)); CUDA_OK(t.obs_slot.reserve(slots * cap)); CUDA_OK(t.obs_idx.reserve(slots * cap));
+  CUDA_OK(t.lm_id.reserve(cap)); CUDA_OK(t.lm_anchor.reserve(cap)); CUDA_OK(t.lm_used.reserve(cap));
+  CUDA_OK(t.result.reserve(2));
+  CUDA_OK(t.desc.reserve((slots - 1) * cap));
   return CTVIO_OK;
 }
 
@@ -2437,11 +2504,7 @@ int ctvio_triangulate_window(ctvio_handle e, int32_t nl, const int32_t* obs_offs
   cudaSetDevice(e->cfg.device);
   ArenaScope arena(e);
   cudaStream_t st = e->stream;
-  ensure_table(e);
-  const int other = e->cur ^ 1;
-  CUDA_OK(e->x[other].rho.reserve(size_t(nl) + 1));
   CUDA_OK(e->d_tri_idx.reserve(size_t(nl) + 1 + 2 * size_t(total)));
-  CUDA_OK(e->d_tri_cnt.reserve(2));
   int32_t* d_off = e->d_tri_idx.p;
   int32_t* d_slot = d_off + nl + 1;
   int32_t* d_idx = d_slot + total;
@@ -2450,27 +2513,182 @@ int ctvio_triangulate_window(ctvio_handle e, int32_t nl, const int32_t* obs_offs
   CUDA_OK(staged_h2d(d_slot, obs_slot, size_t(total) * sizeof(int32_t), st));
   CUDA_OK(staged_h2d(d_idx, obs_idx, size_t(total) * sizeof(int32_t), st));
   e->h2d_bytes += (size_t(nl) + 1 + 2 * size_t(total)) * sizeof(int32_t);
-  CUDA_OK(cudaMemsetAsync(e->d_tri_cnt.p, 0, 2 * sizeof(int32_t), st));
-  ctvio::TriangulateWindowArgs a;
-  a.n_landmarks = nl; a.obs_offset = d_off; a.obs_slot = d_slot; a.obs_idx = d_idx;
-  a.table = e->d_frames.p; a.frame_t = e->d_frame_t.p; a.frame_cap = ctvio_engine::kFrameCap;
-  a.st = e->x[e->cur].ptrs(); a.sp = e->sp; a.R_CI = e->rig.R_CI; a.p_CI = e->rig.p_CI;
-  a.init_depth = init_depth;
-  // written into the other state buffer's array and swapped in only on success: after CTVIO_ERR_TIME_RANGE the
-  // resident inverse depths are the ones before the call
-  a.rho_in = e->x[e->cur].rho.p; a.rho_out = e->x[other].rho.p;
-  a.counts = e->d_tri_cnt.p;
-  e->launches += ctvio::launch_triangulate_window(a, st);
-  int32_t cnt[2];
-  CUDA_OK(cudaMemcpyAsync(cnt, e->d_tri_cnt.p, sizeof(cnt), cudaMemcpyDeviceToHost, st));
-  e->d2h_bytes += sizeof(cnt);
+  return triangulate_window_device(e, nl, d_off, d_slot, d_idx, init_depth, n_triangulated, n_fallback);
+}
+
+int ctvio_triangulate_window_from_table(ctvio_handle e, double init_depth, int32_t* n_triangulated, int32_t* n_fallback) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
+  if (!e->x[e->cur].ld.p) return fail(CTVIO_ERR_STATE, "the line delay has not been set");
+  if (!(init_depth > 0.0) || !std::isfinite(init_depth)) return fail(CTVIO_ERR_INVALID, "init_depth must be positive");
+  if (!e->ft.window_current) return fail(CTVIO_ERR_STATE, "no feature-table window since the last add / slide");
+  if (e->nL != e->ft.n_lm) return fail(CTVIO_ERR_STATE, "the resident inverse depths no longer follow the table's numbering");
+  if (n_triangulated) *n_triangulated = 0;
+  if (n_fallback) *n_fallback = 0;
+  if (e->nL == 0) return CTVIO_OK;
+  cudaSetDevice(e->cfg.device);
+  // the CSR was built on the device by ctvio_feature_table_window: nothing goes up
+  return triangulate_window_device(e, e->nL, e->ft.obs_offset.p, e->ft.obs_slot.p, e->ft.obs_idx.p, init_depth, n_triangulated,
+                                   n_fallback);
+}
+
+int ctvio_feature_table_add(ctvio_handle e, int32_t frame_slot, int32_t* n_tracked, int32_t* n_new) {
+  static_assert(ctvio_engine::kFrameSlots == ctvio::kKeyframeMaxSlots && ctvio_engine::kFrameCap == ctvio::kKeyframeMaxFeatures,
+                "the feature table covers the whole frame table");
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (frame_slot < 0 || frame_slot >= ctvio_engine::kFrameSlots) return fail(CTVIO_ERR_INVALID, "frame slot out of range");
+  if (!(e->h_frame_ingested >> frame_slot & 1u)) return fail(CTVIO_ERR_INVALID, "no feature cloud was ingested into the slot");
+  if (e->ft.held >> frame_slot & 1u) return fail(CTVIO_ERR_STATE, "the feature table still holds the slot");
+  cudaSetDevice(e->cfg.device);
+  if (const int rc = ensure_feature_table(e)) return rc;
+  cudaStream_t st = e->stream;
+  auto& t = e->ft;
+  ctvio::FeatureTableAddArgs a;
+  a.t = t.ptrs(); a.n_entries = t.n_entries;
+  a.key_in = t.key[t.cur_key].p; a.key_out = t.key[t.cur_key ^ 1].p;
+  a.cloud = e->d_frames.p + size_t(frame_slot) * ctvio_engine::kFrameCap;
+  a.n_features = e->h_frame_n[frame_slot];
+  a.slot = frame_slot; a.out = t.result.p;
+  e->launches += ctvio::launch_feature_table_add(a, st);
+  int32_t r[2];
+  CUDA_OK(cudaMemcpyAsync(r, t.result.p, sizeof(r), cudaMemcpyDeviceToHost, st));
+  e->d2h_bytes += sizeof(r);
   CUDA_OK(cudaStreamSynchronize(st));
-  if (cnt[0] < 0) return fail(CTVIO_ERR_TIME_RANGE, "an observation's row time falls outside the spline");
+  t.cur_key ^= 1;
+  t.n_entries += r[1];
+  t.held |= 1u << frame_slot;
+  t.window_current = false;
+  if (n_tracked) *n_tracked = r[0];
+  if (n_new) *n_new = r[1];
+  return CTVIO_OK;
+}
+
+int ctvio_feature_table_window(ctvio_handle e, int32_t n_frames, const int32_t* frame_slots, int32_t window_size,
+                               int32_t* n_landmarks) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (!frame_slots) return fail(CTVIO_ERR_INVALID, "null argument");
+  if (n_frames < 1 || n_frames > ctvio_engine::kFrameSlots) return fail(CTVIO_ERR_INVALID, "n_frames must be 1..16");
+  if (window_size < 3) return fail(CTVIO_ERR_INVALID, "window_size must be >= 3");
+  ctvio::FeatureTableWindowArgs a;
+  uint32_t listed = 0;
+  for (int s = 0; s < ctvio_engine::kFrameSlots; ++s) a.position[s] = -1;
+  for (int k = 0; k < n_frames; ++k) {
+    const int s = frame_slots[k];
+    if (s < 0 || s >= ctvio_engine::kFrameSlots) return fail(CTVIO_ERR_INVALID, "frame slot out of range");
+    if (listed & (1u << s)) return fail(CTVIO_ERR_INVALID, "a frame slot is listed twice");
+    listed |= 1u << s;
+    a.slot[k] = s;
+    a.position[s] = k;
+  }
+  auto& t = e->ft;
+  if (listed != t.held) return fail(CTVIO_ERR_STATE, "the listed frame slots are not the slots the feature table holds");
+  if (t.n_lm >= 0 && e->nL != t.n_lm)
+    return fail(CTVIO_ERR_STATE, "the resident inverse depths no longer follow the table's numbering");
+  cudaSetDevice(e->cfg.device);
+  if (const int rc = ensure_feature_table(e)) return rc;
+  cudaStream_t st = e->stream;
+  const int other = e->cur ^ 1;
+  const size_t cap = ctvio::kFeatureTableMaxEntries;
+  CUDA_OK(e->x[other].rho.reserve(cap + 1));  // only the other buffer: reserve() does not keep the contents
+  a.t = t.ptrs(); a.n_entries = t.n_entries; a.n_frames = n_frames; a.listed = listed; a.window_size = window_size;
+  a.rho_in = e->x[e->cur].rho.p; a.n_rho_in = std::max(t.n_lm, 0);
+  a.rho_out = e->x[other].rho.p;  // the re-laid-out depths go into the other state buffer, then the pointers swap
+  a.obs_offset = t.obs_offset.p; a.obs_slot = t.obs_slot.p; a.obs_idx = t.obs_idx.p;
+  a.lm_id = t.lm_id.p; a.lm_anchor = t.lm_anchor.p; a.lm_used = t.lm_used.p; a.out = t.result.p;
+  e->h2d_bytes += size_t(n_frames) * sizeof(int32_t);  // the slot list goes up with the launch
+  e->launches += ctvio::launch_feature_table_window(a, st);
+  int32_t r[2];
+  CUDA_OK(cudaMemcpyAsync(r, t.result.p, sizeof(r), cudaMemcpyDeviceToHost, st));
+  e->d2h_bytes += sizeof(r);
+  CUDA_OK(cudaStreamSynchronize(st));
   std::swap(e->x[e->cur].rho.p, e->x[other].rho.p);
   std::swap(e->x[e->cur].rho.cap, e->x[other].rho.cap);
+  if (r[0] != e->nL) e->structure_dirty = true;
+  e->nL = r[0];
+  e->have_rho = true;
   e->mirror_valid = false;
-  if (n_triangulated) *n_triangulated = cnt[0];
-  if (n_fallback) *n_fallback = cnt[1];
+  t.n_lm = r[0];
+  t.n_obs = r[1];
+  t.oldest_slot = a.slot[0];
+  t.window_current = true;
+  if (n_landmarks) *n_landmarks = r[0];
+  return CTVIO_OK;
+}
+
+int ctvio_add_image_features_from_table(ctvio_handle e, int32_t marg_oldest, int32_t* n_factors) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (!e->ft.window_current) return fail(CTVIO_ERR_STATE, "no feature-table window since the last add / slide");
+  if (e->nL != e->ft.n_lm) return fail(CTVIO_ERR_STATE, "the resident inverse depths no longer follow the table's numbering");
+  if (!e->img.empty() && e->img_desc.empty()) return fail(CTVIO_ERR_STATE, "image factors with host payload are already present");
+  cudaSetDevice(e->cfg.device);
+  cudaStream_t st = e->stream;
+  auto& t = e->ft;
+  const int n = t.n_obs - t.n_lm;
+  if (n_factors) *n_factors = n;
+  if (n > 0) {
+    ctvio::FeatureTableFactorArgs a;
+    a.n_landmarks = t.n_lm; a.obs_offset = t.obs_offset.p; a.obs_slot = t.obs_slot.p; a.obs_idx = t.obs_idx.p;
+    a.rho = e->x[e->cur].rho.p; a.oldest_slot = t.oldest_slot; a.marg_oldest = marg_oldest ? 1 : 0;
+    a.frame_cap = ctvio_engine::kFrameCap; a.out = t.desc.p;
+    e->launches += ctvio::launch_feature_table_factors(a, st);
+    // the engine's structure build (prepare) runs on the host: the 16-byte descriptors come back, the payload stays
+    const size_t base = e->img_desc.size();
+    e->img_desc.resize(base + size_t(n));
+    CUDA_OK(cudaMemcpyAsync(e->img_desc.data() + base, t.desc.p, size_t(n) * sizeof(ctvio::FactorDesc), cudaMemcpyDeviceToHost, st));
+    e->d2h_bytes += size_t(n) * sizeof(ctvio::FactorDesc);
+    CUDA_OK(cudaStreamSynchronize(st));
+    for (size_t k = base; k < e->img_desc.size(); ++k) {
+      const ctvio::FactorDesc& d = e->img_desc[k];
+      const int si = d.slot_i / ctvio_engine::kFrameCap, sj = d.slot_j / ctvio_engine::kFrameCap;
+      e->img.push_back(HostImage{e->h_frame_t[si], e->h_frame_t[sj], 0, 0, {0, 0}, {0, 0}, d.lm, d.marg});
+    }
+  }
+  e->structure_dirty = true;
+  return CTVIO_OK;
+}
+
+int ctvio_feature_table_slide(ctvio_handle e, int32_t frame_slot, int32_t* n_removed) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (frame_slot < 0 || frame_slot >= ctvio_engine::kFrameSlots) return fail(CTVIO_ERR_INVALID, "frame slot out of range");
+  auto& t = e->ft;
+  if (!(t.held >> frame_slot & 1u)) return fail(CTVIO_ERR_STATE, "the feature table does not hold the slot");
+  if (t.n_lm >= 0 && e->nL != t.n_lm)
+    return fail(CTVIO_ERR_STATE, "the resident inverse depths no longer follow the table's numbering");
+  cudaSetDevice(e->cfg.device);
+  cudaStream_t st = e->stream;
+  ctvio::FeatureTableSlideArgs a;
+  a.t = t.ptrs(); a.n_entries = t.n_entries;
+  a.key_in = t.key[t.cur_key].p; a.key_out = t.key[t.cur_key ^ 1].p; a.new_index = t.new_index.p;
+  a.slot = frame_slot; a.rho = e->x[e->cur].rho.p; a.n_rho = std::max(t.n_lm, 0); a.out = t.result.p;
+  e->launches += ctvio::launch_feature_table_slide(a, st);
+  int32_t r;
+  CUDA_OK(cudaMemcpyAsync(&r, t.result.p, sizeof(r), cudaMemcpyDeviceToHost, st));
+  e->d2h_bytes += sizeof(r);
+  CUDA_OK(cudaStreamSynchronize(st));
+  t.cur_key ^= 1;
+  t.n_entries -= r;
+  t.held &= ~(1u << frame_slot);
+  t.window_current = false;
+  e->h_frame_ingested &= ~(1u << frame_slot);
+  if (n_removed) *n_removed = r;
+  return CTVIO_OK;
+}
+
+int ctvio_feature_table_landmarks(ctvio_handle e, int32_t n_landmarks, int32_t* feature_id, int32_t* anchor_slot,
+                                  int32_t* used_num) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (!e->ft.window_current) return fail(CTVIO_ERR_STATE, "no feature-table window since the last add / slide");
+  if (n_landmarks != e->ft.n_lm) return fail(CTVIO_ERR_INVALID, "n_landmarks differs from the window's landmark count");
+  if (n_landmarks > 0 && (!feature_id || !anchor_slot || !used_num)) return fail(CTVIO_ERR_INVALID, "null argument");
+  if (n_landmarks == 0) return CTVIO_OK;
+  cudaSetDevice(e->cfg.device);
+  cudaStream_t st = e->stream;
+  const size_t bytes = size_t(n_landmarks) * sizeof(int32_t);
+  CUDA_OK(cudaMemcpyAsync(feature_id, e->ft.lm_id.p, bytes, cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync(anchor_slot, e->ft.lm_anchor.p, bytes, cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync(used_num, e->ft.lm_used.p, bytes, cudaMemcpyDeviceToHost, st));
+  e->d2h_bytes += 3 * bytes;
+  CUDA_OK(cudaStreamSynchronize(st));
   return CTVIO_OK;
 }
 
@@ -2539,6 +2757,8 @@ int ctvio_ingest_feature_cloud(ctvio_handle e, int32_t slot, int64_t t_ns, int32
   if (!e || slot < 0 || slot >= ctvio_engine::kFrameSlots || n < 0 || n > ctvio_engine::kFrameCap ||
       (n > 0 && (!points || !ch_id || !ch_v)))
     return fail(CTVIO_ERR_INVALID, "bad feature cloud");
+  // the feature table's indices point into the slot's cloud until ctvio_feature_table_slide frees it
+  if (e->ft.held >> slot & 1u) return fail(CTVIO_ERR_STATE, "the feature table holds the slot");
   cudaSetDevice(e->cfg.device);
   cudaStream_t st = e->stream;
   CUDA_OK(e->d_frames.reserve(size_t(ctvio_engine::kFrameSlots) * ctvio_engine::kFrameCap));
@@ -2546,6 +2766,7 @@ int ctvio_ingest_feature_cloud(ctvio_handle e, int32_t slot, int64_t t_ns, int32
   CUDA_OK(e->d_cloud_stage.reserve(5 * size_t(ctvio_engine::kFrameCap)));
   e->h_frame_t[slot] = t_ns;
   e->h_frame_n[slot] = n;
+  e->h_frame_ingested |= 1u << slot;
   CUDA_OK(cudaMemcpyAsync(e->d_frame_t.p + slot, &e->h_frame_t[slot], sizeof(int64_t), cudaMemcpyHostToDevice, st));
   if (n) {
     // the message arrays go up AS THEY ARE (packed float32 triples + float32 channels); conversion happens on the device

@@ -9,6 +9,9 @@
 //   keyframe_parallax_kernel  replaces FeatureManager::addFeatureCheckParallax (feature_manager.cpp:28-87) as
 //                        VisualOdometry::AddImageToWindow uses it (visual_odometry.cpp:180-183), on the resident frame
 //                        slots: tracked count of the new image and mean parallax between the two frames before it.
+//   feature_table_*_kernel  the feature list of FeatureManager (feature_manager.cpp:28-59 insertion, :111-147
+//                        getDepthVector / setDepth, :148-158 removeFailures, :341-423 the slide) as a resident table keyed
+//                        by the tracker's feature id, and the image-factor loops of trajectory_manager.cpp:206-236, :359-385.
 //   unpack_cloud_kernel  replaces FeatureMsg2Image (visual_odometry/visual_struct.h:98-121) on the tracker's message
 //                        (visual_feature/feature_tracker_node.cpp:146-184): sensor_msgs::PointCloud arrives as packed
 //                        float32 triples + five float32 channels and is converted ON THE DEVICE into the resident
@@ -185,6 +188,30 @@ __device__ __forceinline__ int kf_find(const uint64_t* keys, int n, int32_t id) 
   }
   return (a < n && (keys[a] >> 32) == (lo >> 32)) ? int(uint32_t(keys[a])) : -1;
 }
+// number of the n sorted keys whose id is smaller than the id of x
+__device__ __forceinline__ int kf_rank(const uint64_t* keys, int n, uint64_t x) {
+  const uint64_t lo = x & 0xffffffff00000000ull;
+  int a = 0, b = n;
+  while (a < b) {
+    const int m = (a + b) >> 1;
+    if (keys[m] < lo) a = m + 1; else b = m;
+  }
+  return a;
+}
+// ascending bitonic sort of N keys in shared memory.  Every thread of the block calls it (it synchronises the block after
+// each pass); the threads with `active` set each work on compare pair p, 0 <= p < N/2.
+template <int N>
+__device__ __forceinline__ void bitonic_sort_shared(uint64_t* keys, int p, bool active) {
+  for (int k = 2; k <= N; k <<= 1)
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      if (active) {
+        const int i = 2 * j * (p / j) + p % j;
+        const uint64_t x = keys[i], y = keys[i + j];
+        if ((x > y) == ((i & k) == 0)) { keys[i] = y; keys[i + j] = x; }
+      }
+      __syncthreads();
+    }
+}
 
 __global__ void __launch_bounds__(kKfThreads) keyframe_parallax_kernel(KeyframeArgs a) {
   __shared__ uint64_t s_key[2][kKeyframeMaxFeatures];  // [0]: the new slot, [1]: slot fc-2
@@ -202,18 +229,8 @@ __global__ void __launch_bounds__(kKfThreads) keyframe_parallax_kernel(KeyframeA
   s_tracked[tid] = 0;
   __syncthreads();
   // bitonic sort of both key arrays: threads [0, N/2) work on s_key[0], [N/2, N) on s_key[1]
-  {
-    constexpr int N = kKeyframeMaxFeatures;
-    uint64_t* keys = s_key[tid / (N / 2)];
-    const int p = tid % (N / 2);
-    for (int k = 2; k <= N; k <<= 1)
-      for (int j = k >> 1; j > 0; j >>= 1) {
-        const int i = 2 * j * (p / j) + p % j;
-        const uint64_t x = keys[i], y = keys[i + j];
-        if ((x > y) == ((i & k) == 0)) { keys[i] = y; keys[i + j] = x; }
-        __syncthreads();
-      }
-  }
+  constexpr int N = kKeyframeMaxFeatures;
+  bitonic_sort_shared<N>(s_key[tid / (N / 2)], tid % (N / 2), true);
   // last_track_num (:38-57): the new image's features whose id is already in the window
   for (int f = 0; f < fc; ++f) {
     const FrameFeature* t = a.table + size_t(a.slot[f]) * a.frame_cap;
@@ -255,6 +272,199 @@ __global__ void __launch_bounds__(kKfThreads) keyframe_parallax_kernel(KeyframeA
     else r.is_keyframe = sum / parallax_num >= a.min_parallax;
     *a.out = r;
   }
+}
+
+// ---- resident feature table (FeatureManager's feature list, feature_manager.cpp:28-59, :111-158, :341-423) --------------
+// Add, Slide and Window run as one CTA of kFtThreads threads; the counts come from block scans and __syncthreads_count.
+// Every entry and key is written by exactly one thread: no atomics, bitwise reproducible.
+constexpr int kFtThreads = kKeyframeMaxFeatures;
+static_assert(kFtThreads == 1024, "block_exclusive_scan covers 32 warps");
+
+// exclusive prefix sum of v over the block (kFtThreads threads, in thread order); `total` receives the block sum.
+// s: 32 ints of shared memory.  Synchronises the block (so every read issued before the call is complete on return).
+__device__ __forceinline__ int block_exclusive_scan(int v, int* s, int& total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) s[w] = x;
+  __syncthreads();
+  if (w == 0) {
+    int t = s[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, t, o);
+      if (lane >= o) t += y;
+    }
+    s[lane] = t;
+  }
+  __syncthreads();
+  const int before = (w ? s[w - 1] : 0) + x - v;
+  total = s[31];
+  __syncthreads();
+  return before;
+}
+
+// Add: the new slot's (id, index) keys are sorted; each binary-searches the live entries' sorted (id, entry) keys.  A hit
+// becomes that entry's observation in the slot; the misses, ranked in ascending id order, are appended as new entries.
+// The sorted key array is rebuilt by a rank merge into key_out (ids are distinct between the live entries and the misses).
+__global__ void __launch_bounds__(kFtThreads) feature_table_add_kernel(FeatureTableAddArgs a) {
+  __shared__ uint64_t s_key[kFtThreads];  // the new slot's keys, sorted
+  __shared__ uint64_t s_new[kFtThreads];  // (id, new entry) of the misses, ascending id
+  __shared__ int s_scan[32];
+  const int tid = threadIdx.x;
+  const int n_live = a.n_entries;
+  const FeatureTablePtrs& t = a.t;
+  s_key[tid] = tid < a.n_features ? kf_key(a.cloud[tid].id, tid) : ~0ull;
+  __syncthreads();
+  bitonic_sort_shared<kFtThreads>(s_key, tid, tid < kFtThreads / 2);
+  const uint64_t k = s_key[tid];
+  const bool valid = tid < a.n_features;
+  const int32_t id = int32_t(uint32_t(k >> 32) ^ 0x80000000u);
+  const int i = int(uint32_t(k));
+  const int hit = valid ? kf_find(a.key_in, n_live, id) : -1;
+  if (hit >= 0) {  // ids are unique within a cloud: one thread per entry
+    t.idx[size_t(a.slot) * kFeatureTableMaxEntries + hit] = i;
+    t.mask[hit] |= 1u << a.slot;
+  }
+  const bool miss = valid && hit < 0;
+  int n_new;
+  const int r = block_exclusive_scan(miss, s_scan, n_new);
+  const int n_tracked = __syncthreads_count(hit >= 0);
+  if (miss) {
+    const int e = n_live + r;
+    t.id[e] = id;
+    t.anchor[e] = a.slot;
+    t.mask[e] = 1u << a.slot;
+    t.lm[e] = -1;
+    t.rho[e] = -1.0;  // FeaturePerId: estimated_depth = -1
+    t.idx[size_t(a.slot) * kFeatureTableMaxEntries + e] = i;
+    s_new[r] = (k & 0xffffffff00000000ull) | uint32_t(e);
+  }
+  __syncthreads();
+  for (int j = tid; j < n_live; j += kFtThreads) {
+    const uint64_t x = a.key_in[j];
+    a.key_out[j + kf_rank(s_new, n_new, x)] = x;
+  }
+  if (tid < n_new) a.key_out[tid + kf_rank(a.key_in, n_live, s_new[tid])] = s_new[tid];
+  if (tid == 0) { a.out[0] = n_tracked; a.out[1] = n_new; }
+}
+
+// Slide: removeFailures (an entry numbered in the last window whose resident inverse depth is < 0), then the entries
+// anchored in the leaving slot go and every other one drops its observation there.  A stable in-place compaction of the
+// entries (a chunk is read completely before the scan's barrier, and lands at or below its own positions), then of the
+// sorted key array into key_out with the entries' new indices (a stable filter of a sorted array stays sorted).
+__global__ void __launch_bounds__(kFtThreads) feature_table_slide_kernel(FeatureTableSlideArgs a) {
+  __shared__ int s_scan[32];
+  const int tid = threadIdx.x;
+  const FeatureTablePtrs& t = a.t;
+  const uint32_t bit = 1u << a.slot;
+  constexpr size_t S = kFeatureTableMaxEntries;
+  int kept = 0;
+  for (int c = 0; c < a.n_entries; c += kFtThreads) {
+    const int e = c + tid;
+    const bool in = e < a.n_entries;
+    int32_t id = 0, anchor = 0, lm = -1, idx[kKeyframeMaxSlots];
+    uint32_t mask = 0;
+    double rho = 0.0;
+    bool keep = false;
+    if (in) {
+      id = t.id[e]; anchor = t.anchor[e]; lm = t.lm[e]; mask = t.mask[e]; rho = t.rho[e];
+#pragma unroll
+      for (int s = 0; s < kKeyframeMaxSlots; ++s) idx[s] = (mask >> s) & 1u ? t.idx[s * S + e] : -1;
+      const bool failed = lm >= 0 && lm < a.n_rho && a.rho[lm] < 0.0;  // SolveFail (feature_manager.cpp:148-158)
+      keep = !failed && anchor != a.slot;
+    }
+    int total;
+    const int r = block_exclusive_scan(keep, s_scan, total);
+    if (keep) {
+      const int d = kept + r;
+      t.id[d] = id; t.anchor[d] = anchor; t.lm[d] = lm; t.rho[d] = rho; t.mask[d] = mask & ~bit;
+#pragma unroll
+      for (int s = 0; s < kKeyframeMaxSlots; ++s)
+        if (((mask & ~bit) >> s) & 1u) t.idx[s * S + d] = idx[s];
+    }
+    if (in) a.new_index[e] = keep ? kept + r : -1;
+    kept += total;
+  }
+  __syncthreads();  // new_index complete (global memory written by this block)
+  int placed = 0;
+  for (int c = 0; c < a.n_entries; c += kFtThreads) {
+    const int j = c + tid;
+    const uint64_t x = j < a.n_entries ? a.key_in[j] : 0;
+    const int ne = j < a.n_entries ? a.new_index[uint32_t(x)] : -1;
+    int total;
+    const int r = block_exclusive_scan(ne >= 0, s_scan, total);
+    if (ne >= 0) a.key_out[placed + r] = (x & 0xffffffff00000000ull) | uint32_t(ne);
+    placed += total;
+  }
+  if (tid == 0) a.out[0] = a.n_entries - kept;
+}
+
+// Window: setDepth of the last window's landmarks, then the numbering of getDepthVector (isLandmarkCandidate: used_num >= 2
+// && start_frame < window_size - 2) in table order, the inverse depths re-laid out to it (rho_out) and the observation CSR
+// (anchor first, then the listed slots in window order) with per-landmark records.
+__global__ void __launch_bounds__(kFtThreads) feature_table_window_kernel(FeatureTableWindowArgs a) {
+  __shared__ int s_scan[32];
+  const int tid = threadIdx.x;
+  const FeatureTablePtrs& t = a.t;
+  constexpr size_t S = kFeatureTableMaxEntries;
+  int n_lm = 0, n_obs = 0;
+  for (int c = 0; c < a.n_entries; c += kFtThreads) {
+    const int e = c + tid;
+    const bool in = e < a.n_entries;
+    bool cand = false;
+    int used = 0, anchor = 0;
+    uint32_t mask = 0;
+    double rho = 0.0;
+    if (in) {
+      const int lm = t.lm[e];
+      rho = t.rho[e];
+      if (lm >= 0 && lm < a.n_rho_in) { rho = a.rho_in[lm]; t.rho[e] = rho; }  // setDepth (feature_manager.cpp:126-147)
+      mask = t.mask[e];
+      anchor = t.anchor[e];
+      used = __popc(mask & a.listed);
+      cand = used >= 2 && a.position[anchor] < a.window_size - 2;
+    }
+    int n_cand, n_used;
+    const int rl = block_exclusive_scan(cand, s_scan, n_cand);
+    const int ro = block_exclusive_scan(cand ? used : 0, s_scan, n_used);
+    if (in) t.lm[e] = cand ? n_lm + rl : -1;
+    if (cand) {
+      const int l = n_lm + rl;
+      int o = n_obs + ro;
+      a.rho_out[l] = rho;
+      a.obs_offset[l] = o;
+      a.lm_id[l] = t.id[e];
+      a.lm_anchor[l] = anchor;
+      a.lm_used[l] = used;
+      a.obs_slot[o] = anchor;
+      a.obs_idx[o++] = t.idx[anchor * S + e];
+      for (int k = 0; k < a.n_frames; ++k) {
+        const int s = a.slot[k];
+        if (s != anchor && ((mask >> s) & 1u)) { a.obs_slot[o] = s; a.obs_idx[o++] = t.idx[s * S + e]; }
+      }
+    }
+    n_lm += n_cand;
+    n_obs += n_used;
+  }
+  if (tid == 0) { a.obs_offset[n_lm] = n_obs; a.out[0] = n_lm; a.out[1] = n_obs; }
+}
+
+// image factors of the numbered landmarks (trajectory_manager.cpp:206-236, :359-385): one thread per landmark writes its
+// (anchor, observation) descriptors at obs_offset[l] - l, in the CSR's window order
+__global__ void feature_table_factors_kernel(FeatureTableFactorArgs a) {
+  const int l = blockIdx.x * blockDim.x + threadIdx.x;
+  if (l >= a.n_landmarks) return;
+  const int o0 = a.obs_offset[l], o1 = a.obs_offset[l + 1];
+  const int si = a.obs_slot[o0];
+  const int ti = si * a.frame_cap + a.obs_idx[o0];
+  const int marg = (a.marg_oldest && si == a.oldest_slot && a.rho[l] > 0.0) ? 1 : 0;  // :216-218
+  FactorDesc* d = a.out + (o0 - l);
+  for (int k = o0 + 1; k < o1; ++k) d[k - o0 - 1] = FactorDesc{ti, a.obs_slot[k] * a.frame_cap + a.obs_idx[k], l, marg};
 }
 
 // ---- wire formats -> resident tables ----------------------------------------------------------------
@@ -397,6 +607,23 @@ int launch_triangulate_window(const TriangulateWindowArgs& a, cudaStream_t s) {
 }
 int launch_keyframe_parallax(const KeyframeArgs& a, cudaStream_t s) {
   keyframe_parallax_kernel<<<1, kKfThreads, 0, s>>>(a);
+  return 1;
+}
+int launch_feature_table_add(const FeatureTableAddArgs& a, cudaStream_t s) {
+  feature_table_add_kernel<<<1, kFtThreads, 0, s>>>(a);
+  return 1;
+}
+int launch_feature_table_slide(const FeatureTableSlideArgs& a, cudaStream_t s) {
+  feature_table_slide_kernel<<<1, kFtThreads, 0, s>>>(a);
+  return 1;
+}
+int launch_feature_table_window(const FeatureTableWindowArgs& a, cudaStream_t s) {
+  feature_table_window_kernel<<<1, kFtThreads, 0, s>>>(a);
+  return 1;
+}
+int launch_feature_table_factors(const FeatureTableFactorArgs& a, cudaStream_t s) {
+  if (a.n_landmarks <= 0) return 0;
+  feature_table_factors_kernel<<<(a.n_landmarks + 127) / 128, 128, 0, s>>>(a);
   return 1;
 }
 int launch_unpack_cloud(const UnpackCloudArgs& a, cudaStream_t s) {

@@ -116,6 +116,75 @@ struct KeyframeArgs {
 };
 int launch_keyframe_parallax(const KeyframeArgs& a, cudaStream_t s);
 
+// Resident feature table (FeatureManager's feature list): one entry per landmark in creation order, structure of arrays
+// over kFeatureTableMaxEntries entries.  idx[s * kFeatureTableMaxEntries + e] is entry e's feature index in frame slot s,
+// valid where bit s of mask[e] is set (the anchor slot's bit included).  The live entries' (id, entry) keys are kept
+// sorted (kf_key order) in a separate array.
+constexpr int kFeatureTableMaxEntries = kKeyframeMaxSlots * kKeyframeMaxFeatures;
+struct FeatureTablePtrs {
+  int32_t* id;       // tracker feature id
+  int32_t* anchor;   // anchor frame slot
+  uint32_t* mask;    // slots holding an observation
+  int32_t* lm;       // number in the last window, -1: not numbered
+  double* rho;       // inverse depth (estimated_depth), -1: not initialised
+  int32_t* idx;      // [kKeyframeMaxSlots][kFeatureTableMaxEntries]
+};
+struct FeatureTableAddArgs {
+  FeatureTablePtrs t;
+  int32_t n_entries;
+  const uint64_t* key_in;      // [n_entries] sorted keys of the live entries
+  uint64_t* key_out;           // [n_entries + n_new]
+  const FrameFeature* cloud;   // the slot's features
+  int32_t n_features;          // <= kKeyframeMaxFeatures
+  int32_t slot;
+  int32_t* out;                // {n_tracked, n_new}
+};
+struct FeatureTableSlideArgs {
+  FeatureTablePtrs t;
+  int32_t n_entries;
+  const uint64_t* key_in;
+  uint64_t* key_out;
+  int32_t* new_index;          // [n_entries] scratch
+  int32_t slot;                // the leaving slot
+  const double* rho;           // resident inverse depths of the last window's numbering
+  int32_t n_rho;               // their count (0: no numbering, removeFailures is skipped)
+  int32_t* out;                // {n_removed}
+};
+struct FeatureTableWindowArgs {
+  FeatureTablePtrs t;
+  int32_t n_entries;
+  int32_t n_frames;
+  int32_t slot[kKeyframeMaxSlots];      // the window, oldest to newest
+  int32_t position[kKeyframeMaxSlots];  // window position of each frame slot (-1: not listed)
+  uint32_t listed;                      // mask of the listed slots
+  int32_t window_size;
+  const double* rho_in;        // resident inverse depths of the last numbering
+  int32_t n_rho_in;            // their count (0: no numbering)
+  double* rho_out;             // [n_landmarks] the new numbering's inverse depths (must not alias rho_in)
+  int32_t* obs_offset;         // [n_landmarks + 1]
+  int32_t* obs_slot;           // [n_obs] anchor first, then the listed slots in window order
+  int32_t* obs_idx;            // [n_obs]
+  int32_t* lm_id;              // [n_landmarks] per-landmark records: feature id, anchor slot, used_num
+  int32_t* lm_anchor;
+  int32_t* lm_used;
+  int32_t* out;                // {n_landmarks, n_obs}
+};
+struct FeatureTableFactorArgs {
+  int32_t n_landmarks;
+  const int32_t* obs_offset;
+  const int32_t* obs_slot;
+  const int32_t* obs_idx;
+  const double* rho;           // resident inverse depths (marg flag: rho > 0)
+  int32_t oldest_slot;         // slot of window position 0
+  int32_t marg_oldest;
+  int32_t frame_cap;
+  FactorDesc* out;             // [obs_offset[n_landmarks] - n_landmarks], landmark-major
+};
+int launch_feature_table_add(const FeatureTableAddArgs& a, cudaStream_t s);
+int launch_feature_table_slide(const FeatureTableSlideArgs& a, cudaStream_t s);
+int launch_feature_table_window(const FeatureTableWindowArgs& a, cudaStream_t s);
+int launch_feature_table_factors(const FeatureTableFactorArgs& a, cudaStream_t s);
+
 // device-resident window bookkeeping (all on the device)
 int launch_extend_knots(const StatePtrs& st, int old_n, int new_n, cudaStream_t s);
 int launch_slide_state(const StatePtrs& st, int nK, int nB, int dk, int db, int new_bias, double* tmp, cudaStream_t s);

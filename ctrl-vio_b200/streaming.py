@@ -405,6 +405,113 @@ def keyframe_decision(messages, min_parallax):
     return bool(parallax_sum / parallax_num >= min_parallax), n_tracked, parallax_num, parallax_sum
 
 
+class FeatureTable:
+    """FeatureManager's feature list (feature_manager.cpp:28-59, :111-158, :341-423) over the tracker's messages
+    (FrameClouds.message tuples) put into frame slots: the host restatement of the device's resident feature table
+    (ctvio_feature_table_*), and the reference for those calls.
+
+    One entry per landmark (FeaturePerId), in creation order: the feature id, the anchor slot, the feature index of its
+    observation in each of the 16 frame slots (-1: none; the anchor's own observation included), its number in the last
+    window (-1: not numbered) and its inverse depth (-1: not initialised).  Landmarks leave with their anchor frame (no
+    re-anchoring, the convention of subwindow_frames); an id seen again after its landmark left starts a new entry."""
+
+    N_SLOTS = 16
+
+    def __init__(self):
+        self.id = np.zeros(0, np.int64)
+        self.anchor = np.zeros(0, np.int32)
+        self.idx = np.full((0, self.N_SLOTS), -1, np.int32)
+        self.lm = np.zeros(0, np.int32)
+        self.rho = np.zeros(0)
+        self.held = set()            # frame slots whose cloud the table holds
+        self.numbered = np.zeros(0, np.int64)   # entries of the last window, in landmark order
+        self.slots = None            # the last window's frame slots, oldest to newest
+
+    def add(self, slot, message):
+        """the insertion half of addFeatureCheckParallax for the message put into `slot`: returns (n_tracked, n_new)"""
+        assert slot not in self.held, "the table still holds this slot"
+        ids = (np.asarray(message[1], np.float32).astype(np.float64) + 0.5).astype(np.int64)
+        pos = {int(i): k for k, i in enumerate(self.id)}
+        hit = np.array([pos.get(int(i), -1) for i in ids], np.int64)
+        tracked = hit >= 0
+        self.idx[hit[tracked], slot] = np.nonzero(tracked)[0]
+        order = np.argsort(ids[~tracked], kind="stable")       # new entries in ascending id (std::map) order
+        new_i = np.nonzero(~tracked)[0][order]
+        n = len(new_i)
+        idx = np.full((n, self.N_SLOTS), -1, np.int32)
+        idx[:, slot] = new_i
+        self.id = np.concatenate([self.id, ids[new_i]])
+        self.anchor = np.concatenate([self.anchor, np.full(n, slot, np.int32)])
+        self.idx = np.concatenate([self.idx, idx])
+        self.lm = np.concatenate([self.lm, np.full(n, -1, np.int32)])
+        self.rho = np.concatenate([self.rho, np.full(n, -1.0)])
+        self.held.add(slot)
+        return int(tracked.sum()), n
+
+    def used_num(self, slots):
+        return (self.idx[:, np.asarray(slots)] >= 0).sum(axis=1)
+
+    def window(self, slots, window_size, rho):
+        """setDepth of the last window's landmarks from `rho` (their solved inverse depths), then getDepthVector's
+        numbering: candidates used_num >= 2 && start_frame < window_size - 2 in table order.  Returns the inverse
+        depths of the new numbering (entries never initialised: -1)."""
+        assert set(slots) == self.held and len(set(slots)) == len(slots)
+        old = self.lm >= 0
+        self.rho[old] = np.asarray(rho)[self.lm[old]]
+        position = np.full(self.N_SLOTS, -1, np.int64)
+        position[np.asarray(slots)] = np.arange(len(slots))
+        start = position[self.anchor]
+        cand = (self.used_num(slots) >= 2) & (start < window_size - 2)
+        self.numbered = np.nonzero(cand)[0]
+        self.lm[:] = -1
+        self.lm[self.numbered] = np.arange(len(self.numbered))
+        self.slots = np.asarray(slots, np.int32)
+        return self.rho[self.numbered].copy()
+
+    def landmarks(self):
+        """(feature id, anchor slot, used_num) of each numbered landmark"""
+        e = self.numbered
+        return self.id[e], self.anchor[e], self.used_num(self.slots)[e]
+
+    def observation_csr(self):
+        """(obs_offset, obs_slot, obs_idx) of the window's landmarks: the anchor first, then the other observations in
+        window order"""
+        offset, slot, idx = [0], [], []
+        for e in self.numbered:
+            obs = [self.anchor[e]] + [s for s in self.slots if s != self.anchor[e] and self.idx[e, s] >= 0]
+            slot += obs
+            idx += [self.idx[e, s] for s in obs]
+            offset.append(len(slot))
+        return np.asarray(offset, np.int32), np.asarray(slot, np.int32), np.asarray(idx, np.int32)
+
+    def factors(self, rho, marg_oldest):
+        """image factors (trajectory_manager.cpp:206-236, :359-385), landmark-major and in window order within a
+        landmark: (slot_i, idx_i, slot_j, idx_j, landmark, marg).  marg: anchor in the oldest frame and rho > 0."""
+        off, slot, idx = self.observation_csr()
+        out = [[] for _ in range(6)]
+        for l in range(len(self.numbered)):
+            a = off[l]
+            m = int(bool(marg_oldest) and slot[a] == self.slots[0] and rho[l] > 0)
+            for k in range(a + 1, off[l + 1]):
+                for lst, v in zip(out, (slot[a], idx[a], slot[k], idx[k], l, m)):
+                    lst.append(v)
+        return tuple(np.asarray(x, np.int32) for x in out)
+
+    def slide(self, slot, rho):
+        """removeFailures (landmarks of the last window whose inverse depth in `rho` is < 0), then the landmarks
+        anchored in `slot` leave and every other one loses its observation there.  Returns the number removed."""
+        assert slot in self.held
+        fail = np.zeros(len(self.id), bool)
+        old = self.lm >= 0
+        fail[old] = np.asarray(rho)[self.lm[old]] < 0
+        keep = ~fail & (self.anchor != slot)
+        self.id, self.anchor, self.idx = self.id[keep], self.anchor[keep], self.idx[keep]
+        self.lm, self.rho = self.lm[keep], self.rho[keep]
+        self.idx[:, slot] = -1
+        self.held.discard(slot)
+        return int((~keep).sum())
+
+
 class ResidentRunner(StreamingRunner):
     """The same per-image cycle with the window living in HBM: the new image's PointCloud and the new IMUData records go
     up as they are, control points are extended / dropped on the device, inverse depths are re-indexed on the device,
@@ -424,11 +531,21 @@ class ResidentRunner(StreamingRunner):
     pose from its own IMU propagation (RI_, PI_, :189-190); here it is the predictor-solved spline, which carries the same
     IMU information.  Default (False): new landmarks take the sequence's initial guess rho0, as before.
     triangulate_probe (tests): called as probe(runner, obs_offset, obs_slot, obs_idx, rho_before) right after
-    TriangulateWindow, on the engine state the call used."""
+    TriangulateWindow, on the engine state the call used.
 
-    def __init__(self, lib, seq, triangulate=False, **kw):
+    device_features=True (requires triangulate=True): the feature list lives on the device (the resident feature table,
+    FeatureTable is its host restatement).  Each cloud joins it right after ingestion (FeatureTableAdd), the window's
+    landmarks are numbered and their inverse depths re-laid out by FeatureTableWindow, the triangulation and the image
+    factors come from the table, and the leaving frame's slot leaves it at the end of the step (FeatureTableSlide).  No
+    host association is used: the caller passes only frame slots.  Default (False): the host derives the landmark
+    numbering and the factor index tables from the sequence's ground-truth association, as before."""
+
+    def __init__(self, lib, seq, triangulate=False, device_features=False, **kw):
+        if device_features and not triangulate:
+            raise ValueError("device_features requires triangulate=True: new landmarks enter with inverse depth -1")
         super().__init__(lib, seq, **kw)
         self.triangulate = triangulate
+        self.device_features = device_features
         self.triangulate_probe = None
         if self.clouds is None:
             self.clouds = FrameClouds(seq)
@@ -467,6 +584,8 @@ class ResidentRunner(StreamingRunner):
             e.SetKnots(self.q[:self.ncp], self.p[:self.ncp]); e.SetBiases(self.bias[self.frames]); e.SetLineDelay(self.ld)
             for f in self.frames:
                 e.IngestFeatureCloud(self._assign_slot(f), int(s.kf_times[f]), *self.clouds.message(f))
+                if self.device_features:
+                    e.FeatureTableAdd(self.slot_of[f])
             self.base_knot = 0      # global index of the engine's knot 0
         else:
             self.frames.append(self.next_frame)
@@ -481,6 +600,8 @@ class ResidentRunner(StreamingRunner):
         if not first:
             f = self.frames[-1]
             e.IngestFeatureCloud(int(frame_slots[-1]), t_newest, *self.clouds.message(f))
+            if self.device_features:
+                e.FeatureTableAdd(int(frame_slots[-1]))   # addFeatureCheckParallax's insertion, by feature id
         decision = None
         if self.min_parallax is not None:
             # addFeatureCheckParallax on the device, over the clouds already in the frame table
@@ -506,30 +627,36 @@ class ResidentRunner(StreamingRunner):
         nloc = self.ncp - ks
         nowk, later = 0, self._knot_of(int(kf[1])) - ks
 
-        # ---- host-side index work of the "feature manager" (ids only, not timed like the classic runner's slicing) ----
-        w = syn.subwindow_frames(s, frames, imu_max_ns=min(max_t, t_newest + 1), window_size=WINDOW_SIZE)
-        lm_global = w.meta["lm_global"]
-        if self.prev_lm_global is None:
-            old_index = np.full(len(lm_global), -1, np.int32)
-        else:
-            pos = np.searchsorted(self.prev_lm_global, lm_global)
-            pos = np.clip(pos, 0, len(self.prev_lm_global) - 1)
-            old_index = np.where(self.prev_lm_global[pos] == lm_global, pos, -1).astype(np.int32)
-        # new landmarks (old_index < 0): the sequence's initial guess, or -1 (not initialised) when triangulated below
-        init_rho = np.full(len(lm_global), -1.0) if self.triangulate else s.rho0[lm_global]
-        img_marg = (w.anchor_frame[w.lm] == 0).astype(np.int32)  # (inverse depths are positive in the synthetic sequences)
-        bias_marg = np.zeros(len(w.bf_i), np.int32); bias_marg[0] = 1
+        # bias random walk between consecutive keyframes of the window (trajectory_manager.cpp:420-450)
+        bf_i = np.arange(len(kf) - 1, dtype=np.int32)
+        bf_sqrt_info = syn.bias_sqrt_info(s.imu_t, kf)
+        bias_marg = np.zeros(len(bf_i), np.int32); bias_marg[0] = 1
         if not marg:
-            img_marg[:] = 0; bias_marg[:] = 0
-        # factor -> (frame slot, index in that frame's cloud) of its two observations
-        sel = self._factor_selection(frames, lm_global)
-        g_lm = lm_global[w.lm]
-        slot_i = frame_slots[w.anchor_frame[w.lm]]
-        idx_i = self.clouds.anchor_idx[g_lm]
-        slot_j = frame_slots[w.obs_frame]
-        idx_j = self.clouds.obs_idx[sel]
-        if self.triangulate:
-            tri_csr = self._observation_csr(frames, w, lm_global, slot_j, idx_j, frame_slots)
+            bias_marg[:] = 0
+        if not self.device_features:
+            # ---- host-side index work of the "feature manager" (ids only, not timed like the classic runner's slicing) ----
+            w = syn.subwindow_frames(s, frames, imu_max_ns=min(max_t, t_newest + 1), window_size=WINDOW_SIZE)
+            lm_global = w.meta["lm_global"]
+            if self.prev_lm_global is None:
+                old_index = np.full(len(lm_global), -1, np.int32)
+            else:
+                pos = np.searchsorted(self.prev_lm_global, lm_global)
+                pos = np.clip(pos, 0, len(self.prev_lm_global) - 1)
+                old_index = np.where(self.prev_lm_global[pos] == lm_global, pos, -1).astype(np.int32)
+            # new landmarks (old_index < 0): the sequence's initial guess, or -1 (not initialised) when triangulated below
+            init_rho = np.full(len(lm_global), -1.0) if self.triangulate else s.rho0[lm_global]
+            img_marg = (w.anchor_frame[w.lm] == 0).astype(np.int32)  # (inverse depths are positive in the synthetic sequences)
+            if not marg:
+                img_marg[:] = 0
+            # factor -> (frame slot, index in that frame's cloud) of its two observations
+            sel = self._factor_selection(frames, lm_global)
+            g_lm = lm_global[w.lm]
+            slot_i = frame_slots[w.anchor_frame[w.lm]]
+            idx_i = self.clouds.anchor_idx[g_lm]
+            slot_j = frame_slots[w.obs_frame]
+            idx_j = self.clouds.obs_idx[sel]
+            if self.triangulate:
+                tri_csr = self._observation_csr(frames, w, lm_global, slot_j, idx_j, frame_slots)
         R0 = t0_ = None
         if self.readback is not None:
             qn, pn = self.readback[0][ks - self.prev_ks], self.readback[1][ks - self.prev_ks]
@@ -540,7 +667,11 @@ class ResidentRunner(StreamingRunner):
         # ---- timed region ----
         e.TransferStats(reset=True) if not first else None
         t_start = time.perf_counter()
-        e.RemapLandmarks(old_index, init_rho)
+        if self.device_features:
+            n_lm = e.FeatureTableWindow(frame_slots, WINDOW_SIZE)   # setDepth + getDepthVector, on the device
+        else:
+            e.RemapLandmarks(old_index, init_rho)
+            n_lm = len(lm_global)
         init_summary = None
         if not first and self.predictor:
             e.SetOptions(self._make_options(fixed_knot_index=max_bef_idx - ks, lock_wb=True, lock_ab=True, fix_ld=True))
@@ -553,21 +684,30 @@ class ResidentRunner(StreamingRunner):
         if self.triangulate:
             # FeatureManager::triangulate on the predictor-solved spline (window 0: the initializer's), before the
             # image factors that read the depths
-            rho_before = e.GetInvDepths() if self.triangulate_probe is not None else None
-            n_tri, n_fb = e.TriangulateWindow(*tri_csr)
-            if self.triangulate_probe is not None:
-                self.triangulate_probe(self, *tri_csr, rho_before)
+            if self.device_features:
+                n_tri, n_fb = e.TriangulateWindowFromTable()
+            else:
+                rho_before = e.GetInvDepths() if self.triangulate_probe is not None else None
+                n_tri, n_fb = e.TriangulateWindow(*tri_csr)
+                if self.triangulate_probe is not None:
+                    self.triangulate_probe(self, *tri_csr, rho_before)
         e.SetOptions(self._make_options(fix_ld=False, ld_lower=0.0, ld_upper=syn.LD_UPPER, is_marg_state=marg,
                                         ctrl_to_be_opt_now=nowk, ctrl_to_be_opt_later=later))
         e.ClearFactors()
         e.EnablePrior(True)
-        e.AddImageFeaturesFromSlots(slot_i, idx_i, slot_j, idx_j, w.lm, img_marg)
+        if self.device_features:
+            n_obs = e.AddImageFeaturesFromTable(marg)
+        else:
+            e.AddImageFeaturesFromSlots(slot_i, idx_i, slot_j, idx_j, w.lm, img_marg)
+            n_obs = w.n_obs
         opt_min = s.t0_ns + ks * s.dt_ns
         if marg:
-            e.AddImuFromTable(opt_min, min(max_t, t_newest + 1), kf_times=kf, marg_before_ns=int(kf[1]))
+            n_imu = e.AddImuFromTable(opt_min, min(max_t, t_newest + 1), kf_times=kf, marg_before_ns=int(kf[1]))
         else:
-            e.AddImuFromTable(opt_min, min(max_t, t_newest + 1), kf_times=kf)
-        e.AddBiasFactor(w.bf_i, w.bf_j, w.bf_sqrt_info, bias_marg)
+            n_imu = e.AddImuFromTable(opt_min, min(max_t, t_newest + 1), kf_times=kf)
+        e.AddBiasFactor(bf_i, bf_i + 1, bf_sqrt_info, bias_marg)
+        if not self.device_features:
+            n_imu = len(w.imu_t)
         t_built = time.perf_counter()
         summ = e.Solve(self.iters)
         t_solved = time.perf_counter()
@@ -586,26 +726,34 @@ class ResidentRunner(StreamingRunner):
         else:
             drop_knots = 0
             e.SlideWindowSecondNew()                   # slideWindowNew: the second-newest frame leaves, the prior stays
+        n_removed = None
+        if self.device_features:                       # the leaving frame's landmarks and observations leave the table
+            n_removed = e.FeatureTableSlide(self.slot_of[self.frames[0 if marg else -2]])
         t_wall = time.perf_counter() - t_start
         h2d, d2h = (0, 0) if first else e.TransferStats(reset=True)
 
         del self.slot_of[self.frames.pop(0 if marg else -2)]
         self.q[ks:self.ncp] = qs; self.p[ks:self.ncp] = ps
         self.ld = ld
-        self.readback, self.prev_ks, self.prev_lm_global = (qs, ps), ks, lm_global
+        self.readback, self.prev_ks = (qs, ps), ks
+        if not self.device_features:
+            self.prev_lm_global = lm_global
         self.base_knot = ks + drop_knots
         rec = dict(window=self.step_index, ms=1e3 * (t_wall + t_push), prior_const=0.0,
                    ms_build_and_predict=1e3 * (t_built - t_start + t_push), ms_solve=1e3 * (t_solved - t_built),
                    ms_realign_marginalize=1e3 * (t_marged - t_solved), ms_readback=1e3 * (t_start + t_wall - t_marged),
                    iterations=summ.iterations, final_cost=summ.final_cost, initial_cost=summ.initial_cost,
-                   termination=summ.termination, n_obs=w.n_obs, n_imu=len(w.imu_t), n_knots=nloc, n_lm=len(lm_global),
+                   termination=summ.termination, n_obs=n_obs, n_imu=n_imu, n_knots=nloc, n_lm=n_lm,
                    device_ms=summ.device_ms, marg_flag=marg_flag,
                    init_iterations=None if init_summary is None else init_summary.iterations, init_n_imu=0,
                    init_device_ms=0.0 if init_summary is None else init_summary.device_ms, prior_dim=self.prior_dim,
                    h2d_bytes=h2d, d2h_bytes=d2h)
         if decision is not None:
             rec.update(decision)
-        if self.triangulate:
+        if self.device_features:
+            # n_new_lm: the window's landmarks without a depth yet (-1), which are exactly the ones TriangulateWindow wrote
+            rec.update(n_triangulated=n_tri, n_fallback=n_fb, n_new_lm=n_tri + n_fb, n_removed=n_removed)
+        elif self.triangulate:
             rec.update(n_triangulated=n_tri, n_fallback=n_fb, n_new_lm=int(np.sum(old_index < 0)))
         self.records.append(rec)
         self.step_index += 1

@@ -307,7 +307,8 @@ int ctvio_enable_prior(ctvio_handle h, int32_t on);
  * replaces FeatureMsg2Image (visual_odometry/visual_struct.h:98-121) on the tracker's sensor_msgs::PointCloud
  * (visual_feature/feature_tracker_node.cpp:146-184): points = geometry_msgs::Point32[] (packed float32 x, y, z = 1),
  * channels[0..4] = id, u, v, velocity_x, velocity_y (float32 arrays).  The arrays are uploaded unchanged and unpacked on
- * the device into frame slot `frame_slot` (0..15) of the resident feature table. */
+ * the device into frame slot `frame_slot` (0..15) of the resident feature table.  CTVIO_ERR_STATE (nothing changes) while
+ * the resident feature table (ctvio_feature_table_*) holds the slot: ctvio_feature_table_slide frees it. */
 int ctvio_ingest_feature_cloud(ctvio_handle h, int32_t frame_slot, int64_t t_ns, int32_t n_points, const float* points_xyz,
                                const float* ch_id, const float* ch_u, const float* ch_v, const float* ch_vx,
                                const float* ch_vy);
@@ -327,6 +328,69 @@ int ctvio_ingest_imu(ctvio_handle h, int32_t n, const void* imu_data, int32_t st
  * samples before marg_before_ns are flagged for marginalization (:239-253). */
 int ctvio_add_imu_from_table(ctvio_handle h, int64_t t_min_ns, int64_t t_max_ns, int32_t n_kf, const int64_t* kf_times,
                              int32_t fixed_node, int64_t marg_before_ns, int32_t* n_added);
+/* ---- resident feature table: FeatureManager's feature list on the device ----
+ * One table per engine, empty at ctvio_create.  An entry is one landmark (FeaturePerId, feature_manager.h): the tracker's
+ * feature id, its anchor frame slot, its observations (the feature index in each frame slot that holds one, the
+ * anchor's own included), its number in the last window (or -1) and its inverse depth (estimated_depth; -1 = not
+ * initialised, as the FeaturePerId constructor sets it).  Entries stay in creation order.  Frame slots are those of
+ * ctvio_ingest_feature_cloud; the caller passes only slots, the association by id happens on the device.  The table's
+ * indices point into the slots' clouds, so ctvio_ingest_feature_cloud refuses a slot the table holds until it is slid.
+ * Deliberate deviation from the reference: a landmark leaves with its anchor frame.  The reference re-anchors it in the
+ * next frame (removeBackShiftDepth / removeFront, feature_manager.cpp:341-423); here its remaining observations leave
+ * with it, and when its id comes back in a later cloud it starts a new entry anchored there.
+ *
+ * ctvio_feature_table_add - the insertion half of addFeatureCheckParallax (feature_manager.cpp:28-59) for the cloud last
+ *   ingested into frame_slot: a feature whose id matches a live entry becomes that entry's observation in the slot (the
+ *   count is n_tracked, the reference's last_track_num over the live list); every other feature starts a new entry
+ *   anchored in the slot (n_new), appended in ascending id order (the std::map order of FeatureMsg2Image), not in cloud
+ *   order.  ctvio_check_keyframe is unchanged: its tracked count means "the id occurs in a listed slot", so it also
+ *   counts ids whose landmark has left the table (removeFailures, or an anchor frame that left), which this count does not.
+ *   Errors: CTVIO_ERR_INVALID for a slot outside 0..15 or a slot with no ingested cloud (none yet, or none since the table
+ *   slid it); CTVIO_ERR_STATE when the table still holds the slot.  One launch, one 8-byte read-back. */
+int ctvio_feature_table_add(ctvio_handle h, int32_t frame_slot, int32_t* n_tracked, int32_t* n_new);
+/* ctvio_feature_table_window - getDepthVector / setDepth / isLandmarkCandidate (feature_manager.cpp:111-147,
+ *   feature_manager.h:58-65) for the window frame_slots[0 .. n_frames-1], oldest to newest.  First every entry numbered in
+ *   the previous window takes back its resident inverse depth (setDepth).  Then the candidates - used_num >= 2 &&
+ *   start_frame < window_size - 2, where start_frame is the anchor slot's position in the list and used_num is 1 + its
+ *   observations in the other listed slots - are numbered 0 .. n_landmarks-1 in table order, and the resident inverse
+ *   depths are re-laid out on the device to that numbering, each from its entry (a new landmark: -1).  This replaces the
+ *   host's old-index table + ctvio_remap_landmarks.  The call also builds the observation CSR of
+ *   ctvio_triangulate_window_from_table and the factor list of ctvio_add_image_features_from_table on the device.
+ *   Errors: CTVIO_ERR_INVALID for n_frames outside 1..16, a slot outside 0..15, a repeated slot or window_size < 3;
+ *   CTVIO_ERR_STATE when the listed slots are not exactly the slots the table holds, or when the resident inverse-depth
+ *   count no longer equals the previous window's landmark count (ctvio_set_inv_depths / ctvio_remap_landmarks changed it).
+ *   One launch, one 8-byte read-back. */
+int ctvio_feature_table_window(ctvio_handle h, int32_t n_frames, const int32_t* frame_slots, int32_t window_size,
+                               int32_t* n_landmarks);
+/* ctvio_triangulate_window_from_table - ctvio_triangulate_window (FeatureManager::triangulate / triangulateRS,
+ *   feature_manager.cpp:226-338) over the last window's landmarks, with the CSR ctvio_feature_table_window built on the
+ *   device (anchor first, then the observations in window order): same kernel, same rules (only inverse depths <= 0 are
+ *   written, same init_depth fallback, CTVIO_ERR_TIME_RANGE leaves the depths unchanged).  Nothing goes up.
+ *   Errors: CTVIO_ERR_INVALID for init_depth <= 0; CTVIO_ERR_STATE before the knots / line delay are set, without a
+ *   window since the last add / slide, or when the resident inverse-depth count differs from the window's landmark count. */
+int ctvio_triangulate_window_from_table(ctvio_handle h, double init_depth, int32_t* n_triangulated, int32_t* n_fallback);
+/* ctvio_add_image_features_from_table - the image-factor loops of UpdateTrajectory / UpdateVIOPrior
+ *   (trajectory_manager.cpp:206-236, :359-385) over the last window's landmarks: one factor per (landmark, observation
+ *   other than the anchor), landmark-major, in window order within a landmark.  With marg_oldest != 0 a factor is flagged
+ *   for marginalization when its anchor is the window's oldest slot and the landmark's resident inverse depth is > 0 at
+ *   the time of the call.  The factors join the same path as ctvio_add_image_features_from_slots: the 16-byte
+ *   descriptors are read back (counted in ctvio_transfer_stats) for the host's structure build; the payload stays resident.
+ *   Errors: CTVIO_ERR_STATE without a window since the last add / slide, when the resident inverse-depth count differs
+ *   from the window's landmark count, or when image factors with host payload are present. */
+int ctvio_add_image_features_from_table(ctvio_handle h, int32_t marg_oldest, int32_t* n_factors);
+/* ctvio_feature_table_slide - the feature-list half of SlideWindowOld / SlideWindowNew for the leaving frame_slot.  First
+ *   removeFailures (feature_manager.cpp:148-158): an entry numbered in the last window whose resident inverse depth is
+ *   < 0 leaves (SolveFail; 0 and NaN stay).  Then the entries anchored in frame_slot leave (see the deviation above) and
+ *   every other entry loses its observation there.  The slot is then free for the next ctvio_ingest_feature_cloud.
+ *   Errors: CTVIO_ERR_INVALID for a slot outside 0..15; CTVIO_ERR_STATE when the table does not hold the slot or when
+ *   the resident inverse-depth count differs from the last window's landmark count.  One launch, one 4-byte read-back. */
+int ctvio_feature_table_slide(ctvio_handle h, int32_t frame_slot, int32_t* n_removed);
+/* ctvio_feature_table_landmarks - feature id, anchor slot and used_num of each landmark of the last window, in its
+ *   numbering (GetLandmarksInWindow needs the id).  Errors: CTVIO_ERR_INVALID for a landmark-count mismatch or a NULL
+ *   array; CTVIO_ERR_STATE without a window since the last add / slide. */
+int ctvio_feature_table_landmarks(ctvio_handle h, int32_t n_landmarks, int32_t* feature_id, int32_t* anchor_slot,
+                                  int32_t* used_num);
+
 /* bytes moved host<->device by the C-ABI calls since the last reset (state, factors, priors, index tables) */
 int ctvio_transfer_stats(ctvio_handle h, int64_t* h2d_bytes, int64_t* d2h_bytes, int32_t reset);
 
