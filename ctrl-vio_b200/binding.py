@@ -105,7 +105,7 @@ ABI_SYMBOLS = [
     "ingest_imu", "add_imu_from_table", "transfer_stats", "profile_kernels", "measure_fp64_tflops", "measure_fp64_tensor_tflops",
     "selfcheck_solver", "nccl_unique_id", "comm_init", "triangulate_window", "check_keyframe", "slide_window_second_new",
     "feature_table_add", "feature_table_window", "triangulate_window_from_table", "add_image_features_from_table",
-    "feature_table_slide", "feature_table_landmarks",
+    "feature_table_slide", "feature_table_landmarks", "feature_table_map",
 ]
 
 
@@ -115,7 +115,8 @@ DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enab
                        "ingest_feature_cloud", "add_image_features_from_slots", "ingest_imu", "add_imu_from_table",
                        "transfer_stats", "residual_summary", "triangulate_window", "check_keyframe",
                        "slide_window_second_new", "feature_table_add", "feature_table_window", "triangulate_window_from_table",
-                       "add_image_features_from_table", "feature_table_slide", "feature_table_landmarks")
+                       "add_image_features_from_table", "feature_table_slide", "feature_table_landmarks",
+                       "feature_table_map")
 
 
 def _addr(a):
@@ -498,6 +499,24 @@ class Estimator:
         ids, anchor, used = (np.zeros(max(n, 0), np.int32) for _ in range(3))
         self.lib.call("feature_table_landmarks", self.h, C.c_int32(n), _ip(ids), _ip(anchor), _ip(used))
         return ids, anchor, used
+
+    # capacity of FeatureTableMap's point arrays: every entry the table can hold (16 slots x 1024 features)
+    MAP_CAPACITY = 16 * 1024
+
+    def FeatureTableMap(self, frame_slots, window_size):
+        """GetLandmarksInWindow / GetMarginCloud / PublishVioKeyFrame (visual_odometry.cpp:310-372) over the window's
+        frame slots after the slide, oldest to newest.  Returns (xyz [n, 3], feature ids [n], in_margin_cloud [n] bool,
+        camera q xyzw [n_frames, 4], camera p [n_frames, 3]): the stable landmarks in table order, world points, and
+        the frames' camera poses at the frame time."""
+        slots = _i32(frame_slots)
+        cap = self.MAP_CAPACITY
+        xyz, ids, marg = np.empty((cap, 3)), np.empty(cap, np.int32), np.empty(cap, np.uint8)
+        cq, cp = np.empty((slots.shape[0], 4)), np.empty((slots.shape[0], 3))
+        n = C.c_int32()
+        self.lib.call("feature_table_map", self.h, C.c_int32(slots.shape[0]), _ip(slots), C.c_int32(window_size),
+                      C.c_int32(cap), _dp(xyz), _ip(ids), _ip(marg), C.byref(n), _dp(cq), _dp(cp))
+        k = n.value
+        return xyz[:k].copy(), ids[:k].copy(), marg[:k].astype(bool), cq, cp
 
     def IngestImu(self, records: np.ndarray, off_gyro, off_accel, drop_before_ns=0):
         """packed IMUData records (structured / byte array, one record per row)."""

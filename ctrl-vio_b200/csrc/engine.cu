@@ -253,6 +253,9 @@ struct ctvio_engine {
     int n_obs = 0;
     bool window_current = false;  // the CSR and records describe the table as it is (no add / slide since the window)
     int32_t oldest_slot = 0;
+    // ctvio_feature_table_map's output, written by its kernel: pinned + mapped, allocated on first use
+    ctvio::MapHeader* h_map_head = nullptr;
+    ctvio::MapPoint* h_map_points = nullptr;
     ctvio::FeatureTablePtrs ptrs() { return ctvio::FeatureTablePtrs{id.p, anchor.p, mask.p, lm.p, rho.p, idx.p}; }
   } ft;
   // marginalization workspace (K7), kept across windows: allocation / free costs more than the kernels
@@ -1094,6 +1097,7 @@ int ctvio_destroy(ctvio_handle e) {
   if (e->h_scal) cudaFreeHost(e->h_scal);
   if (e->h_pub) cudaFreeHost(e->h_pub);
   if (e->h_mirror) cudaFreeHost(e->h_mirror);
+  if (e->ft.h_map_head) cudaFreeHost(e->ft.h_map_head);
   if (e->ev_zero) cudaEventDestroy(e->ev_zero);
   cudaEventDestroy(e->ev0);
   cudaEventDestroy(e->ev1);
@@ -2689,6 +2693,76 @@ int ctvio_feature_table_landmarks(ctvio_handle e, int32_t n_landmarks, int32_t* 
   CUDA_OK(cudaMemcpyAsync(used_num, e->ft.lm_used.p, bytes, cudaMemcpyDeviceToHost, st));
   e->d2h_bytes += 3 * bytes;
   CUDA_OK(cudaStreamSynchronize(st));
+  return CTVIO_OK;
+}
+
+int ctvio_feature_table_map(ctvio_handle e, int32_t n_frames, const int32_t* frame_slots, int32_t window_size,
+                            int32_t capacity, double* xyz_world, int32_t* feature_id, uint8_t* in_margin_cloud,
+                            int32_t* n_points, double* cam_q_xyzw, double* cam_p_xyz) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (!frame_slots || !n_points) return fail(CTVIO_ERR_INVALID, "null argument");
+  if (n_frames < 1 || n_frames > ctvio_engine::kFrameSlots) return fail(CTVIO_ERR_INVALID, "n_frames must be 1..16");
+  if (window_size < 3) return fail(CTVIO_ERR_INVALID, "window_size must be >= 3");
+  if (capacity < 0) return fail(CTVIO_ERR_INVALID, "capacity must be >= 0");
+  if (capacity > 0 && (!xyz_world || !feature_id || !in_margin_cloud)) return fail(CTVIO_ERR_INVALID, "null point array");
+  ctvio::FeatureTableMapArgs a;
+  uint32_t listed = 0;
+  for (int s = 0; s < ctvio_engine::kFrameSlots; ++s) a.position[s] = -1;
+  for (int k = 0; k < n_frames; ++k) {
+    const int s = frame_slots[k];
+    if (s < 0 || s >= ctvio_engine::kFrameSlots) return fail(CTVIO_ERR_INVALID, "frame slot out of range");
+    if (listed & (1u << s)) return fail(CTVIO_ERR_INVALID, "a frame slot is listed twice");
+    listed |= 1u << s;
+    a.slot[k] = s;
+    a.position[s] = k;
+  }
+  auto& t = e->ft;
+  if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
+  if (listed != t.held) return fail(CTVIO_ERR_STATE, "the listed frame slots are not the slots the feature table holds");
+  if (t.n_lm >= 0 && e->nL != t.n_lm)
+    return fail(CTVIO_ERR_STATE, "the resident inverse depths no longer follow the table's numbering");
+  for (int k = 0; k < n_frames; ++k) {
+    int32_t s;
+    double u;
+    if (!spline_index(e->sp, e->h_frame_t[a.slot[k]], s, u))
+      return fail(CTVIO_ERR_TIME_RANGE, "a listed frame time falls outside the spline");
+  }
+  cudaSetDevice(e->cfg.device);
+  if (!t.h_map_head) {
+    void* p = nullptr;
+    const size_t bytes = sizeof(ctvio::MapHeader) + size_t(ctvio::kFeatureTableMaxEntries) * sizeof(ctvio::MapPoint);
+    if (cudaHostAlloc(&p, bytes, cudaHostAllocMapped) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(CTVIO_ERR_CUDA, "could not allocate the mapped map buffer");
+    }
+    t.h_map_head = static_cast<ctvio::MapHeader*>(p);
+    t.h_map_points = reinterpret_cast<ctvio::MapPoint*>(t.h_map_head + 1);
+  }
+  cudaStream_t st = e->stream;
+  ensure_table(e);
+  a.t = t.ptrs(); a.n_entries = t.n_entries; a.n_frames = n_frames; a.listed = listed; a.window_size = window_size;
+  a.table = e->d_frames.p; a.frame_t = e->d_frame_t.p; a.frame_cap = ctvio_engine::kFrameCap;
+  a.st = e->x[e->cur].ptrs(); a.sp = e->sp; a.R_CI = e->rig.R_CI; a.p_CI = e->rig.p_CI;
+  a.rho = e->x[e->cur].rho.p; a.n_rho = std::max(t.n_lm, 0);
+  a.head = t.h_map_head; a.points = t.h_map_points;
+  // the slot list goes with the launch parameters; the kernel writes the result straight into mapped host memory
+  e->launches += ctvio::launch_feature_table_map(a, st);
+  CUDA_OK(cudaStreamSynchronize(st));
+  const ctvio::MapHeader& h = *t.h_map_head;
+  const int n = h.n_points;
+  e->d2h_bytes += 8 + 56 * size_t(n_frames) + sizeof(ctvio::MapPoint) * size_t(n);
+  *n_points = n;
+  if (n > capacity) return fail(CTVIO_ERR_INVALID, "capacity is smaller than the number of map points");
+  for (int k = 0; k < n; ++k) {
+    const ctvio::MapPoint& p = t.h_map_points[k];
+    xyz_world[3 * k] = p.xyz[0]; xyz_world[3 * k + 1] = p.xyz[1]; xyz_world[3 * k + 2] = p.xyz[2];
+    feature_id[k] = p.id;
+    in_margin_cloud[k] = uint8_t(p.in_margin_cloud);
+  }
+  for (int k = 0; k < n_frames; ++k) {
+    if (cam_q_xyzw) for (int c = 0; c < 4; ++c) cam_q_xyzw[4 * k + c] = h.cam[k][c];
+    if (cam_p_xyz) for (int c = 0; c < 3; ++c) cam_p_xyz[3 * k + c] = h.cam[k][4 + c];
+  }
   return CTVIO_OK;
 }
 

@@ -12,6 +12,8 @@
 //   feature_table_*_kernel  the feature list of FeatureManager (feature_manager.cpp:28-59 insertion, :111-147
 //                        getDepthVector / setDepth, :148-158 removeFailures, :341-423 the slide) as a resident table keyed
 //                        by the tracker's feature id, and the image-factor loops of trajectory_manager.cpp:206-236, :359-385.
+//                        feature_table_map_kernel publishes its landmark map (GetLandmarksInWindow / GetMarginCloud,
+//                        visual_odometry.cpp:310-372) and the keyframe camera poses (PublishVioKeyFrame).
 //   unpack_cloud_kernel  replaces FeatureMsg2Image (visual_odometry/visual_struct.h:98-121) on the tracker's message
 //                        (visual_feature/feature_tracker_node.cpp:146-184): sensor_msgs::PointCloud arrives as packed
 //                        float32 triples + five float32 channels and is converted ON THE DEVICE into the resident
@@ -467,6 +469,68 @@ __global__ void feature_table_factors_kernel(FeatureTableFactorArgs a) {
   for (int k = o0 + 1; k < o1; ++k) d[k - o0 - 1] = FactorDesc{ti, a.obs_slot[k] * a.frame_cap + a.obs_idx[k], l, marg};
 }
 
+// Map: GetLandmarksInWindow / GetMarginCloud (visual_odometry.cpp:310-372) and the keyframe poses of PublishVioKeyFrame
+// over the listed window.  The listed frames' camera poses (GetCameraPose at the frame time, :197-202) are evaluated
+// first into shared memory; then the entries, in chunks of kFtThreads: IsLandMarkStable (visual_odometry.h:82-93), a
+// block scan, and the stable ones are written compacted, in table order, to mapped host memory.  No atomics.
+__global__ void __launch_bounds__(kFtThreads) feature_table_map_kernel(FeatureTableMapArgs a) {
+  __shared__ double s_cam[kKeyframeMaxSlots][12];  // by window position: camera R (9) | camera t (3)
+  __shared__ int s_scan[32];
+  const int tid = threadIdx.x;
+  const FeatureTablePtrs& t = a.t;
+  constexpr size_t S = kFeatureTableMaxEntries;
+  if (tid < a.n_frames) {
+    int32_t s;
+    double u;
+    spline_index(a.sp, a.frame_t[a.slot[tid]], s, u);
+    SideEval ev;
+    eval_side<false, kPStride>(a.sp, a.st.q, a.st.p, a.st.tab, s, u, ev);
+    const M3 Rc = m3_mul(ev.R, a.R_CI);        // R_c = R * R_CI  (as triangulate_window_kernel)
+    const V3 tc = ev.p + m3_vec(ev.R, a.p_CI);  // t_c = p + R * p_CI
+#pragma unroll
+    for (int e = 0; e < 9; ++e) s_cam[tid][e] = Rc.m[e];
+    s_cam[tid][9] = tc.x; s_cam[tid][10] = tc.y; s_cam[tid][11] = tc.z;
+    const Q4 q = quat_from_matrix(Rc);
+    double* c = a.head->cam[tid];
+    c[0] = q.x; c[1] = q.y; c[2] = q.z; c[3] = q.w;
+    c[4] = tc.x; c[5] = tc.y; c[6] = tc.z;
+  }
+  __syncthreads();
+  const double late = a.window_size * 3.0 / 4.0;
+  int n_points = 0;
+  for (int c = 0; c < a.n_entries; c += kFtThreads) {
+    const int e = c + tid;
+    bool stable = false, margin = false;
+    MapPoint p;
+    if (e < a.n_entries) {
+      const int anchor = t.anchor[e], lm = t.lm[e];
+      const int start = a.position[anchor];
+      const int used = __popc(t.mask[e] & a.listed);
+      const bool numbered = lm >= 0 && lm < a.n_rho;
+      const double depth = 1.0 / (numbered ? a.rho[lm] : t.rho[e]);  // the next setDepth's value, else the stored one
+      // isLandmarkCandidate, start_frame > WINDOW_SIZE * 3 / 4, estimated_depth <= 0 (a NaN depth passes)
+      stable = used >= 2 && start < a.window_size - 2 && !(start > late) && !(depth <= 0.0);
+      // GetMarginCloud: start_frame == 0, used_num <= 2, solve_flag == SovelSucc (setDepth's !(depth < 0) of a numbered
+      // entry, which stable implies)
+      margin = stable && start == 0 && used <= 2 && numbered;
+      if (stable) {
+        const FrameFeature f = a.table[size_t(anchor) * a.frame_cap + t.idx[anchor * S + e]];
+        const double* w = s_cam[start];
+        const V3 pc{f.x * depth, f.y * depth, depth};  // feature_per_frame[0].point * estimated_depth
+#pragma unroll
+        for (int r = 0; r < 3; ++r) p.xyz[r] = w[3 * r] * pc.x + w[3 * r + 1] * pc.y + w[3 * r + 2] * pc.z + w[9 + r];
+        p.id = t.id[e];
+        p.in_margin_cloud = margin ? 1 : 0;
+      }
+    }
+    int total;
+    const int r = block_exclusive_scan(stable, s_scan, total);
+    if (stable) a.points[n_points + r] = p;
+    n_points += total;
+  }
+  if (tid == 0) { a.head->n_points = n_points; a.head->pad = 0; }
+}
+
 // ---- wire formats -> resident tables ----------------------------------------------------------------
 
 __global__ void unpack_cloud_kernel(UnpackCloudArgs a) {
@@ -624,6 +688,10 @@ int launch_feature_table_window(const FeatureTableWindowArgs& a, cudaStream_t s)
 int launch_feature_table_factors(const FeatureTableFactorArgs& a, cudaStream_t s) {
   if (a.n_landmarks <= 0) return 0;
   feature_table_factors_kernel<<<(a.n_landmarks + 127) / 128, 128, 0, s>>>(a);
+  return 1;
+}
+int launch_feature_table_map(const FeatureTableMapArgs& a, cudaStream_t s) {
+  feature_table_map_kernel<<<1, kFtThreads, 0, s>>>(a);
   return 1;
 }
 int launch_unpack_cloud(const UnpackCloudArgs& a, cudaStream_t s) {

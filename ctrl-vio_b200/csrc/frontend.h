@@ -1,6 +1,7 @@
 // Front-end data formats either side of the hot path (frontend.cu): DLT triangulation (from caller poses, and of the
 // resident window from the resident spline), the keyframe decision over the resident frame slots, wire-format unpacking,
-// device-side construction of the sorted image-factor arrays from the resident per-frame feature tables.
+// device-side construction of the sorted image-factor arrays from the resident per-frame feature tables, and the
+// published landmark map of the resident feature table.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -180,10 +181,44 @@ struct FeatureTableFactorArgs {
   int32_t frame_cap;
   FactorDesc* out;             // [obs_offset[n_landmarks] - n_landmarks], landmark-major
 };
+// the published landmark map (GetLandmarksInWindow / GetMarginCloud / PublishVioKeyFrame), written by
+// feature_table_map_kernel straight into mapped host memory: a header with the listed frames' camera poses, then the
+// stable points compacted in table order
+struct MapPoint {              // 32 B
+  double xyz[3];               // world point
+  int32_t id;                  // tracker feature id
+  int32_t in_margin_cloud;     // 0 / 1
+};
+struct MapHeader {
+  int32_t n_points;            // stable entries (all of them are written to points)
+  int32_t pad;
+  double cam[kKeyframeMaxSlots][7];  // camera pose at each listed frame's time: q (x, y, z, w), p
+};
+struct FeatureTableMapArgs {
+  FeatureTablePtrs t;          // read only
+  int32_t n_entries;
+  int32_t n_frames;
+  int32_t slot[kKeyframeMaxSlots];      // the window, oldest to newest
+  int32_t position[kKeyframeMaxSlots];  // window position of each frame slot (-1: not listed)
+  uint32_t listed;                      // mask of the listed slots
+  int32_t window_size;
+  const FrameFeature* table;   // [n_slots][frame_cap]
+  const int64_t* frame_t;      // [n_slots]; every listed frame time lies inside the spline (checked by the caller)
+  int32_t frame_cap;
+  StatePtrs st;                // knots, knot-pair table (valid)
+  SplineParams sp;
+  M3 R_CI;                     // camera -> IMU rotation
+  V3 p_CI;
+  const double* rho;           // resident inverse depths of the last window's numbering
+  int32_t n_rho;               // their count (0: no numbering)
+  MapHeader* head;             // mapped host memory
+  MapPoint* points;            // mapped host memory, [kFeatureTableMaxEntries]
+};
 int launch_feature_table_add(const FeatureTableAddArgs& a, cudaStream_t s);
 int launch_feature_table_slide(const FeatureTableSlideArgs& a, cudaStream_t s);
 int launch_feature_table_window(const FeatureTableWindowArgs& a, cudaStream_t s);
 int launch_feature_table_factors(const FeatureTableFactorArgs& a, cudaStream_t s);
+int launch_feature_table_map(const FeatureTableMapArgs& a, cudaStream_t s);
 
 // device-resident window bookkeeping (all on the device)
 int launch_extend_knots(const StatePtrs& st, int old_n, int new_n, cudaStream_t s);

@@ -426,6 +426,7 @@ class FeatureTable:
         self.held = set()            # frame slots whose cloud the table holds
         self.numbered = np.zeros(0, np.int64)   # entries of the last window, in landmark order
         self.slots = None            # the last window's frame slots, oldest to newest
+        self.bearing = {}            # frame slot -> bearings (x, y) of its cloud, as the wire carries them (float32)
 
     def add(self, slot, message):
         """the insertion half of addFeatureCheckParallax for the message put into `slot`: returns (n_tracked, n_new)"""
@@ -446,6 +447,7 @@ class FeatureTable:
         self.lm = np.concatenate([self.lm, np.full(n, -1, np.int32)])
         self.rho = np.concatenate([self.rho, np.full(n, -1.0)])
         self.held.add(slot)
+        self.bearing[slot] = np.asarray(message[0], np.float32)[:, :2].astype(np.float64)
         return int(tracked.sum()), n
 
     def used_num(self, slots):
@@ -511,6 +513,53 @@ class FeatureTable:
         self.held.discard(slot)
         return int((~keep).sum())
 
+    def map(self, slots, window_size, rho, cam_R, cam_t):
+        """GetLandmarksInWindow / GetMarginCloud (visual_odometry.cpp:310-372) over the window's frame slots after the
+        slide, oldest to newest: the reference of ctvio_feature_table_map.  rho: the resident inverse depths of the last
+        window's numbering; cam_R [n_frames, 3, 3], cam_t [n_frames, 3]: the camera pose of each listed frame.
+        Per entry: start = window position of its anchor, used_num = 1 + its observations in the other listed slots,
+        depth = 1 / (its resident inverse depth when numbered in the last window, else its stored one).  Stable
+        (IsLandMarkStable): used_num >= 2, start < window_size - 2, not start > window_size * 3 / 4, not depth <= 0 (NaN
+        passes).  Margin cloud: stable, start == 0, used_num <= 2 and numbered in the last window (solve_flag ==
+        SovelSucc).  Returns (xyz [n, 3] world points R_c (x, y, 1) depth + t_c, feature ids [n], in_margin_cloud [n]) of
+        the stable entries in table order."""
+        assert set(slots) == self.held and len(set(slots)) == len(slots)
+        slots = np.asarray(slots)
+        position = np.full(self.N_SLOTS, -1, np.int64)
+        position[slots] = np.arange(len(slots))
+        start = position[self.anchor]
+        used = self.used_num(slots)
+        rho = np.asarray(rho, np.float64)
+        numbered = (self.lm >= 0) & (self.lm < len(rho))
+        r = self.rho.copy()
+        r[numbered] = rho[self.lm[numbered]]
+        with np.errstate(divide="ignore"):
+            depth = 1.0 / r
+        stable = (used >= 2) & (start < window_size - 2) & ~(start > window_size * 3.0 / 4.0) & ~(depth <= 0)
+        margin = stable & (start == 0) & (used <= 2) & numbered
+        e = np.nonzero(stable)[0]
+        xy = np.array([self.bearing[a][self.idx[k, a]] for k, a in zip(e, self.anchor[e])]).reshape(-1, 2)
+        d = depth[e]
+        pc = np.stack([xy[:, 0] * d, xy[:, 1] * d, d], -1)
+        s = start[e]
+        xyz = np.einsum("kij,kj->ki", np.asarray(cam_R)[s], pc) + np.asarray(cam_t)[s]
+        return xyz, self.id[e].astype(np.int32), margin[e]
+
+
+def quat_matrix(q):
+    """rotation matrices [n, 3, 3] of unit quaternions [n, 4] (x, y, z, w)"""
+    q = np.asarray(q, np.float64).reshape(-1, 4)
+    return np.stack([syn.qrot(q, np.broadcast_to(np.eye(3)[j], (len(q), 3))) for j in range(3)], -1)
+
+
+def camera_poses(q_imu, p_imu):
+    """the camera pose of IMU poses (x, y, z, w quaternions [n, 4], positions [n, 3]) through the configured extrinsic
+    (GetCameraPose): R_c = R R_CI, t_c = p + R p_CI, R_CI from the configured quaternion.  Returns (R_c [n, 3, 3],
+    t_c [n, 3])."""
+    R = quat_matrix(q_imu)
+    R_CI = quat_matrix(syn.Q_CtoI)[0]
+    return R @ R_CI, np.asarray(p_imu, np.float64).reshape(-1, 3) + R @ syn.P_CinI
+
 
 class ResidentRunner(StreamingRunner):
     """The same per-image cycle with the window living in HBM: the new image's PointCloud and the new IMUData records go
@@ -538,14 +587,23 @@ class ResidentRunner(StreamingRunner):
     landmarks are numbered and their inverse depths re-laid out by FeatureTableWindow, the triangulation and the image
     factors come from the table, and the leaving frame's slot leaves it at the end of the step (FeatureTableSlide).  No
     host association is used: the caller passes only frame slots.  Default (False): the host derives the landmark
-    numbering and the factor index tables from the sequence's ground-truth association, as before."""
+    numbering and the factor index tables from the sequence's ground-truth association, as before.
 
-    def __init__(self, lib, seq, triangulate=False, device_features=False, **kw):
+    publish_map=True (requires device_features=True): right after FeatureTableSlide, inside the timed region, the
+    landmark map and keyframe poses the reference publishes after every image (GetLandmarksInWindow, GetMarginCloud,
+    PublishVioKeyFrame) come from the device (FeatureTableMap over the post-slide window).  The arrays (xyz, ids,
+    in_margin, cam_q, cam_p) are kept on last_map, and the record gains n_map_points and n_margin_points."""
+
+    def __init__(self, lib, seq, triangulate=False, device_features=False, publish_map=False, **kw):
         if device_features and not triangulate:
             raise ValueError("device_features requires triangulate=True: new landmarks enter with inverse depth -1")
+        if publish_map and not device_features:
+            raise ValueError("publish_map requires device_features=True: the map is read from the resident feature table")
         super().__init__(lib, seq, **kw)
         self.triangulate = triangulate
         self.device_features = device_features
+        self.publish_map = publish_map
+        self.last_map = None
         self.triangulate_probe = None
         if self.clouds is None:
             self.clouds = FrameClouds(seq)
@@ -729,6 +787,8 @@ class ResidentRunner(StreamingRunner):
         n_removed = None
         if self.device_features:                       # the leaving frame's landmarks and observations leave the table
             n_removed = e.FeatureTableSlide(self.slot_of[self.frames[0 if marg else -2]])
+        if self.publish_map:                           # the landmark map and keyframe poses of the post-slide window
+            self.last_map = e.FeatureTableMap(np.delete(frame_slots, 0 if marg else len(frame_slots) - 2), WINDOW_SIZE)
         t_wall = time.perf_counter() - t_start
         h2d, d2h = (0, 0) if first else e.TransferStats(reset=True)
 
@@ -753,6 +813,8 @@ class ResidentRunner(StreamingRunner):
         if self.device_features:
             # n_new_lm: the window's landmarks without a depth yet (-1), which are exactly the ones TriangulateWindow wrote
             rec.update(n_triangulated=n_tri, n_fallback=n_fb, n_new_lm=n_tri + n_fb, n_removed=n_removed)
+            if self.publish_map:
+                rec.update(n_map_points=len(self.last_map[1]), n_margin_points=int(self.last_map[2].sum()))
         elif self.triangulate:
             rec.update(n_triangulated=n_tri, n_fallback=n_fb, n_new_lm=int(np.sum(old_index < 0)))
         self.records.append(rec)

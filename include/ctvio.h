@@ -390,6 +390,44 @@ int ctvio_feature_table_slide(ctvio_handle h, int32_t frame_slot, int32_t* n_rem
  *   array; CTVIO_ERR_STATE without a window since the last add / slide. */
 int ctvio_feature_table_landmarks(ctvio_handle h, int32_t n_landmarks, int32_t* feature_id, int32_t* anchor_slot,
                                   int32_t* used_num);
+/* ctvio_feature_table_map - the landmark map and keyframe poses the reference publishes after every image, right after
+ *   SlideWindow (odometry_manager.cpp:281-288): GetLandmarksInWindow, GetMarginCloud (visual_odometry.cpp:310-372) and
+ *   PublishVioKeyFrame(Ps_).  Call it after ctvio_feature_table_slide with frame_slots[0 .. n_frames-1], the post-slide
+ *   window oldest to newest (MARGIN_OLD dropped position 0, MARGIN_SECOND_NEW the second-newest); it is valid whenever the
+ *   listed slots are exactly the slots the table holds.  It only reads: neither the table nor the state changes.
+ *   Per entry, in table order (the reference's std::list order): start = position of its anchor slot in the list,
+ *   used_num = 1 + its observations in the other listed slots, depth = 1 / rho, where rho is the resident inverse depth
+ *   of its number in the last window when it has one (what the next setDepth gives it), else its stored inverse depth
+ *   (-1 for an entry never initialised).
+ *   Stable (IsLandMarkStable, visual_odometry.h:82-93, as written there): used_num >= 2 && start < window_size - 2 &&
+ *   !(start > window_size * 3.0 / 4.0) && !(depth <= 0), so a NaN depth passes, as in the reference.
+ *   Margin cloud (GetMarginCloud): stable, start == 0, used_num <= 2 and solve_flag == SovelSucc.  The table keeps no
+ *   solve_flag; setDepth gives SovelSucc to a numbered entry whose depth is not < 0 (removeFailures has already removed
+ *   the others), so this is "numbered in the last window", which stable's depth test already makes SovelSucc (a NaN depth
+ *   included).  An entry with start == 0 after the slide was a candidate in the last window under both slide rules
+ *   (window_size >= 4): its anchor sat at position 1 (MARGIN_OLD) or 0 (MARGIN_SECOND_NEW), below window_size - 2, and a
+ *   slide only takes observations away, so its used_num was at least 2 then as well.
+ *   World point (Rs_[start] * (point * estimated_depth) + Ps_[start]): p_w = R_c ((x, y, 1) depth) + t_c, (x, y) the anchor
+ *   observation's bearing in the frame table, (R_c, t_c) the camera pose at the anchor slot's frame time
+ *   (GetCameraPose(timestamps_[i]), :197-202, not the row time): the resident spline composed with the configured
+ *   extrinsic, R_c = R R_CI, t_c = p + R p_CI.
+ *   Outputs: the stable points, compacted in table order: xyz_world[k][3], feature_id[k], in_margin_cloud[k] (0 / 1).
+ *   *n_points receives their count whenever the map was computed (on success, and with a capacity below it, in which case
+ *   the call returns CTVIO_ERR_INVALID and writes no point).  cam_q_xyzw[n_frames][4] and cam_p_xyz[n_frames][3] (either
+ *   may be NULL) receive the listed frames' camera poses at the frame time: the reference's Rs_ / Ps_.
+ *   Deviation (inherited from the table, see above): the entries anchored in the leaving frame have left with it, so they
+ *   are not in the map; the reference re-anchors them (removeBackShiftDepth).
+ *   Errors (nothing is written to the caller's arrays): CTVIO_ERR_INVALID for n_frames outside 1..16, a slot outside
+ *   0..15, a repeated slot, window_size < 3, a negative or too small capacity, or NULL point arrays with capacity > 0;
+ *   CTVIO_ERR_STATE before the knots are set, when the listed slots are not exactly the slots the table holds, or when the
+ *   resident inverse-depth count differs from the last window's landmark count; CTVIO_ERR_TIME_RANGE when a listed frame
+ *   time falls outside the spline.
+ *   One launch (plus the knot-pair table when it is stale), nothing goes up (the slots travel as launch parameters), one
+ *   stream synchronise: the kernel writes the points, the poses and the count straight into mapped host memory.
+ *   ctvio_transfer_stats counts d2h = 8 + 56 n_frames + 32 n_points bytes (count, 7 doubles per pose, 32-byte records). */
+int ctvio_feature_table_map(ctvio_handle h, int32_t n_frames, const int32_t* frame_slots, int32_t window_size,
+                            int32_t capacity, double* xyz_world, int32_t* feature_id, uint8_t* in_margin_cloud,
+                            int32_t* n_points, double* cam_q_xyzw, double* cam_p_xyz);
 
 /* bytes moved host<->device by the C-ABI calls since the last reset (state, factors, priors, index tables) */
 int ctvio_transfer_stats(ctvio_handle h, int64_t* h2d_bytes, int64_t* d2h_bytes, int32_t reset);
