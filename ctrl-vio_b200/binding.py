@@ -111,7 +111,7 @@ ABI_SYMBOLS = [
 
 # entry points a checker library (the CPU oracle mirrors the ABI under `ctvo_`) need not provide: multi-GPU plumbing and
 # the device-residency / wire-format calls, which have no CPU meaning
-DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enable_prior", "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior",
+DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enable_prior", "extend_knots_to", "slide_window", "remap_landmarks",
                        "ingest_feature_cloud", "add_image_features_from_slots", "ingest_imu", "add_imu_from_table",
                        "transfer_stats", "residual_summary", "triangulate_window", "check_keyframe",
                        "slide_window_second_new", "feature_table_add", "feature_table_window", "triangulate_window_from_table",

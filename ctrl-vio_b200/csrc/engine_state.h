@@ -1,0 +1,308 @@
+// The engine object behind a ctvio_handle and the host helpers engine.cu and resident.cu share.  The thread-locals are
+// C++17 inline variables, ONE object each across the library: an error raised in either file is what ctvio_last_error
+// reports, and every upload is counted.
+#pragma once
+#include <algorithm>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "../../include/ctvio.h"
+#include "frontend.h"      // + kernels.h
+#include "marginalize.h"
+
+namespace ctvio::host {
+
+inline thread_local std::string g_err;  // ctvio_last_error
+inline int fail(int code, const std::string& msg) {
+  g_err = msg;
+  return code;
+}
+
+#define CUDA_OK(call)                                                                                   \
+  do {                                                                                                  \
+    cudaError_t e_ = (call);                                                                            \
+    if (e_ != cudaSuccess)                                                                              \
+      return fail(CTVIO_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_));                  \
+  } while (0)
+
+inline thread_local size_t g_upload_bytes = 0;  // bytes moved by DevBuf::upload (index tables etc.), see ctvio_transfer_stats
+
+// Pinned staging arena of one engine: every host -> device copy of a C-ABI call is staged here and issued as a truly
+// asynchronous copy (a cudaMemcpyAsync from pageable memory is a synchronous staged copy, and there are ~20 of them per
+// window).  The arena is rewound whenever the engine's stream is found idle at the start of a call (then every copy that
+// read from it has completed); a request that does not fit falls back to the pageable copy and grows the arena at the
+// next rewind.
+struct PinnedArena {
+  unsigned char* base = nullptr;
+  size_t cap = 0, need = 0;  // need: bytes requested since the last rewind (may exceed cap: those requests fell back)
+  ~PinnedArena() { if (base) cudaFreeHost(base); }
+  void rewind() {
+    if (need > cap) {
+      if (base) cudaFreeHost(base);
+      base = nullptr;
+      cap = 0;
+      const size_t n = std::max<size_t>(size_t(1) << 20, need + need / 2);
+      if (cudaHostAlloc(reinterpret_cast<void**>(&base), n, cudaHostAllocDefault) == cudaSuccess) cap = n;
+      else cudaGetLastError();
+    }
+    need = 0;
+  }
+  void* put(const void* src, size_t bytes) {
+    const size_t o = (need + 15) & ~size_t(15);
+    need = o + bytes;
+    if (!base || need > cap) return nullptr;
+    std::memcpy(base + o, src, bytes);
+    return base + o;
+  }
+};
+inline thread_local PinnedArena* g_arena = nullptr;  // arena of the engine whose C-ABI call is running on this thread
+
+inline cudaError_t staged_h2d(void* dst, const void* src, size_t bytes, cudaStream_t s) {
+  if (bytes == 0) return cudaSuccess;
+  if (g_arena) {
+    if (void* st = g_arena->put(src, bytes)) return cudaMemcpyAsync(dst, st, bytes, cudaMemcpyHostToDevice, s);
+  }
+  // pageable source: the runtime stages it synchronously, the caller's buffer is free again on return
+  return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s);
+}
+
+template <typename T>
+struct DevBuf {
+  T* p = nullptr;
+  size_t cap = 0;
+  ~DevBuf() { if (p) cudaFree(p); }
+  cudaError_t reserve(size_t n) {
+    if (n <= cap) return cudaSuccess;
+    if (p) cudaFree(p);
+    p = nullptr;
+    cap = 0;
+    cudaError_t e = cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T));
+    if (e == cudaSuccess) cap = n;
+    return e;
+  }
+  // reallocate to at least n elements that start with elements [from, from + count) of the old buffer (count = 0: a plain
+  // reallocation); the stream is synchronised before the old buffer is freed, since work in flight may still read it
+  cudaError_t grow(size_t n, size_t from, size_t count, cudaStream_t s) {
+    DevBuf<T> nb;
+    cudaError_t e = nb.reserve(n);
+    if (e == cudaSuccess && count) e = cudaMemcpyAsync(nb.p, p + from, count * sizeof(T), cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) swap(*this, nb);
+    return e;
+  }
+  cudaError_t upload(const std::vector<T>& h, cudaStream_t s) {
+    cudaError_t e = reserve(h.size());
+    if (e != cudaSuccess || h.empty()) return e;
+    g_upload_bytes += h.size() * sizeof(T);
+    return staged_h2d(p, h.data(), h.size() * sizeof(T), s);
+  }
+};
+template <typename T>
+void swap(DevBuf<T>& a, DevBuf<T>& b) { std::swap(a.p, b.p); std::swap(a.cap, b.cap); }
+
+struct DevState {
+  DevBuf<double> q, p, bias, rho, ld;
+  DevBuf<KnotPair> tab;
+  StatePtrs ptrs() { return StatePtrs{q.p, p.p, bias.p, rho.p, ld.p, tab.p}; }
+};
+
+struct HostImage { int64_t ti, tj; int32_t rowi, rowj; double pi[2], pj[2]; int32_t lm, marg; };
+struct HostImu { int64_t t; double gyro[3], accel[3]; int32_t node, marg; };
+struct HostBias { int32_t i, j; double s[6]; int32_t marg; };
+
+}  // namespace ctvio::host
+
+using namespace ctvio;
+using namespace ctvio::host;
+
+struct ctvio_engine {
+  ctvio_config cfg;
+  ctvio_options opt;
+  cudaStream_t stream = nullptr, stream2 = nullptr, stream3 = nullptr;  // stream2 / stream3: IMU and bias / prior factors run
+                                                                         // beside the visual kernel
+  cudaEvent_t ev_join3 = nullptr;
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_fork = nullptr, ev_join = nullptr;
+  bool masks_dirty = true;
+  SplineParams sp;
+  RigParams rig;
+  bool deterministic = false;   // ctvio_set_deterministic: ordered flushes, single stream (kernels.h)
+  DevBuf<int32_t> d_ticket;     // [0] kernel flush ticket, [1] scalar flush ticket
+
+  // sizes
+  int nK = 0, nB = 0, nL = 0;
+  bool have_knots = false, have_bias = false, have_rho = false;
+
+  // state: two buffers (current / candidate) + snapshot
+  DevState x[2], snap;
+  DevState xs;                 // third state buffer of the pipelined LM driver (swapped into x[] when it ends up current)
+  DevBuf<LmDecision> d_dec;    // device-side step decision (accept, next radius) read by the speculated linear solve
+  cudaEvent_t ev_iter = nullptr;  // recorded behind the last kernel of every LM step (before anything speculative)
+  DevState& state(int i) { return i < 2 ? x[i] : xs; }
+  int cur = 0;
+  bool table_valid = false;
+
+  // factors (host copies in caller order)
+  std::vector<HostImage> img;
+  std::vector<HostImu> imu;
+  std::vector<HostBias> biasf;
+  bool structure_dirty = true;
+
+  // device factor arrays
+  DevBuf<longlong2> d_img_t;
+  DevBuf<double2> d_img_pi, d_img_pj;
+  DevBuf<int4> d_img_meta;
+  DevBuf<int32_t> d_img_orig;
+  DevBuf<VisualItem> d_items;
+  int n_items = 0;
+  std::vector<int32_t> img_order;  // sorted position -> original index
+  std::vector<int32_t> img_li, img_lj;    // ... and the last knot of those windows
+  std::vector<int32_t> img_wi0, img_wj0;  // first knot of the padded anchor / observation window per factor (caller order)
+  std::vector<VisualItem> h_items;        // K1 work items (one per chunk of a frame-pair group)
+  std::vector<int32_t> imu_order;
+  DevBuf<longlong2> d_imu_t;
+  DevBuf<double2> d_imu_ga;
+  DevBuf<ImuItem> d_imu_items;
+  DevBuf<int32_t> d_imu_orig;
+  int n_imu_items = 0;
+  DevBuf<int2> d_bf_ij;
+  DevBuf<double> d_bf_s;
+
+  // landmark layout / schur batches
+  std::vector<int32_t> h_lo, h_hi;
+  std::vector<int64_t> h_woff;
+  DevBuf<int32_t> d_lo, d_hi;
+  DevBuf<SchurEntry> d_schur_list;
+  DevBuf<int64_t> d_woff;
+  DevBuf<SchurTileItem> d_schur_items;
+  DevBuf<double> d_lis, d_lc;
+  int n_schur_items = 0;
+  DevBuf<uint8_t> d_cmask, d_active;
+  std::vector<uint8_t> h_cmask, h_active;
+
+  // normal equations (two buffers, each one slab: A | gc | hl | gl | wld | W)
+  DevBuf<double> ne_slab[2];
+  size_t ne_slab_len = 0;
+  size_t off_gc = 0, off_hl = 0, off_gl = 0, off_wld = 0, off_W = 0;
+  // linear system
+  DevBuf<double> d_M, d_Linv, d_y, d_sc, d_sl, d_hh, d_dc, d_dl, d_rho_sync, d_chol_part;
+  DevBuf<int32_t> d_chol_flags;
+  DevBuf<uint8_t> d_owned;
+  DevBuf<double> d_shard_pack, d_shard_scal;  // sharded mode: packed all-reduce buffer, scalar all-gather buffer
+  int npad = 0, linv_npad = -1;
+  unsigned chol_seq = 0;  // tile-DAG launches so far (packet buffer parity)
+  DevBuf<LmScalars> d_scal;
+  LmScalars* h_scal = nullptr;  // pinned
+  LmPublished* h_pub = nullptr; // pinned + mapped: written by the last kernel of an LM step
+  unsigned long long pub_seq = 0;
+  cudaEvent_t ev_zero = nullptr;
+  bool slab_zeroed[2] = {false, false};  // the normal-equation buffer was cleared ahead of time on stream2
+
+  // prior
+  ctvio::PriorHost prior, new_prior;
+  DevBuf<double> d_prior_J, d_prior_r, d_prior_JtJ, d_prior_x0, d_prior_dx, d_prior_res;
+  DevBuf<int32_t> d_prior_type, d_prior_index, d_prior_col, d_prior_col2g;
+  bool prior_dirty = true;
+  bool prior_enabled = true;      // ctvio_enable_prior: estimators without the prior (InitTrajectory) keep it resident
+  bool prior_on_device = false;   // the active prior's J / r / x0 / J'J were adopted device-to-device (host vectors empty)
+  bool new_prior_on_host = false; // ctvio_get_prior has fetched the freshly marginalized prior's J / r / x0
+  DevBuf<double> d_newprior_x0;
+  // wire-format ingestion (resident.cu, frontend.cu): resident per-frame feature tables, resident IMU table
+  static constexpr int kFrameSlots = ctvio::kKeyframeMaxSlots, kFrameCap = ctvio::kKeyframeMaxFeatures;  // 16, 1024
+  DevBuf<ctvio::FrameFeature> d_frames;   // [kFrameSlots][kFrameCap]
+  DevBuf<int64_t> d_frame_t;              // [kFrameSlots]
+  DevBuf<float> d_cloud_stage;            // staging for one message (5 floats per point... points 3 + id + v)
+  int64_t h_frame_t[16] = {0};
+  int32_t h_frame_n[16] = {0};
+  std::vector<ctvio::FactorDesc> img_desc;  // parallel to img when the factors came from the resident tables
+  DevBuf<ctvio::FactorDesc> d_img_desc;
+  DevBuf<longlong2> d_imu_tab_t;           // resident IMU table {t, 0}
+  DevBuf<double2> d_imu_tab_ga;            // [cap][3]
+  DevBuf<unsigned char> d_imu_raw;
+  std::vector<int64_t> h_imu_tab_t;        // host mirror: timestamps only
+  std::vector<int32_t> imu_src;            // parallel to imu when the samples came from the resident table (table index)
+  DevBuf<int2> d_imu_src;
+  PinnedArena arena;
+  // pinned host mirror of the state, refreshed by the calls that end with a stream synchronisation anyway (solve,
+  // re-alignment): the getters then cost a memcpy instead of a device copy + synchronise each
+  double* h_mirror = nullptr;
+  size_t h_mirror_cap = 0;
+  bool mirror_valid = false;
+  size_t h2d_bytes = 0, d2h_bytes = 0;     // bytes moved by the C-ABI calls since ctvio_transfer_stats(reset)
+
+  DevBuf<double> d_tmp;  // scratch (gauge inputs, probe outputs)
+  DevBuf<int32_t> d_tri_idx;  // index uploads: ctvio_triangulate, ctvio_remap_landmarks, ctvio_triangulate_window
+  DevBuf<int32_t> d_tri_cnt;  // ctvio_triangulate_window: {triangulated, fallback}
+  DevBuf<ctvio::KeyframeResult> d_kf_result;  // ctvio_check_keyframe
+  uint32_t h_frame_ingested = 0;  // frame slots holding a cloud from ctvio_ingest_feature_cloud (cleared when the table slides it)
+  // resident feature table (ctvio_feature_table_*), allocated at full size on first use
+  struct FeatureTable {
+    DevBuf<int32_t> id, anchor, lm, idx, new_index;
+    DevBuf<uint32_t> mask;
+    DevBuf<double> rho;
+    DevBuf<uint64_t> key[2];  // sorted (id, entry) keys, ping-pong
+    int cur_key = 0;
+    DevBuf<int32_t> obs_offset, obs_slot, obs_idx, lm_id, lm_anchor, lm_used, result;
+    DevBuf<ctvio::FactorDesc> desc;
+    int n_entries = 0;
+    uint32_t held = 0;            // frame slots whose cloud the table holds
+    int n_lm = -1;                // landmarks of the last window (-1: none yet); the resident inverse depths follow it
+    int n_obs = 0;
+    bool window_current = false;  // the CSR and records describe the table as it is (no add / slide since the window)
+    int32_t oldest_slot = 0;
+    // ctvio_feature_table_map's output, written by its kernel: pinned + mapped, allocated on first use
+    ctvio::MapHeader* h_map_head = nullptr;
+    ctvio::MapPoint* h_map_points = nullptr;
+    ctvio::FeatureTablePtrs ptrs() { return ctvio::FeatureTablePtrs{id.p, anchor.p, mask.p, lm.p, rho.p, idx.p}; }
+  } ft;
+  // marginalization workspace (K7), kept across windows: allocation / free costs more than the kernels
+  struct MargWs {
+    DevBuf<int32_t> pos_cam, pos_lm, prior_pos, marg_img, marg_imu;
+    DevBuf<int2> bij;
+    DevBuf<double> eig_scratch, Jrow, bs, A, b, Amm, V, ev, Vs, Ainv, T, Ap, bp, Ap2, V2, ev2, vb, J, r;
+  } mws;
+
+  // multi-GPU
+  void* nccl_comm = nullptr;
+  int rank = 0, world = 1;
+  bool shard_checked = false;  // landmark ownership verified for the current factor set
+
+  int64_t launches = 0;
+
+  ProblemDims dims() const {
+    ProblemDims d;
+    d.nK = nK; d.nB = nB; d.nL = nL;
+    d.idx_bias0 = 6 * nK;
+    d.idx_ld = 6 * nK + 6 * nB;
+    d.np = d.idx_ld + 1;
+    return d;
+  }
+  NormalEqPtrs ne(int b) {
+    double* s = ne_slab[b].p;
+    return NormalEqPtrs{s, s + off_gc, s + off_hl, s + off_gl, s + off_wld, s + off_W, &d_scal.p->cost_eval};
+  }
+  LandmarkLayout lml() { return LandmarkLayout{d_lo.p, d_hi.p, d_woff.p}; }
+};
+
+namespace ctvio::host {
+
+// RAII: route this thread's uploads through the engine's arena for the duration of one C-ABI call
+struct ArenaScope {
+  PinnedArena* prev;
+  explicit ArenaScope(ctvio_engine* e) : prev(g_arena) {
+    if (e->stream && cudaStreamQuery(e->stream) == cudaSuccess) e->arena.rewind();  // idle: nothing reads the arena any more
+    else cudaGetLastError();
+    g_arena = &e->arena;
+  }
+  ~ArenaScope() { g_arena = prev; }
+};
+
+inline int ensure_table(ctvio_engine* e) {
+  if (!e->table_valid) {
+    e->launches += launch_knot_table(e->x[e->cur].ptrs(), e->nK, e->stream);
+    e->table_valid = true;
+  }
+  return CTVIO_OK;
+}
+
+}  // namespace ctvio::host

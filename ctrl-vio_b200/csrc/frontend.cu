@@ -220,11 +220,11 @@ __global__ void __launch_bounds__(kKfThreads) keyframe_parallax_kernel(KeyframeA
   __shared__ double s_par[kKeyframeMaxFeatures];       // parallax of feature i of slot fc-1 (0: not a parallax feature)
   __shared__ uint8_t s_tracked[kKeyframeMaxFeatures];  // feature i of the new slot occurs in another listed slot
   const int tid = threadIdx.x;
-  const int fc = a.n_frames - 1;  // frame_count
+  const int fc = a.w.n_frames - 1;  // frame_count
   const int n_new = a.count[fc];
   const int n_old = fc >= 2 ? a.count[fc - 2] : 0;
-  const FrameFeature* t_new = a.table + size_t(a.slot[fc]) * a.frame_cap;
-  const FrameFeature* t_old = fc >= 2 ? a.table + size_t(a.slot[fc - 2]) * a.frame_cap : nullptr;
+  const FrameFeature* t_new = a.table + size_t(a.w.slot[fc]) * a.frame_cap;
+  const FrameFeature* t_old = fc >= 2 ? a.table + size_t(a.w.slot[fc - 2]) * a.frame_cap : nullptr;
   s_key[0][tid] = tid < n_new ? kf_key(t_new[tid].id, tid) : ~0ull;
   s_key[1][tid] = tid < n_old ? kf_key(t_old[tid].id, tid) : ~0ull;
   s_par[tid] = 0.0;
@@ -235,7 +235,7 @@ __global__ void __launch_bounds__(kKfThreads) keyframe_parallax_kernel(KeyframeA
   bitonic_sort_shared<N>(s_key[tid / (N / 2)], tid % (N / 2), true);
   // last_track_num (:38-57): the new image's features whose id is already in the window
   for (int f = 0; f < fc; ++f) {
-    const FrameFeature* t = a.table + size_t(a.slot[f]) * a.frame_cap;
+    const FrameFeature* t = a.table + size_t(a.w.slot[f]) * a.frame_cap;
     for (int i = tid; i < a.count[f]; i += kKfThreads) {
       const int hit = kf_find(s_key[0], n_new, t[i].id);
       if (hit >= 0) s_tracked[hit] = 1;
@@ -244,7 +244,7 @@ __global__ void __launch_bounds__(kKfThreads) keyframe_parallax_kernel(KeyframeA
   // parallax features (:62-72): start_frame <= fc-2 && endFrame() >= fc-1, i.e. seen in slots fc-2 and fc-1
   bool parallax_feature = false;
   if (fc >= 2 && tid < a.count[fc - 1]) {
-    const FrameFeature fj = a.table[size_t(a.slot[fc - 1]) * a.frame_cap + tid];
+    const FrameFeature fj = a.table[size_t(a.w.slot[fc - 1]) * a.frame_cap + tid];
     const int i = kf_find(s_key[1], n_old, fj.id);
     if (i >= 0) {
       // compensatedParallax2 (:424-456) with z == 1: the compensated and the plain distance coincide.  The products are
@@ -428,8 +428,8 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_window_kernel(Featur
       if (lm >= 0 && lm < a.n_rho_in) { rho = a.rho_in[lm]; t.rho[e] = rho; }  // setDepth (feature_manager.cpp:126-147)
       mask = t.mask[e];
       anchor = t.anchor[e];
-      used = __popc(mask & a.listed);
-      cand = used >= 2 && a.position[anchor] < a.window_size - 2;
+      used = __popc(mask & a.w.listed);
+      cand = used >= 2 && a.w.position[anchor] < a.window_size - 2;
     }
     int n_cand, n_used;
     const int rl = block_exclusive_scan(cand, s_scan, n_cand);
@@ -445,8 +445,8 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_window_kernel(Featur
       a.lm_used[l] = used;
       a.obs_slot[o] = anchor;
       a.obs_idx[o++] = t.idx[anchor * S + e];
-      for (int k = 0; k < a.n_frames; ++k) {
-        const int s = a.slot[k];
+      for (int k = 0; k < a.w.n_frames; ++k) {
+        const int s = a.w.slot[k];
         if (s != anchor && ((mask >> s) & 1u)) { a.obs_slot[o] = s; a.obs_idx[o++] = t.idx[s * S + e]; }
       }
     }
@@ -479,10 +479,10 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_map_kernel(FeatureTa
   const int tid = threadIdx.x;
   const FeatureTablePtrs& t = a.t;
   constexpr size_t S = kFeatureTableMaxEntries;
-  if (tid < a.n_frames) {
+  if (tid < a.w.n_frames) {
     int32_t s;
     double u;
-    spline_index(a.sp, a.frame_t[a.slot[tid]], s, u);
+    spline_index(a.sp, a.frame_t[a.w.slot[tid]], s, u);
     SideEval ev;
     eval_side<false, kPStride>(a.sp, a.st.q, a.st.p, a.st.tab, s, u, ev);
     const M3 Rc = m3_mul(ev.R, a.R_CI);        // R_c = R * R_CI  (as triangulate_window_kernel)
@@ -504,8 +504,8 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_map_kernel(FeatureTa
     MapPoint p;
     if (e < a.n_entries) {
       const int anchor = t.anchor[e], lm = t.lm[e];
-      const int start = a.position[anchor];
-      const int used = __popc(t.mask[e] & a.listed);
+      const int start = a.w.position[anchor];
+      const int used = __popc(t.mask[e] & a.w.listed);
       const bool numbered = lm >= 0 && lm < a.n_rho;
       const double depth = 1.0 / (numbered ? a.rho[lm] : t.rho[e]);  // the next setDepth's value, else the stored one
       // isLandmarkCandidate, start_frame > WINDOW_SIZE * 3 / 4, estimated_depth <= 0 (a NaN depth passes)

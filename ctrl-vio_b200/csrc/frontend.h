@@ -95,10 +95,18 @@ struct TriangulateWindowArgs {
 };
 int launch_triangulate_window(const TriangulateWindowArgs& a, cudaStream_t s);
 
-// Keyframe decision of the new image (addFeatureCheckParallax, feature_manager.cpp:28-87) over resident frame slots:
-// slot[0 .. n_frames-1] lists the window oldest to newest, the last one the new image.  One CTA of
-// kKeyframeMaxFeatures threads; every slot holds at most kKeyframeMaxFeatures features.
 constexpr int kKeyframeMaxSlots = 16, kKeyframeMaxFeatures = 1024;
+// a window listed by the caller as resident frame slots, oldest to newest (each slot at most once)
+struct WindowSlots {
+  int32_t n_frames;                     // 1 .. kKeyframeMaxSlots
+  int32_t slot[kKeyframeMaxSlots];      // frame slot of each window position
+  int32_t position[kKeyframeMaxSlots];  // window position of each frame slot (-1: not listed)
+  uint32_t listed;                      // mask of the listed slots
+};
+
+// Keyframe decision of the new image (addFeatureCheckParallax, feature_manager.cpp:28-87) over resident frame slots:
+// w.slot[0 .. n_frames-1] lists the window oldest to newest, the last one the new image.  One CTA of
+// kKeyframeMaxFeatures threads; every slot holds at most kKeyframeMaxFeatures features.
 struct KeyframeResult {
   int32_t is_keyframe;
   int32_t n_tracked;     // features of the new slot whose id occurs in another listed slot (last_track_num)
@@ -109,9 +117,8 @@ struct KeyframeResult {
 struct KeyframeArgs {
   const FrameFeature* table;  // [n_slots][frame_cap]
   int32_t frame_cap;
-  int32_t n_frames;           // 1 .. kKeyframeMaxSlots
-  int32_t slot[kKeyframeMaxSlots];
-  int32_t count[kKeyframeMaxSlots];  // features ingested in slot[k] (<= kKeyframeMaxFeatures)
+  WindowSlots w;
+  int32_t count[kKeyframeMaxSlots];  // features ingested in w.slot[k] (<= kKeyframeMaxFeatures)
   double min_parallax;        // MIN_PARALLAX
   KeyframeResult* out;
 };
@@ -154,10 +161,7 @@ struct FeatureTableSlideArgs {
 struct FeatureTableWindowArgs {
   FeatureTablePtrs t;
   int32_t n_entries;
-  int32_t n_frames;
-  int32_t slot[kKeyframeMaxSlots];      // the window, oldest to newest
-  int32_t position[kKeyframeMaxSlots];  // window position of each frame slot (-1: not listed)
-  uint32_t listed;                      // mask of the listed slots
+  WindowSlots w;
   int32_t window_size;
   const double* rho_in;        // resident inverse depths of the last numbering
   int32_t n_rho_in;            // their count (0: no numbering)
@@ -197,10 +201,7 @@ struct MapHeader {
 struct FeatureTableMapArgs {
   FeatureTablePtrs t;          // read only
   int32_t n_entries;
-  int32_t n_frames;
-  int32_t slot[kKeyframeMaxSlots];      // the window, oldest to newest
-  int32_t position[kKeyframeMaxSlots];  // window position of each frame slot (-1: not listed)
-  uint32_t listed;                      // mask of the listed slots
+  WindowSlots w;
   int32_t window_size;
   const FrameFeature* table;   // [n_slots][frame_cap]
   const int64_t* frame_t;      // [n_slots]; every listed frame time lies inside the spline (checked by the caller)
