@@ -105,7 +105,7 @@ ABI_SYMBOLS = [
     "ingest_imu", "add_imu_from_table", "transfer_stats", "profile_kernels", "measure_fp64_tflops", "measure_fp64_tensor_tflops",
     "selfcheck_solver", "nccl_unique_id", "comm_init", "triangulate_window", "check_keyframe", "slide_window_second_new",
     "feature_table_add", "feature_table_window", "triangulate_window_from_table", "add_image_features_from_table",
-    "feature_table_slide", "feature_table_landmarks", "feature_table_map",
+    "feature_table_slide", "feature_table_landmarks", "feature_table_map", "feature_table_slide_reanchor",
 ]
 
 
@@ -116,7 +116,7 @@ DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enab
                        "transfer_stats", "residual_summary", "triangulate_window", "check_keyframe",
                        "slide_window_second_new", "feature_table_add", "feature_table_window", "triangulate_window_from_table",
                        "add_image_features_from_table", "feature_table_slide", "feature_table_landmarks",
-                       "feature_table_map")
+                       "feature_table_map", "feature_table_slide_reanchor")
 
 
 def _addr(a):
@@ -492,6 +492,17 @@ class Estimator:
         n = C.c_int32()
         self.lib.call("feature_table_slide", self.h, C.c_int32(frame_slot), C.byref(n))
         return n.value
+
+    def FeatureTableSlideReanchor(self, frame_slots, marg_old, init_depth=5.0):
+        """removeFailures, then SlideWindowOld's removeBackShiftDepth (marg_old: frame_slots[0] leaves, its landmarks are
+        re-anchored in the next frame with their depth shifted there) or SlideWindowNew's removeFront (frame_slots[-2]
+        leaves, its landmarks seen in the newest frame are re-anchored there).  frame_slots: the window before the slide,
+        oldest to newest.  Returns (n_removed, n_reanchored)."""
+        slots = _i32(frame_slots)
+        nr, na = C.c_int32(), C.c_int32()
+        self.lib.call("feature_table_slide_reanchor", self.h, C.c_int32(slots.shape[0]), _ip(slots), C.c_int32(int(marg_old)),
+                      C.c_double(init_depth), C.byref(nr), C.byref(na))
+        return nr.value, na.value
 
     def FeatureTableLandmarks(self, n_landmarks=None):
         """(feature id, anchor slot, used_num) of each landmark of the last window"""

@@ -10,7 +10,8 @@
 //                        VisualOdometry::AddImageToWindow uses it (visual_odometry.cpp:180-183), on the resident frame
 //                        slots: tracked count of the new image and mean parallax between the two frames before it.
 //   feature_table_*_kernel  the feature list of FeatureManager (feature_manager.cpp:28-59 insertion, :111-147
-//                        getDepthVector / setDepth, :148-158 removeFailures, :341-423 the slide) as a resident table keyed
+//                        getDepthVector / setDepth, :148-158 removeFailures, :341-423 the slide, dropping or re-anchoring
+//                        the leaving frame's landmarks) as a resident table keyed
 //                        by the tracker's feature id, and the image-factor loops of trajectory_manager.cpp:206-236, :359-385.
 //                        feature_table_map_kernel publishes its landmark map (GetLandmarksInWindow / GetMarginCloud,
 //                        visual_odometry.cpp:310-372) and the keyframe camera poses (PublishVioKeyFrame).
@@ -355,10 +356,31 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_add_kernel(FeatureTa
   if (tid == 0) { a.out[0] = n_tracked; a.out[1] = n_new; }
 }
 
+// camera pose at time t (GetCameraPose, visual_odometry.cpp:197-202): the resident spline composed with the extrinsic,
+// R_c = R R_CI, t_c = p + R p_CI (as triangulate_window_kernel).  t must lie inside the spline.
+__device__ __forceinline__ void camera_pose_at(const StatePtrs& st, const SplineParams& sp, const M3& R_CI, const V3& p_CI,
+                                               int64_t t, M3& Rc, V3& tc) {
+  int32_t s;
+  double u;
+  spline_index(sp, t, s, u);
+  SideEval ev;
+  eval_side<false, kPStride>(sp, st.q, st.p, st.tab, s, u, ev);
+  Rc = m3_mul(ev.R, R_CI);
+  tc = ev.p + m3_vec(ev.R, p_CI);
+}
+
 // Slide: removeFailures (an entry numbered in the last window whose resident inverse depth is < 0), then the entries
 // anchored in the leaving slot go and every other one drops its observation there.  A stable in-place compaction of the
 // entries (a chunk is read completely before the scan's barrier, and lands at or below its own positions), then of the
 // sorted key array into key_out with the entries' new indices (a stable filter of a sorted array stays sorted).
+// kReanchor: an entry anchored in the leaving slot is re-anchored instead where the reference keeps it.  MARGIN_OLD
+// (removeBackShiftDepth, feature_manager.cpp:341-378): with >= 2 observations left, its anchor becomes the earliest
+// listed slot holding one and its depth is shifted from the camera at w.slot[0] into the camera at w.slot[1] (poses
+// evaluated first into shared memory), INIT_DEPTH when the shifted depth is not > 0.  MARGIN_SECOND_NEW (removeFront,
+// :398-423): with an observation in the newest slot, its anchor moves there and its depth is kept.  Either way the entry
+// keeps its place and id (the key array stays a stable filter), stores its inverse depth, loses its number and carries
+// solve_flag in kFeatureSolvedBit.
+template <bool kReanchor>
 __global__ void __launch_bounds__(kFtThreads) feature_table_slide_kernel(FeatureTableSlideArgs a) {
   __shared__ int s_scan[32];
   const int tid = threadIdx.x;
@@ -366,6 +388,19 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_slide_kernel(Feature
   const uint32_t bit = 1u << a.slot;
   constexpr size_t S = kFeatureTableMaxEntries;
   int kept = 0;
+  [[maybe_unused]] int n_reanchored = 0;
+  [[maybe_unused]] __shared__ double s_cam[2][12];  // kReanchor: camera R (9) | t (3) at w.slot[0], w.slot[1]
+  if constexpr (kReanchor) {
+    if (a.marg_old && tid < 2) {
+      M3 Rc;
+      V3 tc;
+      camera_pose_at(a.st, a.sp, a.R_CI, a.p_CI, a.frame_t[a.w.slot[tid]], Rc, tc);
+#pragma unroll
+      for (int k = 0; k < 9; ++k) s_cam[tid][k] = Rc.m[k];
+      s_cam[tid][9] = tc.x; s_cam[tid][10] = tc.y; s_cam[tid][11] = tc.z;
+    }
+    __syncthreads();
+  }
   for (int c = 0; c < a.n_entries; c += kFtThreads) {
     const int e = c + tid;
     const bool in = e < a.n_entries;
@@ -373,13 +408,50 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_slide_kernel(Feature
     uint32_t mask = 0;
     double rho = 0.0;
     bool keep = false;
+    [[maybe_unused]] bool reanchored = false;
     if (in) {
       id = t.id[e]; anchor = t.anchor[e]; lm = t.lm[e]; mask = t.mask[e]; rho = t.rho[e];
 #pragma unroll
       for (int s = 0; s < kKeyframeMaxSlots; ++s) idx[s] = (mask >> s) & 1u ? t.idx[s * S + e] : -1;
       const bool failed = lm >= 0 && lm < a.n_rho && a.rho[lm] < 0.0;  // SolveFail (feature_manager.cpp:148-158)
       keep = !failed && anchor != a.slot;
+      if constexpr (kReanchor) {
+        if (!failed && anchor == a.slot) {
+          const bool numbered = lm >= 0 && lm < a.n_rho;
+          const double r_now = numbered ? a.rho[lm] : rho;  // setDepth's value, else the stored one
+          const uint32_t rest = mask & ~bit & a.w.listed;
+          if (a.marg_old) {
+            if (__popc(rest) >= 2) {
+              int k = 1;
+              while (!((rest >> a.w.slot[k]) & 1u)) ++k;  // the earliest listed slot holding an observation
+              const FrameFeature f = a.table[size_t(anchor) * a.frame_cap + t.idx[anchor * S + e]];
+              const double depth = 1.0 / r_now;
+              const double* c0 = s_cam[0];
+              const double* c1 = s_cam[1];
+              const V3 pc{f.x * depth, f.y * depth, depth};  // uv_i * estimated_depth
+              double d[3];
+#pragma unroll
+              for (int r = 0; r < 3; ++r)  // w_pts_i - new_P
+                d[r] = c0[3 * r] * pc.x + c0[3 * r + 1] * pc.y + c0[3 * r + 2] * pc.z + c0[9 + r] - c1[9 + r];
+              const double z = c1[2] * d[0] + c1[5] * d[1] + c1[8] * d[2];  // (new_R^T (w_pts_i - new_P)).z
+              rho = 1.0 / (z > 0.0 ? z : a.init_depth);  // dep_j > 0, else INIT_DEPTH (a NaN falls back as well)
+              anchor = a.w.slot[k];
+              reanchored = true;
+            }
+          } else if ((rest >> a.w.slot[a.w.n_frames - 1]) & 1u) {
+            anchor = a.w.slot[a.w.n_frames - 1];
+            rho = r_now;
+            reanchored = true;
+          }
+          if (reanchored) {
+            if (numbered) mask |= kFeatureSolvedBit;  // setDepth set SovelSucc (SolveFail has left above)
+            lm = -1;
+            keep = true;
+          }
+        }
+      }
     }
+    if constexpr (kReanchor) n_reanchored += __syncthreads_count(reanchored);
     int total;
     const int r = block_exclusive_scan(keep, s_scan, total);
     if (keep) {
@@ -403,7 +475,10 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_slide_kernel(Feature
     if (ne >= 0) a.key_out[placed + r] = (x & 0xffffffff00000000ull) | uint32_t(ne);
     placed += total;
   }
-  if (tid == 0) a.out[0] = a.n_entries - kept;
+  if (tid == 0) {
+    a.out[0] = a.n_entries - kept;
+    if constexpr (kReanchor) a.out[1] = n_reanchored;
+  }
 }
 
 // Window: setDepth of the last window's landmarks, then the numbering of getDepthVector (isLandmarkCandidate: used_num >= 2
@@ -480,13 +555,9 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_map_kernel(FeatureTa
   const FeatureTablePtrs& t = a.t;
   constexpr size_t S = kFeatureTableMaxEntries;
   if (tid < a.w.n_frames) {
-    int32_t s;
-    double u;
-    spline_index(a.sp, a.frame_t[a.w.slot[tid]], s, u);
-    SideEval ev;
-    eval_side<false, kPStride>(a.sp, a.st.q, a.st.p, a.st.tab, s, u, ev);
-    const M3 Rc = m3_mul(ev.R, a.R_CI);        // R_c = R * R_CI  (as triangulate_window_kernel)
-    const V3 tc = ev.p + m3_vec(ev.R, a.p_CI);  // t_c = p + R * p_CI
+    M3 Rc;
+    V3 tc;
+    camera_pose_at(a.st, a.sp, a.R_CI, a.p_CI, a.frame_t[a.w.slot[tid]], Rc, tc);
 #pragma unroll
     for (int e = 0; e < 9; ++e) s_cam[tid][e] = Rc.m[e];
     s_cam[tid][9] = tc.x; s_cam[tid][10] = tc.y; s_cam[tid][11] = tc.z;
@@ -504,15 +575,16 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_map_kernel(FeatureTa
     MapPoint p;
     if (e < a.n_entries) {
       const int anchor = t.anchor[e], lm = t.lm[e];
+      const uint32_t mask = t.mask[e];
       const int start = a.w.position[anchor];
-      const int used = __popc(t.mask[e] & a.w.listed);
+      const int used = __popc(mask & a.w.listed);
       const bool numbered = lm >= 0 && lm < a.n_rho;
       const double depth = 1.0 / (numbered ? a.rho[lm] : t.rho[e]);  // the next setDepth's value, else the stored one
       // isLandmarkCandidate, start_frame > WINDOW_SIZE * 3 / 4, estimated_depth <= 0 (a NaN depth passes)
       stable = used >= 2 && start < a.window_size - 2 && !(start > late) && !(depth <= 0.0);
       // GetMarginCloud: start_frame == 0, used_num <= 2, solve_flag == SovelSucc (setDepth's !(depth < 0) of a numbered
-      // entry, which stable implies)
-      margin = stable && start == 0 && used <= 2 && numbered;
+      // entry, which stable implies; a re-anchored entry carries it in kFeatureSolvedBit)
+      margin = stable && start == 0 && used <= 2 && (numbered || (mask & kFeatureSolvedBit));
       if (stable) {
         const FrameFeature f = a.table[size_t(anchor) * a.frame_cap + t.idx[anchor * S + e]];
         const double* w = s_cam[start];
@@ -678,7 +750,11 @@ int launch_feature_table_add(const FeatureTableAddArgs& a, cudaStream_t s) {
   return 1;
 }
 int launch_feature_table_slide(const FeatureTableSlideArgs& a, cudaStream_t s) {
-  feature_table_slide_kernel<<<1, kFtThreads, 0, s>>>(a);
+  feature_table_slide_kernel<false><<<1, kFtThreads, 0, s>>>(a);
+  return 1;
+}
+int launch_feature_table_slide_reanchor(const FeatureTableSlideArgs& a, cudaStream_t s) {
+  feature_table_slide_kernel<true><<<1, kFtThreads, 0, s>>>(a);
   return 1;
 }
 int launch_feature_table_window(const FeatureTableWindowArgs& a, cudaStream_t s) {

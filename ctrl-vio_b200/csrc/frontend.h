@@ -127,12 +127,15 @@ int launch_keyframe_parallax(const KeyframeArgs& a, cudaStream_t s);
 // Resident feature table (FeatureManager's feature list): one entry per landmark in creation order, structure of arrays
 // over kFeatureTableMaxEntries entries.  idx[s * kFeatureTableMaxEntries + e] is entry e's feature index in frame slot s,
 // valid where bit s of mask[e] is set (the anchor slot's bit included).  The live entries' (id, entry) keys are kept
-// sorted (kf_key order) in a separate array.
+// sorted (kf_key order) in a separate array.  Bit kFeatureSolvedBit of mask[e] carries solve_flag == SovelSucc across a
+// re-anchoring slide, which clears the entry's number (only the re-anchoring slide sets it; it is never cleared).
 constexpr int kFeatureTableMaxEntries = kKeyframeMaxSlots * kKeyframeMaxFeatures;
+constexpr uint32_t kFeatureSolvedBit = 1u << 31;
+static_assert(kKeyframeMaxSlots <= 31, "the solved bit sits above the slot bits");
 struct FeatureTablePtrs {
   int32_t* id;       // tracker feature id
   int32_t* anchor;   // anchor frame slot
-  uint32_t* mask;    // slots holding an observation
+  uint32_t* mask;    // slots holding an observation (bits 0..15), kFeatureSolvedBit
   int32_t* lm;       // number in the last window, -1: not numbered
   double* rho;       // inverse depth (estimated_depth), -1: not initialised
   int32_t* idx;      // [kKeyframeMaxSlots][kFeatureTableMaxEntries]
@@ -156,7 +159,18 @@ struct FeatureTableSlideArgs {
   int32_t slot;                // the leaving slot
   const double* rho;           // resident inverse depths of the last window's numbering
   int32_t n_rho;               // their count (0: no numbering, removeFailures is skipped)
-  int32_t* out;                // {n_removed}
+  int32_t* out;                // {n_removed}; the re-anchoring slide: {n_removed, n_reanchored}
+  // the re-anchoring slide (feature_table_slide_kernel<true>) only
+  WindowSlots w;               // the window before the slide, oldest to newest (w.listed: the held slots)
+  int32_t marg_old;            // 1: slot == w.slot[0] (removeBackShiftDepth); 0: slot == w.slot[n_frames-2] (removeFront)
+  double init_depth;           // INIT_DEPTH, for a shifted depth that is not > 0
+  const FrameFeature* table;   // MARGIN_OLD: the anchor bearings, [n_slots][frame_cap]
+  int32_t frame_cap;
+  const int64_t* frame_t;      // MARGIN_OLD: w.slot[0] and w.slot[1]'s frame times lie inside the spline (caller checks)
+  StatePtrs st;                // MARGIN_OLD: knots, knot-pair table (valid)
+  SplineParams sp;
+  M3 R_CI;                     // camera -> IMU rotation
+  V3 p_CI;
 };
 struct FeatureTableWindowArgs {
   FeatureTablePtrs t;
@@ -217,6 +231,7 @@ struct FeatureTableMapArgs {
 };
 int launch_feature_table_add(const FeatureTableAddArgs& a, cudaStream_t s);
 int launch_feature_table_slide(const FeatureTableSlideArgs& a, cudaStream_t s);
+int launch_feature_table_slide_reanchor(const FeatureTableSlideArgs& a, cudaStream_t s);
 int launch_feature_table_window(const FeatureTableWindowArgs& a, cudaStream_t s);
 int launch_feature_table_factors(const FeatureTableFactorArgs& a, cudaStream_t s);
 int launch_feature_table_map(const FeatureTableMapArgs& a, cudaStream_t s);

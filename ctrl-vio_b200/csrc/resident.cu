@@ -392,6 +392,53 @@ int ctvio_feature_table_slide(ctvio_handle e, int32_t frame_slot, int32_t* n_rem
   return CTVIO_OK;
 }
 
+int ctvio_feature_table_slide_reanchor(ctvio_handle e, int32_t n_frames, const int32_t* frame_slots, int32_t marg_old,
+                                       double init_depth, int32_t* n_removed, int32_t* n_reanchored) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (!frame_slots) return fail(CTVIO_ERR_INVALID, "null argument");
+  if (n_frames < 2 || n_frames > ctvio_engine::kFrameSlots) return fail(CTVIO_ERR_INVALID, "n_frames must be 2..16");
+  if (!(init_depth > 0.0) || !std::isfinite(init_depth)) return fail(CTVIO_ERR_INVALID, "init_depth must be positive");
+  ctvio::FeatureTableSlideArgs a;
+  if (const int rc = parse_window_slots(n_frames, frame_slots, a.w)) return rc;
+  auto& t = e->ft;
+  if (a.w.listed != t.held) return fail(CTVIO_ERR_STATE, "the listed frame slots are not the slots the feature table holds");
+  if (const int rc = check_numbering(e, TableWindow::kNumbered)) return rc;
+  a.marg_old = marg_old ? 1 : 0;
+  if (a.marg_old) {
+    // removeBackShiftDepth's poses: the cameras at the leaving frame's and the next frame's time
+    if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
+    for (int k = 0; k < 2; ++k) {
+      int32_t s;
+      double u;
+      if (!spline_index(e->sp, e->h_frame_t[a.w.slot[k]], s, u))
+        return fail(CTVIO_ERR_TIME_RANGE, "a frame time of the depth shift falls outside the spline");
+    }
+  }
+  const int frame_slot = a.w.slot[a.marg_old ? 0 : n_frames - 2];
+  cudaSetDevice(e->cfg.device);
+  cudaStream_t st = e->stream;
+  if (a.marg_old) ensure_table(e);
+  a.t = t.ptrs(); a.n_entries = t.n_entries;
+  a.key_in = t.key[t.cur_key].p; a.key_out = t.key[t.cur_key ^ 1].p; a.new_index = t.new_index.p;
+  a.slot = frame_slot; a.rho = e->x[e->cur].rho.p; a.n_rho = std::max(t.n_lm, 0); a.out = t.result.p;
+  a.init_depth = init_depth;
+  a.table = e->d_frames.p; a.frame_cap = ctvio_engine::kFrameCap; a.frame_t = e->d_frame_t.p;
+  a.st = e->x[e->cur].ptrs(); a.sp = e->sp; a.R_CI = e->rig.R_CI; a.p_CI = e->rig.p_CI;
+  // the slot list goes up with the launch parameters
+  e->h2d_bytes += size_t(n_frames) * sizeof(int32_t);
+  e->launches += ctvio::launch_feature_table_slide_reanchor(a, st);
+  int32_t r[2];
+  if (const int rc = read_result(e, r, t.result.p, 2)) return rc;
+  t.cur_key ^= 1;
+  t.n_entries -= r[0];
+  t.held &= ~(1u << frame_slot);
+  t.window_current = false;
+  e->h_frame_ingested &= ~(1u << frame_slot);
+  if (n_removed) *n_removed = r[0];
+  if (n_reanchored) *n_reanchored = r[1];
+  return CTVIO_OK;
+}
+
 int ctvio_feature_table_landmarks(ctvio_handle e, int32_t n_landmarks, int32_t* feature_id, int32_t* anchor_slot,
                                   int32_t* used_num) {
   if (!e) return fail(CTVIO_ERR_INVALID, "null handle");

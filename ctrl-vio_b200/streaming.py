@@ -412,8 +412,10 @@ class FeatureTable:
 
     One entry per landmark (FeaturePerId), in creation order: the feature id, the anchor slot, the feature index of its
     observation in each of the 16 frame slots (-1: none; the anchor's own observation included), its number in the last
-    window (-1: not numbered) and its inverse depth (-1: not initialised).  Landmarks leave with their anchor frame (no
-    re-anchoring, the convention of subwindow_frames); an id seen again after its landmark left starts a new entry."""
+    window (-1: not numbered), its inverse depth (-1: not initialised) and its solved status (solve_flag == SovelSucc,
+    carried across a re-anchoring slide).  slide: landmarks leave with their anchor frame (no re-anchoring, the
+    convention of subwindow_frames); an id seen again after its landmark left starts a new entry.  slide_reanchor: they
+    are re-anchored as the reference does (removeBackShiftDepth / removeFront)."""
 
     N_SLOTS = 16
 
@@ -423,6 +425,7 @@ class FeatureTable:
         self.idx = np.full((0, self.N_SLOTS), -1, np.int32)
         self.lm = np.zeros(0, np.int32)
         self.rho = np.zeros(0)
+        self.solved = np.zeros(0, bool)
         self.held = set()            # frame slots whose cloud the table holds
         self.numbered = np.zeros(0, np.int64)   # entries of the last window, in landmark order
         self.slots = None            # the last window's frame slots, oldest to newest
@@ -446,6 +449,7 @@ class FeatureTable:
         self.idx = np.concatenate([self.idx, idx])
         self.lm = np.concatenate([self.lm, np.full(n, -1, np.int32)])
         self.rho = np.concatenate([self.rho, np.full(n, -1.0)])
+        self.solved = np.concatenate([self.solved, np.zeros(n, bool)])
         self.held.add(slot)
         self.bearing[slot] = np.asarray(message[0], np.float32)[:, :2].astype(np.float64)
         return int(tracked.sum()), n
@@ -508,10 +512,60 @@ class FeatureTable:
         fail[old] = np.asarray(rho)[self.lm[old]] < 0
         keep = ~fail & (self.anchor != slot)
         self.id, self.anchor, self.idx = self.id[keep], self.anchor[keep], self.idx[keep]
-        self.lm, self.rho = self.lm[keep], self.rho[keep]
+        self.lm, self.rho, self.solved = self.lm[keep], self.rho[keep], self.solved[keep]
         self.idx[:, slot] = -1
         self.held.discard(slot)
         return int((~keep).sum())
+
+    def slide_reanchor(self, slots, marg_old, rho, cam_R=None, cam_t=None, init_depth=5.0):
+        """the reference of ctvio_feature_table_slide_reanchor.  slots: the window before the slide, oldest to newest;
+        the leaving slot is slots[0] (marg_old) or slots[-2].  removeFailures as slide(), then an entry anchored in the
+        leaving slot:
+          marg_old (removeBackShiftDepth): with >= 2 observations left in the listed slots, its anchor becomes the
+            earliest listed slot holding one and its inverse depth 1 / p_1.z (1 / init_depth when p_1.z is not > 0), with
+            p_w = cam_R[0] (x, y, 1) depth + cam_t[0], p_1 = cam_R[1]^T (p_w - cam_t[1]), depth = 1 / its inverse depth
+            (from `rho` when numbered in the last window, else its stored one), (x, y) the old anchor's bearing; else it
+            leaves.  cam_R [>= 2, 3, 3], cam_t [>= 2, 3]: the camera poses of slots[0] and slots[1].
+          not marg_old (removeFront): with an observation in the newest slot its anchor moves there and its inverse depth
+            is kept; else it leaves.
+        A re-anchored entry keeps its place, loses its number and stays solved when it was numbered.  Every other entry
+        loses its observation in the leaving slot.  Returns (n_removed, n_reanchored)."""
+        slots = [int(x) for x in slots]
+        assert set(slots) == self.held and len(set(slots)) == len(slots) and len(slots) >= 2
+        leave = slots[0] if marg_old else slots[-2]
+        rho = np.asarray(rho, np.float64)
+        numbered = (self.lm >= 0) & (self.lm < len(rho))
+        r_now = self.rho.copy()
+        r_now[numbered] = rho[self.lm[numbered]]
+        fail = numbered & (r_now < 0)
+        keep = ~fail & (self.anchor != leave)
+        moved = np.zeros(len(self.id), bool)
+        rest = self.idx[:, slots] >= 0
+        rest[:, slots.index(leave)] = False
+        for e in np.nonzero(~fail & (self.anchor == leave))[0]:
+            if marg_old:
+                if rest[e].sum() < 2:
+                    continue
+                x, y = self.bearing[leave][self.idx[e, leave]]
+                with np.errstate(divide="ignore", invalid="ignore"):
+                    depth = 1.0 / r_now[e]
+                    p_w = np.asarray(cam_R[0]) @ np.array([x * depth, y * depth, depth]) + np.asarray(cam_t[0])
+                    z = (np.asarray(cam_R[1]).T @ (p_w - np.asarray(cam_t[1])))[2]
+                self.rho[e] = 1.0 / (z if z > 0 else init_depth)
+                self.anchor[e] = slots[int(np.argmax(rest[e]))]
+            else:
+                if not rest[e, -1]:
+                    continue
+                self.rho[e] = r_now[e]
+                self.anchor[e] = slots[-1]
+            moved[e] = keep[e] = True
+            self.solved[e] |= numbered[e]
+            self.lm[e] = -1
+        self.id, self.anchor, self.idx = self.id[keep], self.anchor[keep], self.idx[keep]
+        self.lm, self.rho, self.solved = self.lm[keep], self.rho[keep], self.solved[keep]
+        self.idx[:, leave] = -1
+        self.held.discard(leave)
+        return int((~keep).sum()), int(moved.sum())
 
     def map(self, slots, window_size, rho, cam_R, cam_t):
         """GetLandmarksInWindow / GetMarginCloud (visual_odometry.cpp:310-372) over the window's frame slots after the
@@ -520,9 +574,9 @@ class FeatureTable:
         Per entry: start = window position of its anchor, used_num = 1 + its observations in the other listed slots,
         depth = 1 / (its resident inverse depth when numbered in the last window, else its stored one).  Stable
         (IsLandMarkStable): used_num >= 2, start < window_size - 2, not start > window_size * 3 / 4, not depth <= 0 (NaN
-        passes).  Margin cloud: stable, start == 0, used_num <= 2 and numbered in the last window (solve_flag ==
-        SovelSucc).  Returns (xyz [n, 3] world points R_c (x, y, 1) depth + t_c, feature ids [n], in_margin_cloud [n]) of
-        the stable entries in table order."""
+        passes).  Margin cloud: stable, start == 0, used_num <= 2 and solve_flag == SovelSucc (numbered in the last
+        window, or solved before a re-anchoring slide).  Returns (xyz [n, 3] world points R_c (x, y, 1) depth + t_c,
+        feature ids [n], in_margin_cloud [n]) of the stable entries in table order."""
         assert set(slots) == self.held and len(set(slots)) == len(slots)
         slots = np.asarray(slots)
         position = np.full(self.N_SLOTS, -1, np.int64)
@@ -536,7 +590,7 @@ class FeatureTable:
         with np.errstate(divide="ignore"):
             depth = 1.0 / r
         stable = (used >= 2) & (start < window_size - 2) & ~(start > window_size * 3.0 / 4.0) & ~(depth <= 0)
-        margin = stable & (start == 0) & (used <= 2) & numbered
+        margin = stable & (start == 0) & (used <= 2) & (numbered | self.solved)
         e = np.nonzero(stable)[0]
         xy = np.array([self.bearing[a][self.idx[k, a]] for k, a in zip(e, self.anchor[e])]).reshape(-1, 2)
         d = depth[e]
@@ -592,17 +646,28 @@ class ResidentRunner(StreamingRunner):
     publish_map=True (requires device_features=True): right after FeatureTableSlide, inside the timed region, the
     landmark map and keyframe poses the reference publishes after every image (GetLandmarksInWindow, GetMarginCloud,
     PublishVioKeyFrame) come from the device (FeatureTableMap over the post-slide window).  The arrays (xyz, ids,
-    in_margin, cam_q, cam_p) are kept on last_map, and the record gains n_map_points and n_margin_points."""
+    in_margin, cam_q, cam_p) are kept on last_map, and the record gains n_map_points and n_margin_points.
 
-    def __init__(self, lib, seq, triangulate=False, device_features=False, publish_map=False, **kw):
+    reanchor=True (requires device_features=True): the table slides as the reference's feature list does
+    (FeatureTableSlideReanchor: removeBackShiftDepth / removeFront), after GaugeRealign and the marginalization and
+    before SlideWindow / SlideWindowSecondNew, while the leaving frame's time is still inside the spline.  The landmarks
+    anchored in the leaving frame are re-anchored instead of dropped; the record gains n_reanchored.  On C5 the solve
+    diverges in window 8: as in the reference, every MARGIN_OLD marginalizes all factors of the landmarks anchored in the
+    oldest frame, so a re-anchored landmark's observations enter the prior again at every slide (DESIGN §6).
+    Default (False): FeatureTableSlide after the window's slide, as before."""
+
+    def __init__(self, lib, seq, triangulate=False, device_features=False, publish_map=False, reanchor=False, **kw):
         if device_features and not triangulate:
             raise ValueError("device_features requires triangulate=True: new landmarks enter with inverse depth -1")
         if publish_map and not device_features:
             raise ValueError("publish_map requires device_features=True: the map is read from the resident feature table")
+        if reanchor and not device_features:
+            raise ValueError("reanchor requires device_features=True: landmarks are re-anchored in the resident feature table")
         super().__init__(lib, seq, **kw)
         self.triangulate = triangulate
         self.device_features = device_features
         self.publish_map = publish_map
+        self.reanchor = reanchor
         self.last_map = None
         self.triangulate_probe = None
         if self.clouds is None:
@@ -778,14 +843,16 @@ class ResidentRunner(StreamingRunner):
             self.prior_dim = n_out.value
         t_marged = time.perf_counter()
         qs, ps = e.GetKnots(); ld = e.GetLineDelay()   # the trajectory is the product the caller publishes
+        n_removed = n_reanchored = None
+        if self.reanchor:                              # removeFailures + removeBackShiftDepth / removeFront
+            n_removed, n_reanchored = e.FeatureTableSlideReanchor(frame_slots, marg)
         if marg:
             drop_knots = later
             e.SlideWindow(drop_knots, 1, 1)            # slideWindowOld: oldest frame's control points and bias node leave
         else:
             drop_knots = 0
             e.SlideWindowSecondNew()                   # slideWindowNew: the second-newest frame leaves, the prior stays
-        n_removed = None
-        if self.device_features:                       # the leaving frame's landmarks and observations leave the table
+        if self.device_features and not self.reanchor:  # the leaving frame's landmarks and observations leave the table
             n_removed = e.FeatureTableSlide(self.slot_of[self.frames[0 if marg else -2]])
         if self.publish_map:                           # the landmark map and keyframe poses of the post-slide window
             self.last_map = e.FeatureTableMap(np.delete(frame_slots, 0 if marg else len(frame_slots) - 2), WINDOW_SIZE)
@@ -813,6 +880,8 @@ class ResidentRunner(StreamingRunner):
         if self.device_features:
             # n_new_lm: the window's landmarks without a depth yet (-1), which are exactly the ones TriangulateWindow wrote
             rec.update(n_triangulated=n_tri, n_fallback=n_fb, n_new_lm=n_tri + n_fb, n_removed=n_removed)
+            if self.reanchor:
+                rec.update(n_reanchored=n_reanchored)
             if self.publish_map:
                 rec.update(n_map_points=len(self.last_map[1]), n_margin_points=int(self.last_map[2].sum()))
         elif self.triangulate:
