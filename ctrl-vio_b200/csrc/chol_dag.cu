@@ -454,9 +454,8 @@ __global__ void __launch_bounds__(256, 1) chol_dag_kernel(CholDagArgs a) {
   double* xf_pub = a.part + 2 * nn;     // [j][64] forward-solved x_j
   double* xb_pub = xf_pub + size_t(nb) * kCholNB;  // [j][64] solution x_j
   const double sv = sentinel_value();
-  // speculated step behind a rejected / terminating one: nothing has been sent or reset yet, and the host takes the
-  // launch out of its parity count (engine.cu)
-  if (a.go && *a.go == 0) return;
+  // (go is written two launches back: read before the wait)
+  const bool go = !a.go || *a.go != 0;
 
   // chain order: position p = blockIdx.x: p even < 2 nb - 1: diagonal CTA p / 2; p odd: sub-diagonal tile
   // ((p + 1) / 2, (p - 1) / 2); then the other tiles (i >= j + 2) column by column; then fillers (grid padded to the
@@ -476,7 +475,15 @@ __global__ void __launch_bounds__(256, 1) chol_dag_kernel(CholDagArgs a) {
     }
     __syncthreads();
     cluster_arrive();
-    if (pos >= nb * (nb + 1) / 2) { cluster_wait(); return; }  // filler CTA
+  }
+  // everything above touches this CTA's shared memory only; M and rhs come from schur_tile_kernel
+  pdl_wait();
+  pdl_launch_dependents();
+  // speculated step behind a rejected / terminating one: nothing has been sent or reset yet, and the host takes the
+  // launch out of its parity count (engine.cu)
+  if (!go || (dsm && pos >= nb * (nb + 1) / 2)) {  // (or a filler CTA)
+    if (dsm) cluster_wait();
+    return;
   }
   if (!is_diag) {
     // ======================= tile (i, j), i > j =======================
@@ -795,14 +802,21 @@ int launch_chol_dag(const LinearLaunch& l, cudaStream_t s) {
     cfg.blockDim = dim3(256);
     cfg.dynamicSmemBytes = kCholDagSmem;
     cfg.stream = s;
-    cudaLaunchAttribute at[2];
+    cudaLaunchAttribute at[3];
     at[0].id = cudaLaunchAttributeClusterDimension;
     at[0].val.clusterDim.x = kDagCluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     at[1].id = cudaLaunchAttributeCooperative;
     at[1].val.cooperative = 1;
+    at[2].id = cudaLaunchAttributeProgrammaticStreamSerialization;  // pipelined driver (launch_chained, kernels.h)
+    at[2].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at;
-    cfg.numAttrs = 2;
-    const cudaError_t cerr = cudaLaunchKernelEx(&cfg, chol_dag_kernel, a);
+    cfg.numAttrs = l.pdl ? 3 : 2;
+    cudaError_t cerr = cudaLaunchKernelEx(&cfg, chol_dag_kernel, a);
+    if (cerr != cudaSuccess && l.pdl) {  // the three attributes refused together: the plain cluster launch
+      cudaGetLastError();
+      cfg.numAttrs = 2;
+      cerr = cudaLaunchKernelEx(&cfg, chol_dag_kernel, a);
+    }
     if (cerr == cudaSuccess) {
       cluster_state.store(1, std::memory_order_relaxed);
       g_dag_cluster_launches.fetch_add(1, std::memory_order_relaxed);

@@ -581,10 +581,12 @@ int shard_check_ownership(ctvio_engine* e) {
 }
 
 // the LM step: reduced system (+ all-reduce of [M | rhs | diagA] over NVLink in sharded mode), factor, solve
+// pdl: the kernels are chained by programmatic dependent launch (pipelined driver only, see launch_chained)
 int lm_step(ctvio_engine* e, int nb, double radius, const ApplyLaunch* fused_apply = nullptr, const double* radius_dev = nullptr,
-            const int32_t* go = nullptr) {
+            const int32_t* go = nullptr, bool pdl = false) {
   LinearLaunch lin = linear_launch(e, nb);
   lin.go = go;
+  lin.pdl = pdl ? 1 : 0;
   cudaStream_t st = e->stream;
   if (e->deterministic) cudaMemsetAsync(e->d_ticket.p, 0, 2 * sizeof(int32_t), st);
   e->launches += launch_reduced_system(lin, radius, st, radius_dev);
@@ -1100,7 +1102,6 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
     bool spec_in_flight = false; // speculated kernels that read ne_slab[cur_ne ^ 1] may still be running
     int spec_out = -1;
     unsigned spec_chol_seq0 = e->chol_seq;
-    cudaEventRecord(e->ev_iter, st);
     while (true) {
       if (iter >= max_iterations) { term = CTVIO_TERM_NO_CONVERGENCE; break; }
       if (last_ok && gmax <= gradient_tolerance) { term = CTVIO_TERM_GRADIENT; break; }
@@ -1118,7 +1119,7 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
         while (cand == cur) ++cand;
         if (!spec_in_flight) prezero_slab(e, cand_ne);  // else: cleared in stream order by evaluate()
         const ApplyLaunch full_step = make_apply(cur, cand, 1.0);
-        rc = lm_step(e, cur_ne, radius, &full_step);
+        rc = lm_step(e, cur_ne, radius, &full_step, nullptr, nullptr, true);
         if (rc) return rc;
       }
       sum.num_linear_solves++;
@@ -1126,9 +1127,12 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
       sum.num_jacobian_evals++;
       const LmDecideArgs da{e->d_dec.p, x_cost, radius, min_relative_decrease, max_radius,
                             parameter_tolerance, function_tolerance, gradient_tolerance, min_radius};
-      e->launches += launch_gradient_norm(linear_launch(e, cand_ne), e->state(cand).ptrs(), e->opt.fix_ld, e->opt.ld_lower,
-                                          e->opt.ld_upper, st, false, e->h_pub, ++e->pub_seq, &da);
-      cudaEventRecord(e->ev_iter, st);
+      LinearLaunch lin_cand = linear_launch(e, cand_ne);
+      lin_cand.pdl = 1;
+      e->launches += launch_gradient_norm(lin_cand, e->state(cand).ptrs(), e->opt.fix_ld, e->opt.ld_lower, e->opt.ld_upper, st,
+                                          false, e->h_pub, ++e->pub_seq, &da);
+      // (no event between this kernel and the speculated scale_copy_kernel: a stream operation there would cost the
+      // two kernels their programmatic dependent launch; ev_iter is recorded after the loop, DESIGN §6)
       // ---- speculate: step iter + 1 from (cand, cand_ne), radius from the device-side decision ----
       spec_ready = false;
       if (iter < max_iterations) {
@@ -1136,7 +1140,7 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
         while (spec_out == cur || spec_out == cand) ++spec_out;
         const ApplyLaunch spec_step = make_apply(cand, spec_out, 1.0);
         spec_chol_seq0 = e->chol_seq;
-        rc = lm_step(e, cand_ne, 0.0, &spec_step, &e->d_dec.p->radius_next, &e->d_dec.p->go);
+        rc = lm_step(e, cand_ne, 0.0, &spec_step, &e->d_dec.p->radius_next, &e->d_dec.p->go, true);
         if (rc) return rc;
         spec_ready = true;
         spec_in_flight = true;
@@ -1194,8 +1198,11 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
     e->cur = cur;
     e->table_valid = true;
     e->slab_zeroed[0] = e->slab_zeroed[1] = false;  // (a pending clear is ordered by ev_zero only inside this loop)
-    // results: wait for the last REAL kernel only (ev_iter); speculated leftovers keep running behind it and are
-    // ordered before anything the next call enqueues on the engine stream
+    // results: the solve ends with its last gradient_norm_kernel, or, when it stopped on a tolerance or a failed step,
+    // with the speculated step enqueued behind that kernel, which the device has cancelled (LmDecision::go = 0: its
+    // kernels return at once).  ev_iter is recorded here and not after each gradient_norm_kernel (see above), so
+    // summary.device_ms includes such a cancelled tail.
+    cudaEventRecord(e->ev_iter, st);
     CUDA_OK(cudaStreamWaitEvent(e->stream2, e->ev_iter, 0));
     {
       const int rcm = refresh_mirror(e, e->stream2);

@@ -5,6 +5,7 @@
 #include <atomic>
 
 #include <cstdint>
+#include <utility>
 
 #include "spline_eval.cuh"
 
@@ -194,6 +195,36 @@ __device__ __forceinline__ void det_ticket_done(int* ticket, int my) {
   __syncthreads();
   if (threadIdx.x == 0) asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(ticket), "r"(my + 1) : "memory");
 }
+// programmatic dependent launch (see launch_chained): both are no-ops in a kernel that was launched without it
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+#endif
+
+// ---- programmatic dependent launch (PDL) on the pipelined LM driver's main stream ---------------
+// pdl = true: the kernel may be launched while the kernel before it on the stream is still running, and runs the part of
+// it in front of pdl_wait() early; pdl_wait() returns when that kernel has completed and its writes are visible.
+// The rule every kernel launched this way follows:
+//   nothing before pdl_wait() reads a buffer the immediately preceding kernel writes, and nothing before it writes a
+//   buffer that kernel reads; pdl_launch_dependents() comes no earlier than right after the kernel's own pdl_wait(),
+//   and every thread passes pdl_wait() before it exits.
+// So a kernel's successor is let in only after everything two launches back has completed: data written two or more
+// kernels back may be read before the wait.  The deterministic, sharded and line-search paths launch plainly.
+#if defined(__CUDACC__)
+template <typename... KArgs, typename... Args>
+cudaError_t launch_chained(bool pdl, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
+                           Args&&... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = s;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = pdl ? 1 : 0;
+  return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
 #endif
 
 // ---- launch wrappers (each returns the number of kernels it launched) ----------------------------
@@ -282,6 +313,7 @@ struct LinearLaunch {
   LmScalars* scal;
   int* det_ticket;              // deterministic mode (K4 parts, step kernels): flush in block order; else null
   const int32_t* go;            // speculated step only: &LmDecision::go - the expensive kernels return at once when it is 0
+  int32_t pdl = 0;              // pipelined driver: the step's kernels are chained by launch_chained(pdl = true)
 };
 int launch_jacobi_scale(const LinearLaunch& a, cudaStream_t s);
 // builds the damped, scaled reduced system, factors it, solves and back-substitutes: dc, dl, gd, dHd

@@ -51,6 +51,10 @@ int launch_jacobi_scale(const LinearLaunch& a, cudaStream_t s) {
 
 // M = S A S + clamp(diag)/radius on the full (padded, symmetric) matrix; rhs = S g
 __global__ void scale_copy_kernel(LinearLaunch a, double radius, const double* __restrict__ radius_dev) {
+  // (nothing worth starting early: every output depends on the radius gradient_norm_kernel decides, and on the
+  // accumulators it reads before this kernel may reset them)
+  pdl_wait();
+  pdl_launch_dependents();
   if (radius_dev) radius = *radius_dev;  // speculated step: decided by the previous step's gradient_norm_kernel
   const int npad = a.npad, np = a.dims.np;
   const size_t idx = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -148,8 +152,10 @@ __global__ void __launch_bounds__(256, 2) schur_tile_kernel(LinearLaunch a) {
     scB[tid] = (gb < np && !a.cmask[gb]) ? a.sc[gb] : 0.0;
   }
   const double sc_ld = a.cmask[ild] ? 0.0 : a.sc[ild];
-  const int go = a.go ? *a.go : 1;  // (issued together with the loads above)
+  const int go = a.go ? *a.go : 1;  // (issued together with the loads above; written two launches back)
   __syncthreads();
+  pdl_wait();  // lis, lc and M come from scale_copy_kernel
+  pdl_launch_dependents();
   if (!go) return;  // speculated step behind a rejected / terminating one
   Frag acc;
   frag_zero(acc);
@@ -339,10 +345,10 @@ int launch_jacobi_scale_from_diag(const LinearLaunch& a, cudaStream_t s) {
 int launch_reduced_system(const LinearLaunch& a, double radius, cudaStream_t s, const double* radius_dev) {
   int launches = 0;
   const size_t total = std::max(size_t(a.npad) * a.npad, size_t(a.dims.nL));
-  scale_copy_kernel<<<unsigned((total + 255) / 256), 256, 0, s>>>(a, radius, radius_dev);
+  launch_chained(a.pdl, scale_copy_kernel, dim3(unsigned((total + 255) / 256)), dim3(256), 0, s, a, radius, radius_dev);
   ++launches;
   if (a.n_schur_items > 0) {
-    schur_tile_kernel<<<a.n_schur_items, 256, 0, s>>>(a);
+    launch_chained(a.pdl, schur_tile_kernel, dim3(a.n_schur_items), dim3(256), 0, s, a);
     ++launches;
   }
   return launches;
@@ -365,6 +371,8 @@ __global__ void __launch_bounds__(1024) gradient_norm_kernel(LinearLaunch a, Sta
                                                              double ld_upper, LmPublished* pub, unsigned long long seq,
                                                              LmDecideArgs da) {
   __shared__ double red[32];
+  pdl_wait();
+  pdl_launch_dependents();
   const int np = a.dims.np, nL = a.dims.nL;
   double v = 0.0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < np + nL; i += gridDim.x * blockDim.x) {
@@ -452,7 +460,7 @@ int launch_gradient_norm(const LinearLaunch& a, const StatePtrs& st, int fix_ld,
   if (decide) da = *decide;
   const int n = a.dims.np + a.dims.nL;
   const int grid = std::min(16, std::max(1, (n + 1023) / 1024));
-  gradient_norm_kernel<<<grid, 1024, 0, s>>>(a, st, fix_ld, ld_lower, ld_upper, pub, seq, da);
+  launch_chained(a.pdl, gradient_norm_kernel, dim3(grid), dim3(1024), 0, s, a, st, fix_ld, ld_lower, ld_upper, pub, seq, da);
   return 1;
 }
 
@@ -557,6 +565,8 @@ int launch_apply_step(const ApplyLaunch& a, cudaStream_t s, bool reset) {
 __global__ void __launch_bounds__(256) step_apply_kernel(LinearLaunch a, ApplyLaunch ap, int ncb, int nlb) {
   extern __shared__ double step_dsh[];  // [np]
   const int b = blockIdx.x;
+  pdl_wait();
+  pdl_launch_dependents();
   if (b < ncb) camera_step_block(a, b, step_dsh);
   else if (b < ncb + nlb) landmark_step_block(a, b - ncb, &ap);
   else apply_step_block(ap, StepSource{nullptr, a.y, a.sc, a.cmask}, b - ncb - nlb, false);
@@ -565,7 +575,8 @@ __global__ void __launch_bounds__(256) step_apply_kernel(LinearLaunch a, ApplyLa
 int launch_step_and_apply(const LinearLaunch& a, const ApplyLaunch& ap, cudaStream_t s) {
   const int ncb = (a.dims.np + 7) / 8, nlb = (a.dims.nL + 7) / 8;
   const int nab = (a.dims.nK + 6 * a.dims.nB + 1 + 255) / 256;
-  step_apply_kernel<<<ncb + nlb + nab, 256, size_t(a.dims.np) * sizeof(double), s>>>(a, ap, ncb, nlb);
+  launch_chained(a.pdl, step_apply_kernel, dim3(ncb + nlb + nab), dim3(256), size_t(a.dims.np) * sizeof(double), s, a, ap,
+                 ncb, nlb);
   return 1;
 }
 
