@@ -151,23 +151,36 @@ int prepare(ctvio_engine* e) {
       hpj[k] = make_double2(o.pj[0], o.pj[1]);
       hm[k] = make_int4(o.rowi, o.rowj, o.lm, o.marg);
     }
-    // work items: chunks of one group; chunk size adapts so that small problems still spread over the SMs
-    // one evaluation round (<= 128 observations, a lane pair each) per CTA: the round is latency bound whatever its
-    // fill, so a group is cut into EQUAL chunks of at most one round (263 observations -> 3 x 88, not 128 + 128 + 7)
-    // and every chunk gets its own CTA
-    constexpr int cap = kVisObsPerRound;
-    std::vector<VisualItem>& items = e->h_items;
-    items.clear();
+    // work items: chunks of one group, one evaluation round (<= 128 observations, a lane pair each) per CTA.  The
+    // round is latency bound whatever its fill, so a group is cut into EQUAL chunks (263 observations -> 3 x 88, not
+    // 128 + 128 + 7) and every chunk gets its own CTA.  A window with fewer chunks than SMs has its groups cut finer
+    // (the cap halved down to kVisMinChunk) as long as all chunks still run at once: each CTA then has fewer rows to
+    // evaluate and to reduce in its SYRK, on SMs that would otherwise idle.  A window that fills the SMs keeps full
+    // rounds (finer chunks would only add flushes).
+    std::vector<int2> groups;  // [first, end) in sorted order
     for (int k = 0; k < n;) {
       const int a = e->img_order[k];
       int end = k;
       while (end < n && wi0[e->img_order[end]] == wi0[a] && wj0[e->img_order[end]] == wj0[a]) ++end;
-      const int cnt = end - k;
-      // a few stragglers beyond a full round are cheaper as their own small item than as an extra round
+      groups.push_back(make_int2(k, end));
+      k = end;
+    }
+    auto n_chunks = [&](int c) {
+      size_t m = 0;
+      for (const int2& g : groups) m += (g.y - g.x + c - 1) / c;
+      return m;
+    };
+    int cap = kVisObsPerRound;
+    const size_t n_sm = size_t(device_sm_count());
+    while (cap / 2 >= kVisMinChunk && n_chunks(cap / 2) <= n_sm) cap /= 2;
+    std::vector<VisualItem>& items = e->h_items;
+    items.clear();
+    for (const int2& g : groups) {
+      const int a = e->img_order[g.x];
+      const int cnt = g.y - g.x;
       const int nchunks = (cnt + cap - 1) / cap;
       const int per = (cnt + nchunks - 1) / nchunks;
-      for (int s = k; s < end; s += per) items.push_back(VisualItem{s, std::min(per, end - s), wi0[a], wj0[a]});
-      k = end;
+      for (int s = g.x; s < g.y; s += per) items.push_back(VisualItem{s, std::min(per, g.y - s), wi0[a], wj0[a]});
     }
     e->n_items = int(items.size());
     if (!e->img_desc.empty()) {

@@ -14,6 +14,8 @@ namespace ctvio {
 constexpr int kPStride = 4;        // knot positions are stored [N][4] (32 B) so that TMA windows are 16-B aligned
 constexpr int kVisThreads = 256;   // visual kernel CTA: 128 lane pairs
 constexpr int kVisObsPerRound = 128;
+constexpr int kVisMinChunk = 64;  // smallest chunk a frame-pair group is cut into to fill the SMs (engine.cu); 32 tips the
+                                  // ill-conditioned window 8 of the re-anchoring runner into divergence (DESIGN §6)
 constexpr int kLocalDim = 64;      // padded local Jacobian width of one frame-pair group
 constexpr int kRowStride = 66;     // shared-memory stride of one Jacobian row (doubles); 16-B aligned
 constexpr int kObsStride = 2 * kRowStride + 2;  // stride of one observation's 2 rows: 268 words -> 2-way store conflicts instead of 16-way

@@ -17,7 +17,7 @@
 //   * a LANE PAIR evaluates one observation: even lane = anchor pose, odd lane = observation pose
 //     (eval_side), 18 doubles exchanged by warp shuffles, each lane then chain-rules its own 4 knots;
 //   * Jacobian rows never go to HBM: they are written to a shared-memory tile (128 obs x 2 rows x 64)
-//     and reduced by a register-tiled SYRK (8x8 tiles, 7 row groups) into a shared accumulator that
+//     and reduced by a SYRK on the fp64 tensor cores (syrk_round) into a shared accumulator that
 //     is flushed once per CTA with fp64 atomics into the upper-triangular camera block A and g;
 //   * landmark Schur pieces (h_l, g_l, W_l) are reduced with fp64 RED atomics into the compact
 //     per-landmark rows.
@@ -118,12 +118,18 @@ __constant__ uint8_t c_tile_j[36] = {0, 1, 2, 3, 4, 5, 6, 7, 1, 2, 3, 4, 5, 6, 7
 
 #ifdef CTVIO_CHOL_TIMING
 __device__ long long g_vis_clk[8];
+__device__ long long g_imu_clk[8];
 #define VCLK(i) do { if (blockIdx.x == 0 && threadIdx.x == 0) g_vis_clk[(i)] = clock64(); } while (0)
+#define ICLK(i) do { if (blockIdx.x == 0 && threadIdx.x == 0) g_imu_clk[(i)] = clock64(); } while (0)
 extern "C" int ctvio_debug_vis_clk(long long* out) {
   return cudaMemcpyFromSymbol(out, g_vis_clk, sizeof(g_vis_clk)) == cudaSuccess ? 0 : -1;
 }
+extern "C" int ctvio_debug_imu_clk(long long* out) {
+  return cudaMemcpyFromSymbol(out, g_imu_clk, sizeof(g_imu_clk)) == cudaSuccess ? 0 : -1;
+}
 #else
 #define VCLK(i)
+#define ICLK(i)
 #endif
 
 size_t visual_smem_bytes() {
@@ -135,29 +141,29 @@ size_t visual_smem_bytes() {
 // (warps 0..5: the six off-diagonal blocks, warps 6, 7: two diagonal blocks each), so that every tile has ONE owner
 // warp over all rows: no cross-warp merge, the partial sums of earlier rounds are simply reloaded from accs.
 // Rows of inactive observation slots are zero (written by the evaluation phase), so K runs in whole 4-row steps.
-__device__ __noinline__ void syrk_round(const double* Jt, double* accs, int nround, int tid) {
-  const int warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
-  const int nblk = warp < 6 ? 1 : 2;
-  int bi[2], bj[2];
-  if (warp < 6) {
-    bi[0] = warp < 3 ? 0 : (warp < 5 ? 1 : 2);
-    bj[0] = warp < 3 ? warp + 1 : (warp < 5 ? warp - 1 : 3);
-    bi[1] = bj[1] = 0;
-  } else {
+// The two kinds of warp are two instantiations (every DMMA unconditional, see DESIGN §4 on WARPSYNC).
+template <bool DIAG>
+__device__ __noinline__ void syrk_round_warp(const double* Jt, double* accs, int nround, int warp, int lane) {
+  constexpr int NB = DIAG ? 2 : 1;
+  const int g = lane >> 2, q = lane & 3;
+  int bi[NB], bj[NB];
+  if constexpr (DIAG) {
     bi[0] = bj[0] = 2 * (warp - 6);
     bi[1] = bj[1] = 2 * (warp - 6) + 1;
+  } else {
+    bi[0] = warp < 3 ? 0 : (warp < 5 ? 1 : 2);
+    bj[0] = warp < 3 ? warp + 1 : (warp < 5 ? warp - 1 : 3);
   }
-  const bool dg = warp >= 6;
-  double acc[2][2][2][2];
+  double acc[NB][2][2][2];
 #pragma unroll
-  for (int b = 0; b < 2; ++b)
+  for (int b = 0; b < NB; ++b)
 #pragma unroll
     for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
       for (int nj = 0; nj < 2; ++nj) {
+        if (DIAG && mi == 1 && nj == 0) continue;  // strictly lower tile of a diagonal block
         const int ti = 2 * bi[b] + mi, tj = 2 * bj[b] + nj;
-        double2 v = make_double2(0.0, 0.0);
-        if (b < nblk && ti <= tj) v = *reinterpret_cast<const double2*>(accs + (ti * 8 - ti * (ti - 1) / 2 + (tj - ti)) * 64 + g * 8 + 2 * q);
+        const double2 v = *reinterpret_cast<const double2*>(accs + (ti * 8 - ti * (ti - 1) / 2 + (tj - ti)) * 64 + g * 8 + 2 * q);
         acc[b][mi][nj][0] = v.x; acc[b][mi][nj][1] = v.y;
       }
   const int nsteps = (2 * nround + 3) >> 2;
@@ -166,37 +172,41 @@ __device__ __noinline__ void syrk_round(const double* Jt, double* accs, int nrou
     const int row = 4 * st + q;
     const double* rp = Jt + size_t(row >> 1) * kObsStride + (row & 1) * kRowStride + g;
 #pragma unroll
-    for (int b = 0; b < 2; ++b) {
-      if (b < nblk) {
-        double av[2], bv[2];
+    for (int b = 0; b < NB; ++b) {
+      double av[2], bv[2];
 #pragma unroll
-        for (int m = 0; m < 2; ++m) {
-          av[m] = rp[16 * bi[b] + 8 * m];
-          bv[m] = dg ? av[m] : rp[16 * bj[b] + 8 * m];
-        }
-#pragma unroll
-        for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-          for (int nj = 0; nj < 2; ++nj) {
-            if (dg && mi == 1 && nj == 0) continue;  // strictly lower tile of a diagonal block
-            asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                         : "+d"(acc[b][mi][nj][0]), "+d"(acc[b][mi][nj][1])
-                         : "d"(av[mi]), "d"(bv[nj]));
-          }
+      for (int m = 0; m < 2; ++m) {
+        av[m] = rp[16 * bi[b] + 8 * m];
+        bv[m] = DIAG ? av[m] : rp[16 * bj[b] + 8 * m];
       }
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int nj = 0; nj < 2; ++nj) {
+          if (DIAG && mi == 1 && nj == 0) continue;
+          asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+                       : "+d"(acc[b][mi][nj][0]), "+d"(acc[b][mi][nj][1])
+                       : "d"(av[mi]), "d"(bv[nj]));
+        }
     }
   }
 #pragma unroll
-  for (int b = 0; b < 2; ++b)
+  for (int b = 0; b < NB; ++b)
 #pragma unroll
     for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
       for (int nj = 0; nj < 2; ++nj) {
+        if (DIAG && mi == 1 && nj == 0) continue;
         const int ti = 2 * bi[b] + mi, tj = 2 * bj[b] + nj;
-        if (b < nblk && ti <= tj)
-          *reinterpret_cast<double2*>(accs + (ti * 8 - ti * (ti - 1) / 2 + (tj - ti)) * 64 + g * 8 + 2 * q) =
-              make_double2(acc[b][mi][nj][0], acc[b][mi][nj][1]);
+        *reinterpret_cast<double2*>(accs + (ti * 8 - ti * (ti - 1) / 2 + (tj - ti)) * 64 + g * 8 + 2 * q) =
+            make_double2(acc[b][mi][nj][0], acc[b][mi][nj][1]);
       }
+}
+
+__device__ __forceinline__ void syrk_round(const double* Jt, double* accs, int nround, int tid) {
+  const int warp = tid >> 5, lane = tid & 31;
+  if (warp < 6) syrk_round_warp<false>(Jt, accs, nround, warp, lane);
+  else syrk_round_warp<true>(Jt, accs, nround, warp, lane);
   __syncthreads();
 }
 
@@ -486,10 +496,12 @@ int launch_visual(const VisualLaunch& l, bool full, cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// K2: IMU factors.  One CTA per (start knot, bias node) run of samples (<= 32): lanes of warp 0 evaluate
-// one sample each, the 6 x 31 Jacobian rows (24 knot dims | 6 bias dims | residual) go to shared memory and
-// all 64 threads reduce J'J with the same 8x8 register-tiled SYRK as K1 (10 upper tiles x 6 row groups),
-// flushing one fp64 atomic per non-zero entry per CTA.
+// K2: IMU factors.  One CTA of four warps per (start knot, bias node) run of samples (<= 32).  Lane l of every warp
+// evaluates sample l up to its residual (imu_stage), then warp w writes a quarter of the sample's 6 x 31 Jacobian rows
+// (24 knot dims | 6 bias dims | residual): the gyro (w = 0, 1) or accel (w = 2, 3) rows of the knots 2 (w & 1) and
+// 2 (w & 1) + 1, warps 1 and 3 also the bias columns and the residual.  The rows go column-major to shared memory and
+// J'J is formed on the fp64 tensor cores (m8n8k4, K = Jacobian rows): each of the 10 upper 8x8 tiles of the 32 local
+// dims has one owner warp over all rows and is flushed from its fragments, one fp64 atomic per non-zero entry per CTA.
 
 struct ImuArgs {
   ImuObsPtrs obs;
@@ -504,24 +516,116 @@ struct ImuArgs {
   int* det_ticket;
 };
 
-constexpr int kImuThreads = 64;
-constexpr int kImuCols = 32;      // 24 knot dims + 6 bias dims + residual + pad
-constexpr int kImuRowStride = 34; // doubles; 16-B aligned rows, fewer store conflicts
-__constant__ uint8_t c_imu_tile_i[10] = {0, 0, 0, 0, 1, 1, 1, 2, 2, 3};
-__constant__ uint8_t c_imu_tile_j[10] = {0, 1, 2, 3, 1, 2, 3, 2, 3, 3};
+constexpr int kImuThreads = 128;
+constexpr int kImuCols = 32;          // 24 knot dims + 6 bias dims + residual + zero pad
+constexpr int kImuColStride = 196;    // doubles per column: 6 x 32 rows + 4; = 4 mod 16, so the fragment loads of a
+                                      // half-warp (4 columns x 4 rows) hit 16 different banks
+static_assert(kImuColStride >= 6 * kImuMaxPerItem && kImuColStride % 16 == 4, "K2 shared column stride");
+
+// Tile t of warp w as 4 ti + tj, chosen so that a warp loads 2 or 3 of the 4 column tiles per 4-row step:
+// warp 0 (0,0) (0,1) (1,1), warp 1 (2,2) (2,3) (3,3), warp 2 (0,2) (0,3), warp 3 (1,2) (1,3)
+__host__ __device__ constexpr int imu_tile(int w, int t) {
+  return w == 0 ? (t == 0 ? 0 : t == 1 ? 1 : 5)
+       : w == 1 ? (t == 0 ? 10 : t == 1 ? 11 : 15)
+       : w == 2 ? (t == 0 ? 2 : 3)
+                : (t == 0 ? 6 : 7);
+}
+__host__ __device__ constexpr int imu_ntiles(int w) { return w < 2 ? 3 : 2; }
+__host__ __device__ constexpr bool imu_uses(int w, int c) {
+  bool u = false;
+  for (int t = 0; t < imu_ntiles(w); ++t) u = u || imu_tile(w, t) >> 2 == c || (imu_tile(w, t) & 3) == c;
+  return u;
+}
+
+// Zero this warp's part of one sample's rows (an invalid sample, or the sample after the last one when the row count is
+// not a multiple of the 4-row step)
+__device__ __forceinline__ void imu_zero_part(double* J, int warp) {
+  const int r0 = 3 * (warp >> 1), c0 = 12 * (warp & 1), c1 = (warp & 1) ? kImuCols : 12;
+  for (int c = c0; c < c1; ++c)
+#pragma unroll
+    for (int r = 0; r < 3; ++r) J[c * kImuColStride + r0 + r] = 0.0;
+}
+
+template <bool ACCEL, int H>
+__device__ __forceinline__ void imu_write_part(const ImuArgs& a, const ImuStage& st, int s, int node, double* J) {
+  constexpr int r0 = ACCEL ? 3 : 0;
+  imu_jacobian_half<ACCEL, H>(a.rig, a.st.tab, s, st, [&](int k, const double rot[9], const double pos[9]) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const bool mr = a.cmask[6 * (s + k) + c] != 0, mp = a.cmask[6 * (s + k) + 3 + c] != 0;
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+        J[(k * 6 + c) * kImuColStride + r0 + r] = mr ? 0.0 : rot[3 * r + c];
+        J[(k * 6 + 3 + c) * kImuColStride + r0 + r] = mp ? 0.0 : pos[3 * r + c];
+      }
+    }
+  });
+  if (H == 1) {
+    const int gb0 = a.dims.idx_bias0 + 6 * node;
+#pragma unroll
+    for (int c = 0; c < 6; ++c) {
+      const bool mb = a.cmask[gb0 + c] != 0;
+#pragma unroll
+      for (int r = 0; r < 3; ++r) J[(24 + c) * kImuColStride + r0 + r] = (c == r0 + r && !mb) ? a.rig.imu_info[r0 + r] : 0.0;
+    }
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      J[30 * kImuColStride + r0 + r] = st.r[r0 + r];
+      J[31 * kImuColStride + r0 + r] = 0.0;
+    }
+  }
+}
+
+// This warp's J'J tiles over all rows: lane (g, q) of a step reads rows 4 st + q of the local columns 8 t + g
+template <int W>
+__device__ __forceinline__ void imu_syrk(const double* Js, int nsteps, int lane, double acc[3][2]) {
+  const double* rp = Js + (lane >> 2) * kImuColStride + (lane & 3);
+#pragma unroll
+  for (int t = 0; t < 3; ++t) acc[t][0] = acc[t][1] = 0.0;
+#pragma unroll 4
+  for (int st = 0; st < nsteps; ++st, rp += 4) {
+    double v[4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) v[c] = imu_uses(W, c) ? rp[8 * c * kImuColStride] : 0.0;
+#pragma unroll
+    for (int t = 0; t < imu_ntiles(W); ++t)
+      asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+                   : "+d"(acc[t][0]), "+d"(acc[t][1])
+                   : "d"(v[imu_tile(W, t) >> 2]), "d"(v[imu_tile(W, t) & 3]));
+  }
+}
+
+// Flush of this warp's tiles: lane (g, q) holds the entries (8 ti + g, 8 tj + 2 q + {0, 1})
+template <int W>
+__device__ __forceinline__ void imu_flush(const ImuArgs& a, const ImuItem& item, int lane, const double acc[3][2]) {
+  const int np = a.dims.np;
+#pragma unroll
+  for (int t = 0; t < imu_ntiles(W); ++t)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const double val = acc[t][e];
+      const int la = 8 * (imu_tile(W, t) >> 2) + (lane >> 2), lb = 8 * (imu_tile(W, t) & 3) + 2 * (lane & 3) + e;
+      if (val == 0.0 || la > lb || lb > 30 || la >= 30) continue;
+      const int ga = la < 24 ? 6 * item.s + la : a.dims.idx_bias0 + 6 * item.node + (la - 24);
+      if (lb == 30) {
+        atomicAdd(a.ne.gc + ga, val);
+        continue;
+      }
+      const int gb = lb < 24 ? 6 * item.s + lb : a.dims.idx_bias0 + 6 * item.node + (lb - 24);
+      atomicAdd(a.ne.A + size_t(ga) * np + gb, val);  // ga <= gb: knot dims precede bias dims
+    }
+}
 
 template <bool FULL>
 __global__ void __launch_bounds__(kImuThreads) imu_kernel(const __grid_constant__ ImuArgs a) {
-  extern __shared__ __align__(16) unsigned char dyn_smem[];
-  double* Js = reinterpret_cast<double*>(dyn_smem);            // [32 samples x 6 rows][kImuRowStride]
-  double* accs = Js + kImuMaxPerItem * 6 * kImuRowStride;      // [10][64]
-  const int tid = threadIdx.x;
+  extern __shared__ __align__(128) unsigned char dyn_smem[];
+  double* Js = reinterpret_cast<double*>(dyn_smem);  // [kImuCols][kImuColStride]: column-major rows 6 l + r of sample l
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const ImuItem item = a.items[blockIdx.x];
   double cost = 0.0;
-  if (FULL)
-    for (int i = tid; i < 10 * 64; i += kImuThreads) accs[i] = 0.0;
-  if (tid < item.count) {
-    const int n = item.start + tid;
+  ICLK(0);
+  if ((FULL || warp == 0) && lane < item.count) {
+    const int n = item.start + lane;
     const longlong2 tn = a.obs.t_node[n];
     const double2 g0 = a.obs.ga[3 * n], g1 = a.obs.ga[3 * n + 1], g2 = a.obs.ga[3 * n + 2];
     const double gyro[3] = {g0.x, g0.y, g1.x}, accel[3] = {g1.y, g2.x, g2.y};
@@ -532,94 +636,61 @@ __global__ void __launch_bounds__(kImuThreads) imu_kernel(const __grid_constant_
     int32_t s;
     double u;
     const bool ok = spline_index(a.sp, tn.x, s, u) && s == item.s;
-    double* J = Js + size_t(tid) * 6 * kImuRowStride;
+    double* J = Js + 6 * lane;
     if (!ok) {
-      atomicOr(&a.scal->error_flags, 1);
-      if (FULL)
-        for (int e = 0; e < 6 * kImuRowStride; ++e) J[e] = 0.0;
+      if (warp == 0) atomicOr(&a.scal->error_flags, 1);
+      if (FULL) imu_zero_part(J, warp);
     } else {
-      ImuEvalOut o;
-      eval_imu<FULL, kPStride>(a.sp, a.rig, a.st.q, a.st.p, a.st.tab, s, u, gyro, accel, bias, o);
-      cost = o.cost;
+      ImuStage st;
+      imu_stage<kPStride>(a.sp, a.rig, a.st.q, a.st.p, a.st.tab, s, u, gyro, accel, bias, st);
+      cost = st.cost;
       if (FULL) {
-        const int gb0 = a.dims.idx_bias0 + 6 * node;
-#pragma unroll
-        for (int r = 0; r < 6; ++r) {
-          double* Jr = J + r * kImuRowStride;
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              Jr[k * 6 + c] = a.cmask[6 * (s + k) + c] ? 0.0 : o.Jrot[k][3 * r + c];
-              Jr[k * 6 + 3 + c] = a.cmask[6 * (s + k) + 3 + c] ? 0.0 : o.Jpos[k][3 * r + c];
-            }
-#pragma unroll
-          for (int c = 0; c < 6; ++c) Jr[24 + c] = (c == r && !a.cmask[gb0 + c]) ? a.rig.imu_info[r] : 0.0;
-          Jr[30] = o.r[r];
-          Jr[31] = 0.0;
+        switch (warp) {
+          case 0: imu_write_part<false, 0>(a, st, s, node, J); break;
+          case 1: imu_write_part<false, 1>(a, st, s, node, J); break;
+          case 2: imu_write_part<true, 0>(a, st, s, node, J); break;
+          default: imu_write_part<true, 1>(a, st, s, node, J); break;
         }
       }
     }
+  } else if (FULL && lane == item.count) {
+    imu_zero_part(Js + 6 * lane, warp);
   }
   if (FULL) {
+    ICLK(1);
     __syncthreads();
-    const int grp = tid / 10, tile = tid % 10;
-    double acc[64];
-    if (tid < 60) {
-      const int ti = c_imu_tile_i[tile], tj = c_imu_tile_j[tile];
-#pragma unroll
-      for (int e = 0; e < 64; ++e) acc[e] = 0.0;
-      const int nrows = 6 * item.count;
-      for (int row = grp; row < nrows; row += 6) {
-        const double2* ra = reinterpret_cast<const double2*>(Js + size_t(row) * kImuRowStride + ti * 8);
-        const double2* rb = reinterpret_cast<const double2*>(Js + size_t(row) * kImuRowStride + tj * 8);
-        double av[8], bv[8];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const double2 x = ra[e], y = rb[e];
-          av[2 * e] = x.x; av[2 * e + 1] = x.y;
-          bv[2 * e] = y.x; bv[2 * e + 1] = y.y;
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-#pragma unroll
-          for (int j = 0; j < 8; ++j) acc[i * 8 + j] = fma(av[i], bv[j], acc[i * 8 + j]);
-      }
+    ICLK(2);
+    const int nsteps = (6 * item.count + 3) >> 2;
+    double acc[3][2];
+    switch (warp) {
+      case 0: imu_syrk<0>(Js, nsteps, lane, acc); break;
+      case 1: imu_syrk<1>(Js, nsteps, lane, acc); break;
+      case 2: imu_syrk<2>(Js, nsteps, lane, acc); break;
+      default: imu_syrk<3>(Js, nsteps, lane, acc); break;
     }
-    for (int g = 0; g < 6; ++g) {
-      if (tid < 60 && grp == g) {
-#pragma unroll
-        for (int e = 0; e < 64; ++e) accs[tile * 64 + e] += acc[e];
-      }
-      __syncthreads();
-    }
-    const int np = a.dims.np;
+    ICLK(3);
+    ICLK(4);  // (no shared-memory reduction: every tile has one owner warp)
     det_ticket_wait(a.det_ticket, blockIdx.x);
-    for (int idx = tid; idx < 10 * 64; idx += kImuThreads) {
-      const double val = accs[idx];
-      if (val == 0.0) continue;
-      const int tile2 = idx >> 6, e = idx & 63;
-      const int la = c_imu_tile_i[tile2] * 8 + (e >> 3), lb = c_imu_tile_j[tile2] * 8 + (e & 7);
-      if (la > lb || lb > 30 || la >= 30) continue;
-      const int ga = la < 24 ? 6 * item.s + la : a.dims.idx_bias0 + 6 * item.node + (la - 24);
-      if (lb == 30) {
-        atomicAdd(a.ne.gc + ga, val);
-        continue;
-      }
-      const int gb = lb < 24 ? 6 * item.s + lb : a.dims.idx_bias0 + 6 * item.node + (lb - 24);
-      atomicAdd(a.ne.A + size_t(ga) * np + gb, val);  // ga <= gb: knot dims precede bias dims
+    switch (warp) {
+      case 0: imu_flush<0>(a, item, lane, acc); break;
+      case 1: imu_flush<1>(a, item, lane, acc); break;
+      case 2: imu_flush<2>(a, item, lane, acc); break;
+      default: imu_flush<3>(a, item, lane, acc); break;
     }
+    ICLK(5);
   }
   if (!FULL) det_ticket_wait(a.det_ticket, blockIdx.x);
-  cost = warp_sum(cost);
-  if (tid == 0 && cost != 0.0) atomicAdd(a.ne.cost, cost);  // only warp 0 evaluates (count <= 32)
+  if (warp == 0) {  // every warp evaluated the same samples; warp 0's lanes hold them in sample order
+    cost = warp_sum(cost);
+    if (lane == 0 && cost != 0.0) atomicAdd(a.ne.cost, cost);
+  }
   det_ticket_done(a.det_ticket, blockIdx.x);
 }
 
 int launch_imu(const ImuLaunch& l, bool full, cudaStream_t s) {
   if (l.n_items <= 0) return 0;
   ImuArgs a{l.obs, l.items, l.st, l.ne, l.dims, l.sp, l.rig, l.cmask, l.scal, l.det_ticket};
-  const size_t smem = (size_t(kImuMaxPerItem) * 6 * kImuRowStride + 10 * 64) * sizeof(double);
+  const size_t smem = size_t(kImuCols) * kImuColStride * sizeof(double);
   static PerDeviceOnce once;
   if (once.first()) cudaFuncSetAttribute(imu_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
   if (full) imu_kernel<true><<<l.n_items, kImuThreads, smem, s>>>(a);

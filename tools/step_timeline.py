@@ -5,7 +5,8 @@
 The estimator is set up as bench.py sets it up (config_c2, SaveState / RestoreState, a 256 MiB buffer written between
 solves to flush L2).  For each profiled solve it prints every kernel / memset of the engine stream (the stream of
 gradient_norm_kernel) with its duration and the gap since the previous operation on that stream, grouped per LM step
-(a step starts at each visual_kernel), and the summed gaps of the critical chain (engine-stream operations from the
+(a step starts at each visual_kernel), the median in-solve duration of every kernel of a step on all streams, the
+evaluation phase per step (first start to last end of its factor kernels), and the summed gaps of the critical chain (engine-stream operations from the
 solve's first one up to the end of the last gradient_norm_kernel, which is where summary.device_ms ends for this solve:
 it runs all 15 iterations, so no speculated step is left behind) as a fraction of summary.device_ms.  For each gap it names the operation on another stream that ended last before the gap closed,
 when that one ended inside the gap: such a gap is a cross-stream wait, not a launch boundary.  A negative gap is overlap:
@@ -29,6 +30,7 @@ sys.path.insert(0, ROOT)
 pkg = importlib.import_module("ctrl-vio_b200")
 syn = pkg.synthetic
 MAX_ITERS = 15
+FACTOR_KERNELS = ("visual_kernel", "imu_kernel", "small_factors_kernel", "prior_add_jtj_kernel")
 
 
 def card():
@@ -86,6 +88,19 @@ def analyse(ops, device_ms):
         row = {"name": o["name"], "dur_us": o["dur"], "gap_us": gap, "after_other_stream": waited}
         (steps[-1] if steps else rows).append(row)
     span_us = chain[-1]["ts"] + chain[-1]["dur"] - chain[0]["ts"]
+    # every stream's kernels per LM step (a step's window opens when the engine-stream operation in front of its
+    # visual_kernel ends: the fork onto the other streams is recorded there), and the evaluation phase: first start to
+    # last end of the step's factor kernels (fork -> join)
+    vis = [i for i, o in enumerate(chain) if o["name"].startswith("visual_kernel")]
+    opens = [chain[i - 1]["ts"] + chain[i - 1]["dur"] if i > 0 else chain[i]["ts"] for i in vis]
+    opens.append(chain[-1]["ts"] + chain[-1]["dur"])
+    per_kernel, eval_us = {}, []
+    for a, b in zip(opens, opens[1:]):
+        ks = [o for o in ops if a <= o["ts"] < b]
+        for o in ks:
+            per_kernel.setdefault(o["name"], []).append(o["dur"])
+        fac = [o for o in ks if o["name"].split("<")[0] in FACTOR_KERNELS]
+        eval_us.append(max(o["ts"] + o["dur"] for o in fac) - min(o["ts"] for o in fac))
     by_pair = {}
     for s in steps:
         for a, b in zip(s, s[1:]):
@@ -93,6 +108,8 @@ def analyse(ops, device_ms):
     return {"engine_stream": eng, "pre_steps": rows, "steps": steps, "chain_gap_us": gaps, "chain_span_us": span_us,
             "device_ms": device_ms, "gap_fraction_of_device_ms": gaps * 1e-3 / device_ms,
             "median_gap_by_boundary_us": {k: float(np.median(v)) for k, v in by_pair.items()},
+            "median_dur_by_kernel_us": {k: float(np.median(v)) for k, v in per_kernel.items()},
+            "eval_phase_us": eval_us, "eval_phase_median_us": float(np.median(eval_us)),
             "other_stream_ops": sorted({f"{o['name']}@s{o['stream']}" for o in other})}
 
 
@@ -159,6 +176,11 @@ def main():
     print("median gap before each boundary (us):")
     for k, v in sorted(r["median_gap_by_boundary_us"].items(), key=lambda kv: -kv[1]):
         print(f"   {v:7.2f}  {k}")
+    print("median in-solve duration per kernel over the LM steps, all streams (us):")
+    for k, v in sorted(r["median_dur_by_kernel_us"].items(), key=lambda kv: -kv[1]):
+        print(f"   {v:8.2f}  {k}")
+    print(f"evaluation phase (first start -> last end of the step's factor kernels): median "
+          f"{r['eval_phase_median_us']:.2f} us over {len(r['eval_phase_us'])} steps")
     for k, r in enumerate(results):
         print(f"solve {k}: device_ms {r['device_ms']:.3f} (profiled), {r['iterations']} iterations, {r['passes']} passes; "
               f"critical-chain gaps {r['chain_gap_us']:.1f} us = {100 * r['gap_fraction_of_device_ms']:.1f} % of device_ms "
