@@ -1,6 +1,6 @@
-// The engine object behind a ctvio_handle and the host helpers engine.cu and resident.cu share.  The thread-locals are
-// C++17 inline variables, ONE object each across the library: an error raised in either file is what ctvio_last_error
-// reports, and every upload is counted.
+// The engine object behind a ctvio_handle and the host helpers engine.cu, resident.cu and solve.cu share.  The
+// thread-locals are C++17 inline variables, ONE object each across the library: an error raised in any of the files is
+// what ctvio_last_error reports, and every upload is counted.
 #pragma once
 #include <algorithm>
 #include <cstring>
@@ -137,7 +137,6 @@ struct ctvio_engine {
   DevState x[2], snap;
   DevState xs;                 // third state buffer of the pipelined LM driver (swapped into x[] when it ends up current)
   DevBuf<LmDecision> d_dec;    // device-side step decision (accept, next radius) read by the speculated linear solve
-  cudaEvent_t ev_iter = nullptr;  // recorded behind the last kernel of every LM step (before anything speculative)
   DevState& state(int i) { return i < 2 ? x[i] : xs; }
   int cur = 0;
   bool table_valid = false;
@@ -304,5 +303,13 @@ inline int ensure_table(ctvio_engine* e) {
   }
   return CTVIO_OK;
 }
+
+// engine.cu, used by the LM driver in solve.cu
+int prepare(ctvio_engine* e);  // host-side structures of the factor set, uploaded
+void evaluate(ctvio_engine* e, int xb, int nb, bool full, bool reset_cost = true);
+int read_scalars(ctvio_engine* e, bool published = false);
+LinearLaunch linear_launch(ctvio_engine* e, int nb);
+int refresh_mirror(ctvio_engine* e);
+int alloc_state(ctvio_engine* e, DevState& s);
 
 }  // namespace ctvio::host
