@@ -1430,6 +1430,12 @@ int ctvio_marginalize(ctvio_handle e, int32_t* n_out, int32_t* nb_out) {
   }
   // ---- dense Schur complement through eigen-decompositions (marginalization_factor.cpp:240-263) ----
   const double eps = 1e-30;
+  auto eig = [&](double* A, double* V, double* ev, int k) {
+    const int launched = ctvio::launch_jacobi_eig(A, V, ev, k, ws.eig_scratch.p, st);
+    if (launched < 0) return fail(CTVIO_ERR_CUDA, "marginalization: eigen-solver launch refused at n = " + std::to_string(k));
+    e->launches += launched;
+    return int(CTVIO_OK);
+  };
   DevBuf<double>&d_Amm = ws.Amm, &d_V = ws.V, &d_ev = ws.ev, &d_Vs = ws.Vs, &d_Ainv = ws.Ainv, &d_T = ws.T, &d_Ap = ws.Ap,
       &d_bp = ws.bp, &d_Ap2 = ws.Ap2, &d_V2 = ws.V2, &d_ev2 = ws.ev2, &d_vb = ws.vb, &d_J = ws.J, &d_r = ws.r;
   CUDA_OK(d_Ap.reserve(size_t(n) * n));
@@ -1442,7 +1448,7 @@ int ctvio_marginalize(ctvio_handle e, int32_t* n_out, int32_t* nb_out) {
     CUDA_OK(d_Vs.reserve(size_t(m) * m)); CUDA_OK(d_Ainv.reserve(size_t(m) * m)); CUDA_OK(d_T.reserve(size_t(n) * m));
     e->launches += ctvio::launch_marg_elementwise(0, m, P, d_A.p, d_Amm.p, nullptr, nullptr, nullptr, eps, st);
     CUDA_OK(ws.eig_scratch.reserve(ctvio::jacobi_log_bytes(std::max(m, n), 40) / sizeof(double) + 1));
-    e->launches += ctvio::launch_jacobi_eig(d_Amm.p, d_V.p, d_ev.p, m, ws.eig_scratch.p, st);
+    if ((rc = eig(d_Amm.p, d_V.p, d_ev.p, m))) return rc;
     e->launches += ctvio::launch_marg_elementwise(1, m, m, d_V.p, d_Vs.p, d_ev.p, nullptr, nullptr, eps, st);
     e->launches += ctvio::launch_dense_gemm(m, m, m, 1.0, d_Vs.p, m, false, d_V.p, m, true, 0.0, d_Ainv.p, m, st);
     // T = Arm * Amm_inv ; A' = Arr - T * Amr ; b' = brr - T * bmm
@@ -1454,7 +1460,7 @@ int ctvio_marginalize(ctvio_handle e, int32_t* n_out, int32_t* nb_out) {
   CUDA_OK(d_vb.reserve(n)); CUDA_OK(d_J.reserve(size_t(n) * n)); CUDA_OK(d_r.reserve(n));
   e->launches += ctvio::launch_marg_elementwise(2, n, n, d_Ap.p, d_Ap2.p, nullptr, nullptr, nullptr, eps, st);
   CUDA_OK(ws.eig_scratch.reserve(ctvio::jacobi_log_bytes(n, 40) / sizeof(double) + 1));
-  e->launches += ctvio::launch_jacobi_eig(d_Ap2.p, d_V2.p, d_ev2.p, n, ws.eig_scratch.p, st);
+  if ((rc = eig(d_Ap2.p, d_V2.p, d_ev2.p, n))) return rc;
   e->launches += ctvio::launch_dense_gemm(n, 1, n, 1.0, d_V2.p, n, true, d_bp.p, 1, false, 0.0, d_vb.p, 1, st);
   e->launches += ctvio::launch_marg_elementwise(3, n, n, d_V2.p, d_J.p, d_ev2.p, d_vb.p, d_r.p, eps, st);
   rc = read_scalars(e);

@@ -409,8 +409,7 @@ extern "C" int ctvio_debug_eig(int n, const double* A, double* V, double* ev, in
   if (!rc) {
     cudaMemcpy(dA, A, nn, cudaMemcpyHostToDevice);
     cudaMemset(dV, 0, nn);
-    ctvio::launch_jacobi_eig(dA, dV, dev_, n, log, 0);
-    if (cudaGetLastError() != cudaSuccess) rc = -5;
+    if (ctvio::launch_jacobi_eig(dA, dV, dev_, n, log, 0) < 0) rc = -5;
     if (cudaDeviceSynchronize() != cudaSuccess) rc = -4;
     cudaMemcpy(V, dV, nn, cudaMemcpyDeviceToHost);
     cudaMemcpy(ev, dev_, n * sizeof(double), cudaMemcpyDeviceToHost);

@@ -516,31 +516,38 @@ size_t jacobi_log_bytes(int n, int max_sweeps) {
 int launch_jacobi_eig(double* A, double* V, double* ev, int n, void* log_buf, cudaStream_t s) {
   if (n <= 0) return 0;
   constexpr int kMaxSweeps = 40;
+  // a refused launch (e.g. more dynamic shared memory than the kernel was opted into) leaves V / ev as they were: report
+  // it, the caller must not build anything from them
+  auto checked = [](int launches) { return cudaGetLastError() == cudaSuccess ? launches : -1; };
   // streaming-window sizes: blocked solver (jacobi_blocked.cu); CTVIO_JACOBI=elementwise keeps the solver below
   if (log_buf && jacobi_blocked_fits(n)) {
     const char* v = std::getenv("CTVIO_JACOBI");
-    if (!(v && std::strcmp(v, "elementwise") == 0)) return launch_jacobi_blocked(A, V, ev, n, log_buf, kMaxSweeps, s);
+    if (!(v && std::strcmp(v, "elementwise") == 0)) return checked(launch_jacobi_blocked(A, V, ev, n, log_buf, kMaxSweeps, s));
   }
   const int ne = (n + 1) & ~1, npairs = ne / 2;
   const size_t pairs = size_t(npairs) * (2 * sizeof(double) + 2 * sizeof(int));
   const size_t mat = size_t(n) * (n | 1) * sizeof(double);
   const size_t limit = 224 * 1024;
-  // per-thread block slots: npairs (npairs + 1) / 2 blocks over 1024 threads, at most 12 each (n <= ~310); 2 pairs per
+  // per-thread block slots: npairs (npairs + 1) / 2 blocks over 1024 threads, at most 12 each (n <= 312); 2 pairs per
   // thread in the replay kernel (n <= 512)
   if (size_t(npairs) * (npairs + 1) / 2 > size_t(12) * 1024 || !log_buf) {
     jacobi_eig_kernel<<<1, 1024, pairs, s>>>(A, V, ev, n, 60);
-    return 1;
+    return checked(1);
   }
+  // the replay stages kLogChunk rounds of the log next to its row of V: above the 48 KiB default from n = 245 on
+  // (62 400 B at n = 312)
+  const size_t replay = size_t(ne) * sizeof(double) + size_t(kLogChunk) * npairs * sizeof(JacobiRot);
   static PerDeviceOnce once;
-  if (once.first())
+  if (once.first()) {
     cudaFuncSetAttribute(jacobi_eig_block_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(limit));
+    cudaFuncSetAttribute(jacobi_apply_log_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(limit));
+  }
   int* rounds = reinterpret_cast<int*>(log_buf);
   JacobiRot* log = reinterpret_cast<JacobiRot*>(reinterpret_cast<unsigned char*>(log_buf) + 64);
   if (mat + pairs <= limit) jacobi_eig_block_kernel<true><<<1, 1024, mat + pairs, s>>>(A, ev, log, rounds, n, kMaxSweeps);
   else jacobi_eig_block_kernel<false><<<1, 1024, pairs, s>>>(A, ev, log, rounds, n, kMaxSweeps);
-  jacobi_apply_log_kernel<<<n, 128, size_t((n + 1) & ~1) * sizeof(double) + size_t(kLogChunk) * npairs * sizeof(JacobiRot), s>>>(
-      log, rounds, n, V);
-  return 2;
+  jacobi_apply_log_kernel<<<n, 128, replay, s>>>(log, rounds, n, V);
+  return checked(2);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -87,10 +87,10 @@ int launch_marg_imu(const MargImuArgs& a, cudaStream_t s);
 int launch_marg_small(const MargSmallArgs& a, cudaStream_t s);
 // symmetric eigen-decomposition (parallel cyclic Jacobi): A overwritten, V <- eigenvectors (columns), ev <- eigenvalues
 // log_buf: jacobi_log_bytes(n, 40) bytes of global scratch for the rotation log (eigenvalues by one CTA, eigenvectors
-// by a replay kernel with one CTA per row)
+// by a replay kernel with one CTA per row).  Returns the number of kernels launched, or -1 if a launch was refused.
 size_t jacobi_log_bytes(int n, int max_sweeps);
 int launch_jacobi_eig(double* A, double* V, double* ev, int n, void* log_buf, cudaStream_t s);
-// blocked variant (jacobi_blocked.cu): 16 <= n and the padded matrix fits one SM's shared memory (n <= 112)
+// blocked variant (jacobi_blocked.cu): 16 <= n and the padded matrix fits one SM's shared memory (n <= 128)
 bool jacobi_blocked_fits(int n);
 size_t jacobi_blocked_log_bytes(int n, int max_sweeps);
 int launch_jacobi_blocked(const double* A, double* V, double* ev, int n, void* log_buf, int max_sweeps, cudaStream_t s);
