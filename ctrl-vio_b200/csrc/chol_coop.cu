@@ -16,6 +16,7 @@
 #include <cooperative_groups.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cstdlib>
 #include <string>
 
@@ -277,6 +278,8 @@ int launch_factor_solve(const LinearLaunch& a, cudaStream_t s) {
   return launch_chol_coop(a, s);
 }
 
+static std::atomic<long long> g_coop_launches{0};
+
 int launch_chol_coop(const LinearLaunch& a, cudaStream_t s) {
   static PerDeviceOnce once;
   if (once.first()) cudaFuncSetAttribute(chol_coop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kCholCoopSmem));
@@ -298,8 +301,13 @@ int launch_chol_coop(const LinearLaunch& a, cudaStream_t s) {
     // terminates with FAILURE) instead of consuming a stale solution
     cudaGetLastError();
     cudaMemsetAsync(&scal->chol_fail, 0xff, sizeof(int32_t), s);
+  } else {
+    g_coop_launches.fetch_add(1, std::memory_order_relaxed);
   }
   return 1;
 }
+
+// test / tools hook: launches of the barrier kernel so far
+extern "C" long long ctvio_debug_chol_coop_launches() { return g_coop_launches.load(); }
 
 }  // namespace ctvio

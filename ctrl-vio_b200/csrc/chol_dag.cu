@@ -729,6 +729,7 @@ __global__ void __launch_bounds__(256, 1) chol_dag_kernel(CholDagArgs a) {
 
 constexpr int kDagCluster = 8;
 static std::atomic<long long> g_dag_cluster_launches{0};
+static std::atomic<long long> g_dag_plain_launches{0};
 // number of CTAs the DAG kernel needs for nb block columns
 static int dag_grid(int nb) { return nb * (nb + 1) / 2; }
 
@@ -834,10 +835,13 @@ int launch_chol_dag(const LinearLaunch& l, cudaStream_t s) {
     cudaGetLastError();
     return launch_chol_coop(l, s);
   }
+  g_dag_plain_launches.fetch_add(1, std::memory_order_relaxed);
   return 1;
 }
 
 // test / tools hook: launches of the tile-DAG kernel that ran with thread-block clusters so far
 extern "C" long long ctvio_debug_chol_cluster_launches() { return g_dag_cluster_launches.load(); }
+// ... and without clusters (plain cooperative launch)
+extern "C" long long ctvio_debug_chol_plain_launches() { return g_dag_plain_launches.load(); }
 
 }  // namespace ctvio

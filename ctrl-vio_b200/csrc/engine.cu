@@ -575,6 +575,12 @@ void evaluate(ctvio_engine* e, int xb, int nb, bool full, bool reset_cost) {
   if (split) cudaStreamWaitEvent(st, e->ev_join3, 0);
 }
 
+// deterministic mode: the flush tickets start at 0 before every ticketed launch (K4 takes [0], the step kernels [1]);
+// after an evaluation [0] holds the last factor CTA's value, and a CTA waiting for 0 would spin forever
+void reset_tickets(ctvio_engine* e) {
+  if (e->deterministic) cudaMemsetAsync(e->d_ticket.p, 0, 2 * sizeof(int32_t), e->stream);
+}
+
 // published = true: the last kernel of the step (gradient_norm_kernel) has been asked to write the scalar block to
 // mapped host memory with sequence number e->pub_seq: spin on it instead of copy + stream synchronise
 int read_scalars(ctvio_engine* e, bool published) {
@@ -1127,6 +1133,7 @@ int ctvio_profile_kernels(ctvio_handle e, int32_t reps, int32_t flush_l2, double
     for (int it = -3; it < reps; ++it) {
       if (flush_l2) cudaMemsetAsync(flush.p, it & 0xff, flush_bytes, st);
       cudaMemsetAsync(e->ne_slab[cur].p, 0, e->ne_slab_len * sizeof(double), st);
+      reset_tickets(e);
       cudaEventRecord(e->ev0, st);
       launch_visual(visual_launch(e, cur, cur, e->cfg.cauchy_solve), true, st);
       cudaEventRecord(e->ev1, st);
@@ -1144,6 +1151,7 @@ int ctvio_profile_kernels(ctvio_handle e, int32_t reps, int32_t flush_l2, double
   evaluate(e, cur, cur, true);
   LinearLaunch lin = linear_launch(e, cur);
   launch_jacobi_scale(lin, st);
+  reset_tickets(e);
   launch_lm_step(lin, 1e4, st);
   rc = read_scalars(e);
   if (rc) return rc;
@@ -1160,6 +1168,7 @@ int ctvio_profile_kernels(ctvio_handle e, int32_t reps, int32_t flush_l2, double
       if (flush_l2) cudaMemsetAsync(flush.p, it & 0xff, flush_bytes, st);
       if (stage == 0 || stage == 1 || stage == 2)
         cudaMemsetAsync(e->ne_slab[cur].p, 0, e->ne_slab_len * sizeof(double), st);
+      reset_tickets(e);
       cudaEventRecord(e->ev0, st);
       switch (stage) {
         case 0: launch_visual(visual_launch(e, cur, cur, e->cfg.cauchy_solve), true, st); break;
@@ -1188,6 +1197,7 @@ int ctvio_profile_kernels(ctvio_handle e, int32_t reps, int32_t flush_l2, double
     for (int it = -3; it < reps; ++it) {
       float ms;
       if (flush_l2) cudaMemsetAsync(flush.p, it & 0xff, flush_bytes, st);
+      reset_tickets(e);  // (both: K4 takes [0], the step kernels below [1])
       cudaEventRecord(e->ev0, st); launch_reduced_system(lin, 1e4, st); cudaEventRecord(e->ev1, st);
       cudaEventSynchronize(e->ev1); cudaEventElapsedTime(&ms, e->ev0, e->ev1); if (it >= 0) total3 += ms;
       if (flush_l2) cudaMemsetAsync(flush.p, it & 0xff, flush_bytes, st);
@@ -1217,6 +1227,7 @@ int ctvio_selfcheck_solver(ctvio_handle e, int32_t reps, int32_t* mismatches, do
   evaluate(e, cur, cur, true);
   LinearLaunch lin = linear_launch(e, cur);
   launch_jacobi_scale(lin, st);
+  reset_tickets(e);
   launch_reduced_system(lin, 1e4, st);
   const size_t n = size_t(e->npad), len = n * n + n;  // M | rhs are contiguous
   DevBuf<double> backup;
@@ -1246,6 +1257,94 @@ int ctvio_selfcheck_solver(ctvio_handle e, int32_t reps, int32_t* mismatches, do
   *rel_residual = bmax > 0 ? rmax / bmax : rmax;
   cudaMemsetAsync(&e->d_scal.p->error_flags, 0, sizeof(int32_t), st);
   CUDA_OK(cudaStreamSynchronize(st));
+  return CTVIO_OK;
+}
+
+// Test hook (not part of include/ctvio.h): the stages of one LM step at the current state, with the launchers lm_step
+// uses (K6 as the separate step-vector kernel: the state is not updated), and every stage's inputs and outputs copied
+// to `out`.  *len: capacity of `out` in doubles on entry, the length needed on return (out == nullptr: query only).
+// Layout, np = 6 (nK + nB) + 1, npad = np rounded up to 64, all row-major doubles:
+//   header[16]  np, npad, nL, K4 work items, gd, dHd, dir_max, chol_fail, 0...
+//   A[np][np] (upper triangle valid, unscaled) | gc[np] | hl[nL] | gl[nL] | W[nL][np] (dense; wld in column np - 1)
+//   | cmask[np] (1 = constant) | sc[np] | sl[nL] | hh[nL]           -- what K4 reads (hh: written by K4's first kernel)
+//   | M[npad][npad] (lower triangle valid) | rhs[npad]             -- K4's output, before K5 factors M in place
+//   | y[npad]                                                         -- K5
+//   | dc[np] | dl[nL]                                                 -- K6
+int ctvio_debug_lm_step(ctvio_handle e, double radius, double* out, int64_t* len) {
+  if (!e || !len || !(radius > 0.0)) return fail(CTVIO_ERR_INVALID, "bad argument");
+  cudaSetDevice(e->cfg.device);
+  int rc = prepare(e);
+  if (rc) return rc;
+  const ProblemDims d = e->dims();
+  const size_t np = size_t(d.np), nL = size_t(e->nL), npad = size_t(e->npad);
+  const size_t need = 16 + np * np + np + 2 * nL + nL * np + 2 * np + 2 * nL + npad * npad + 2 * npad + np + nL;
+  const int64_t cap = *len;
+  *len = int64_t(need);
+  if (!out) return CTVIO_OK;
+  if (cap < int64_t(need)) return fail(CTVIO_ERR_INVALID, "output slab too small");
+  ensure_table(e);
+  cudaStream_t st = e->stream;
+  const int cur = e->cur;
+  evaluate(e, cur, cur, true);
+  rc = read_scalars(e);
+  if (rc) return rc;
+  LinearLaunch lin = linear_launch(e, cur);
+  launch_jacobi_scale(lin, st);
+  reset_tickets(e);
+  launch_reduced_system(lin, radius, st);
+  double* o = out + 16;
+  double* A = o; o += np * np;
+  double* gc = o; o += np;
+  double* hl = o; o += nL;
+  double* gl = o; o += nL;
+  double* W = o; o += nL * np;
+  double* cm = o; o += np;
+  double* sc = o; o += np;
+  double* sl = o; o += nL;
+  double* hh = o; o += nL;
+  double* M = o; o += npad * npad;
+  double* rhs = o; o += npad;
+  double* y = o; o += npad;
+  double* dc = o; o += np;
+  double* dl = o;
+  // (pageable destinations: each copy has completed when it returns, so M and rhs are taken before K5 runs)
+  CUDA_OK(cudaMemcpyAsync(M, lin.M, npad * npad * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync(rhs, lin.rhs, npad * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  launch_factor_solve(lin, st);
+  CUDA_OK(cudaMemcpyAsync(y, lin.y, npad * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  launch_step_vectors(lin, st);
+  const NormalEqPtrs ne = e->ne(cur);
+  std::vector<double> Wc(size_t(e->h_woff[e->nL])), wld(nL);
+  std::vector<uint8_t> hm(np);
+  CUDA_OK(cudaMemcpyAsync(A, ne.A, np * np * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync(gc, ne.gc, np * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync(hm.data(), lin.cmask, np, cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync(sc, lin.sc, np * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync(dc, lin.dc, np * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (nL) {
+    CUDA_OK(cudaMemcpyAsync(hl, ne.hl, nL * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaMemcpyAsync(gl, ne.gl, nL * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaMemcpyAsync(wld.data(), ne.wld, nL * sizeof(double), cudaMemcpyDeviceToHost, st));
+    if (!Wc.empty()) CUDA_OK(cudaMemcpyAsync(Wc.data(), ne.W, Wc.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaMemcpyAsync(sl, lin.sl, nL * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaMemcpyAsync(hh, lin.hh, nL * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaMemcpyAsync(dl, lin.dl, nL * sizeof(double), cudaMemcpyDeviceToHost, st));
+  }
+  CUDA_OK(cudaMemcpyAsync(e->h_scal, e->d_scal.p, sizeof(LmScalars), cudaMemcpyDeviceToHost, st));
+  cudaMemsetAsync(&e->d_scal.p->error_flags, 0, sizeof(int32_t), st);
+  CUDA_OK(cudaStreamSynchronize(st));
+  std::memset(W, 0, nL * np * sizeof(double));
+  for (size_t l = 0; l < nL; ++l) {
+    for (int g = e->h_lo[l]; g < e->h_hi[l]; ++g) W[l * np + g] = Wc[size_t(e->h_woff[l]) + (g - e->h_lo[l])];
+    W[l * np + size_t(d.idx_ld)] = wld[l];
+  }
+  for (size_t i = 0; i < np; ++i) cm[i] = hm[i] ? 1.0 : 0.0;
+  const LmScalars& s = *e->h_scal;
+  std::memset(out, 0, 16 * sizeof(double));
+  out[0] = double(np); out[1] = double(npad); out[2] = double(nL); out[3] = double(e->n_schur_items);
+  out[4] = s.gd; out[5] = s.dHd; out[6] = s.dir_max; out[7] = double(s.chol_fail);
   return CTVIO_OK;
 }
 

@@ -210,6 +210,46 @@ __device__ __forceinline__ void syrk_round(const double* Jt, double* accs, int n
   __syncthreads();
 }
 
+// deterministic mode, one round of visual_kernel<true>: the landmark pieces (hl, gl, wld, W) of the round's observations
+// from the finished rows of the shared tile.  The observations of one landmark are adjacent in an item (sorted by
+// landmark), and several of them can share a round (target frames whose knot windows coincide); the lane of the first
+// one adds them all in slot order, so that no two lanes of the CTA add to the same entry at the same time.  The two knot
+// windows of an observation may overlap (same global dims): anchor side first, then the other one.  (Out of line: it
+// runs in deterministic mode only and must not cost the fast path registers.)
+__device__ __noinline__ void det_landmark_round(const VisArgs& a, const double* Jt, int base) {
+  // (the lane's slot and side and the item are re-derived here: nothing extra stays live across the call)
+  const VisualItem item = a.items[blockIdx.x];
+  const int o0 = item.start + base, nround = min(kVisObsPerRound, item.count - base);
+  const int ol = threadIdx.x >> 1, side = threadIdx.x & 1, wk0 = side ? item.wj0 : item.wi0;
+  for (int ph = 0; ph < 2; ++ph) {
+    if (ol < nround && side == ph) {
+      const int l = a.obs.meta[o0 + ol].z;
+      if (ol == 0 || a.obs.meta[o0 + ol - 1].z != l) {
+        double* Wl = a.ne.W + (a.lm.woff[l] - a.lm.lo[l]) + 6 * wk0;
+        const int cb = side * 30;
+        for (int o = ol; o < nround && a.obs.meta[o0 + o].z == l; ++o) {
+          const double* r0 = Jt + size_t(o) * kObsStride;
+          const double* r1 = r0 + kRowStride;
+          const double j0 = r0[kColRho], j1 = r1[kColRho];
+          if (j0 == 0.0 && j1 == 0.0) continue;  // invalid observation (its rows are zero): nothing to add
+          if (side == 0) {
+            atomicAdd(a.ne.hl + l, j0 * j0 + j1 * j1);
+            atomicAdd(a.ne.gl + l, j0 * r0[kColR] + j1 * r1[kColR]);
+          } else {
+            atomicAdd(a.ne.wld + l, r0[kColLd] * j0 + r1[kColLd] * j1);
+          }
+          for (int c = 0; c < 30; ++c) {
+            const double v = r0[cb + c] * j0 + r1[cb + c] * j1;
+            if (v != 0.0) atomicAdd(Wl + c, v);
+          }
+        }
+      }
+    }
+    __threadfence();
+    __syncthreads();
+  }
+}
+
 template <bool FULL>
 __global__ void __launch_bounds__(kVisThreads, 1) visual_kernel(const __grid_constant__ VisArgs a) {
   extern __shared__ __align__(128) unsigned char dyn_smem[];
@@ -386,33 +426,7 @@ __global__ void __launch_bounds__(kVisThreads, 1) visual_kernel(const __grid_con
         // deterministic mode: the landmark pieces of this round's observations from the finished rows of the shared tile
         // (same products as the per-lane atomics of the fast path), issued in the CTA's turn
         det_ticket_wait(a.det_ticket, blockIdx.x * 1024 + base / kVisObsPerRound);
-        if (active && valid) {
-          const int oi = item.start + base + ol;
-          const int l = a.obs.meta[oi].z;
-          const double j0 = row0[kColRho], j1 = row1[kColRho];
-          if (side == 0) {
-            atomicAdd(a.ne.hl + l, j0 * j0 + j1 * j1);
-            atomicAdd(a.ne.gl + l, j0 * row0[kColR] + j1 * row1[kColR]);
-          } else {
-            atomicAdd(a.ne.wld + l, row0[kColLd] * j0 + row1[kColLd] * j1);
-          }
-        }
-        // the two knot windows of an observation may overlap (same global dims): anchor side first, then the other one
-        for (int ph = 0; ph < 2; ++ph) {
-          if (active && valid && side == ph) {
-            const int oi = item.start + base + ol;
-            const int l = a.obs.meta[oi].z;
-            const double j0 = row0[kColRho], j1 = row1[kColRho];
-            double* Wl = a.ne.W + (a.lm.woff[l] - a.lm.lo[l]);
-            const int cb = side * 30, gk0 = w0[side];
-            for (int c = 0; c < 30; ++c) {
-              const double v = row0[cb + c] * j0 + row1[cb + c] * j1;
-              if (v != 0.0) atomicAdd(Wl + 6 * gk0 + c, v);
-            }
-          }
-          __threadfence();
-          __syncthreads();
-        }
+        det_landmark_round(a, Jt, base);
         det_ticket_done(a.det_ticket, blockIdx.x * 1024 + base / kVisObsPerRound);
       }
       syrk_round(Jt, accs, nround, tid);
