@@ -106,6 +106,7 @@ ABI_SYMBOLS = [
     "selfcheck_solver", "nccl_unique_id", "comm_init", "triangulate_window", "check_keyframe", "slide_window_second_new",
     "feature_table_add", "feature_table_window", "triangulate_window_from_table", "add_image_features_from_table",
     "feature_table_slide", "feature_table_landmarks", "feature_table_map", "feature_table_slide_reanchor",
+    "debug_structure",
 ]
 
 
@@ -116,7 +117,7 @@ DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enab
                        "transfer_stats", "residual_summary", "triangulate_window", "check_keyframe",
                        "slide_window_second_new", "feature_table_add", "feature_table_window", "triangulate_window_from_table",
                        "add_image_features_from_table", "feature_table_slide", "feature_table_landmarks",
-                       "feature_table_map", "feature_table_slide_reanchor")
+                       "feature_table_map", "feature_table_slide_reanchor", "debug_structure")
 
 
 def _addr(a):
@@ -550,6 +551,27 @@ class Estimator:
         a, b = C.c_int64(), C.c_int64()
         self.lib.call("transfer_stats", self.h, C.byref(a), C.byref(b), C.c_int32(int(reset)))
         return a.value, b.value
+
+    def DebugStructure(self):
+        """the structure the engine built for the current factor set (ctvio_debug_structure), as int64 arrays: desc
+        (n_desc x 4), orig, items (x 4), lo, hi, woff, schur_items (x 4), entries (x 5), active, and after a
+        marginalization that built its blocks pos_cam, pos_lm, marg_img (else None)."""
+        n = C.c_int64(0)
+        self.lib.call("debug_structure", self.h, None, C.byref(n))
+        out = np.zeros(n.value, np.int64)
+        self.lib.call("debug_structure", self.h, _lp(out), C.byref(n))
+        hdr = out[:16]
+        n_f, n_desc, n_items, nL, n_si, n_e, np_, n_marg = (int(x) for x in hdr[:8])
+        parts = [("desc", (n_desc, 4)), ("orig", (n_f,)), ("items", (n_items, 4)), ("lo", (nL,)), ("hi", (nL,)),
+                 ("woff", (nL + 1,)), ("schur_items", (n_si, 4)), ("entries", (n_e, 5)), ("active", (np_ + nL,))]
+        if n_marg >= 0:
+            parts += [("pos_cam", (np_,)), ("pos_lm", (nL,)), ("marg_img", (n_marg,))]
+        res, o = {"pos_cam": None, "pos_lm": None, "marg_img": None}, 16
+        for name, shape in parts:
+            k = int(np.prod(shape))
+            res[name] = out[o:o + k].reshape(shape)
+            o += k
+        return res
 
     def ProfileKernels(self, reps=20, flush_l2=True):
         out = np.zeros(8)

@@ -146,6 +146,12 @@ struct ctvio_engine {
   std::vector<HostImu> imu;
   std::vector<HostBias> biasf;
   bool structure_dirty = true;
+  // image factors whose descriptors live on the device (caller order): set as soon as ctvio_add_image_features_from_table
+  // adds to the factor set; slot-named factors of the same set are uploaded next to them.  No host record exists for
+  // these factors, and their structure is built by structure.cu.
+  DevBuf<ctvio::FactorDesc> d_img_in;
+  int n_img_dev = 0;
+  size_t n_img() const { return img.size() + size_t(n_img_dev); }
 
   // device factor arrays
   DevBuf<longlong2> d_img_t;
@@ -175,9 +181,15 @@ struct ctvio_engine {
   DevBuf<int64_t> d_woff;
   DevBuf<SchurTileItem> d_schur_items;
   DevBuf<double> d_lis, d_lc;
-  int n_schur_items = 0;
+  int n_schur_items = 0, n_schur_entries = 0;
+  int64_t w_len = 0;                        // length of the compact W array (woff[nL])
   DevBuf<uint8_t> d_cmask, d_active;
   std::vector<uint8_t> h_cmask, h_active;
+  // device structure build (structure.cu): scratch, its count block and the knot bitmask of the image factors' windows
+  DevBuf<uint64_t> sb_key;
+  DevBuf<int32_t> sb_idx;
+  DevBuf<uint32_t> sb_counts;
+  std::vector<uint32_t> h_struct_counts, img_knots;
 
   // normal equations (two buffers, each one slab: A | gc | hl | gl | wld | W)
   DevBuf<double> ne_slab[2];
@@ -213,7 +225,7 @@ struct ctvio_engine {
   DevBuf<float> d_cloud_stage;            // staging for one message (5 floats per point... points 3 + id + v)
   int64_t h_frame_t[16] = {0};
   int32_t h_frame_n[16] = {0};
-  std::vector<ctvio::FactorDesc> img_desc;  // parallel to img when the factors came from the resident tables
+  std::vector<ctvio::FactorDesc> img_desc;  // parallel to img when the factors are slot-named (host-built set)
   DevBuf<ctvio::FactorDesc> d_img_desc;
   DevBuf<longlong2> d_imu_tab_t;           // resident IMU table {t, 0}
   DevBuf<double2> d_imu_tab_ga;            // [cap][3]
@@ -256,10 +268,11 @@ struct ctvio_engine {
   } ft;
   // marginalization workspace (K7), kept across windows: allocation / free costs more than the kernels
   struct MargWs {
-    DevBuf<int32_t> pos_cam, pos_lm, prior_pos, marg_img, marg_imu;
+    DevBuf<int32_t> pos_cam, pos_lm, prior_pos, marg_img, marg_imu, new_type, new_index;
     DevBuf<int2> bij;
     DevBuf<double> eig_scratch, Jrow, bs, A, b, Amm, V, ev, Vs, Ainv, T, Ap, bp, Ap2, V2, ev2, vb, J, r;
   } mws;
+  int n_marg_img = -1;  // marginalized image factors of the last ctvio_marginalize (-1: pos_cam / pos_lm / marg_img not built)
 
   // multi-GPU
   void* nccl_comm = nullptr;
@@ -304,8 +317,19 @@ inline int ensure_table(ctvio_engine* e) {
   return CTVIO_OK;
 }
 
+// structure.cu: the structure build of a factor set with device-resident descriptors (T: tiles per side of the reduced
+// system).  structure_build_device reads back the one count block; schur_lists_device fills the K4 lists it sized.
+int structure_build_device(ctvio_engine* e, int T);
+int schur_lists_device(ctvio_engine* e, int T);
+// ctvio_marginalize's image part: marg_img, pos_lm relative to the first inverse-depth position (offset_pos_lm_device
+// adds it), the knot bitmask of the marginalized factors' windows and the counts, in one read-back
+int marg_discover_device(ctvio_engine* e, std::vector<uint32_t>& knots, int& n_marg, int& n_rho);
+int offset_pos_lm_device(ctvio_engine* e, int base);
+// sharded mode: per-landmark owned flags (hi > 0 of the built structure) into either buffer (may be null)
+int owned_flags_device(ctvio_engine* e, double* as_double, uint8_t* as_byte);
+
 // engine.cu, used by the LM driver in solve.cu
-int prepare(ctvio_engine* e);  // host-side structures of the factor set, uploaded
+int prepare(ctvio_engine* e);  // structures of the factor set, built on the host (or by structure.cu) and uploaded
 void evaluate(ctvio_engine* e, int xb, int nb, bool full, bool reset_cost = true);
 int read_scalars(ctvio_engine* e, bool published = false);
 LinearLaunch linear_launch(ctvio_engine* e, int nb);

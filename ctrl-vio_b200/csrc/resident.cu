@@ -93,6 +93,22 @@ int ensure_feature_table(ctvio_engine* e) {
   return CTVIO_OK;
 }
 
+// room for n descriptors in the factor set's device-side list, keeping the ones it holds
+int reserve_device_descriptors(ctvio_engine* e, size_t n) {
+  if (n > e->d_img_in.cap) CUDA_OK(e->d_img_in.grow(2 * n, 0, size_t(e->n_img_dev), e->stream));
+  return CTVIO_OK;
+}
+
+// append descriptors to the factor set's device-side list (staged through the caller's arena)
+int append_device_descriptors(ctvio_engine* e, const std::vector<ctvio::FactorDesc>& d) {
+  const size_t base = size_t(e->n_img_dev), bytes = d.size() * sizeof(ctvio::FactorDesc);
+  if (const int rc = reserve_device_descriptors(e, base + d.size())) return rc;
+  CUDA_OK(staged_h2d(e->d_img_in.p + base, d.data(), bytes, e->stream));
+  e->h2d_bytes += bytes;
+  e->n_img_dev += int(d.size());
+  return CTVIO_OK;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -352,17 +368,21 @@ int ctvio_add_image_features_from_table(ctvio_handle e, int32_t marg_oldest, int
     ctvio::FeatureTableFactorArgs a;
     a.n_landmarks = t.n_lm; a.obs_offset = t.obs_offset.p; a.obs_slot = t.obs_slot.p; a.obs_idx = t.obs_idx.p;
     a.rho = e->x[e->cur].rho.p; a.oldest_slot = t.oldest_slot; a.marg_oldest = marg_oldest ? 1 : 0;
-    a.frame_cap = ctvio_engine::kFrameCap; a.out = t.desc.p;
-    e->launches += ctvio::launch_feature_table_factors(a, st);
-    // the engine's structure build (prepare) runs on the host: the 16-byte descriptors come back, the payload stays
-    const size_t base = e->img_desc.size();
-    e->img_desc.resize(base + size_t(n));
-    if (const int rc = read_result(e, e->img_desc.data() + base, t.desc.p, size_t(n))) return rc;
-    for (size_t k = base; k < e->img_desc.size(); ++k) {
-      const ctvio::FactorDesc& d = e->img_desc[k];
-      const int si = d.slot_i / ctvio_engine::kFrameCap, sj = d.slot_j / ctvio_engine::kFrameCap;
-      e->img.push_back(HostImage{e->h_frame_t[si], e->h_frame_t[sj], 0, 0, {0, 0}, {0, 0}, d.lm, d.marg});
+    a.frame_cap = ctvio_engine::kFrameCap;
+    // the descriptors are appended to the factor set's device-side list and never come back: the structure build
+    // runs on the device (structure.cu).  Slot-named factors added before go up first, so that the list keeps the
+    // caller order.
+    if (!e->img_desc.empty()) {
+      ArenaScope arena(e);
+      if (const int rc = append_device_descriptors(e, e->img_desc)) return rc;
+      e->img.clear();
+      e->img_desc.clear();
     }
+    const size_t base = size_t(e->n_img_dev);
+    if (const int rc = reserve_device_descriptors(e, base + size_t(n))) return rc;
+    a.out = e->d_img_in.p + base;
+    e->launches += ctvio::launch_feature_table_factors(a, st);
+    e->n_img_dev += n;
   }
   e->structure_dirty = true;
   return CTVIO_OK;
@@ -601,18 +621,32 @@ int ctvio_add_image_features_from_slots(ctvio_handle e, int32_t n, const int32_t
                                         const int32_t* slot_j, const int32_t* idx_j, const int32_t* lm, const int32_t* marg) {
   if (!e || n < 0 || (n > 0 && (!slot_i || !idx_i || !slot_j || !idx_j || !lm))) return fail(CTVIO_ERR_INVALID, "null argument");
   if (!e->img.empty() && e->img_desc.empty()) return fail(CTVIO_ERR_STATE, "image factors with host payload are already present");
+  // the factors before the first bad one are added, as the call always did
+  std::vector<ctvio::FactorDesc> desc;
+  int rc = CTVIO_OK;
   for (int k = 0; k < n; ++k) {
     const int si = slot_i[k], sj = slot_j[k];
     if (si < 0 || si >= ctvio_engine::kFrameSlots || sj < 0 || sj >= ctvio_engine::kFrameSlots || idx_i[k] < 0 ||
-        idx_i[k] >= e->h_frame_n[si] || idx_j[k] < 0 || idx_j[k] >= e->h_frame_n[sj])
-      return fail(CTVIO_ERR_INVALID, "feature slot / index out of range");
-    HostImage o{e->h_frame_t[si], e->h_frame_t[sj], 0, 0, {0, 0}, {0, 0}, lm[k], marg ? marg[k] : 0};
-    e->img.push_back(o);
-    e->img_desc.push_back(ctvio::FactorDesc{si * ctvio_engine::kFrameCap + idx_i[k], sj * ctvio_engine::kFrameCap + idx_j[k], lm[k],
-                                            marg ? marg[k] : 0});
+        idx_i[k] >= e->h_frame_n[si] || idx_j[k] < 0 || idx_j[k] >= e->h_frame_n[sj]) {
+      rc = fail(CTVIO_ERR_INVALID, "feature slot / index out of range");
+      break;
+    }
+    desc.push_back(ctvio::FactorDesc{si * ctvio_engine::kFrameCap + idx_i[k], sj * ctvio_engine::kFrameCap + idx_j[k], lm[k],
+                                     marg ? marg[k] : 0});
+  }
+  if (e->n_img_dev > 0) {
+    // the set already holds table-built factors: these join them on the device, in caller order
+    cudaSetDevice(e->cfg.device);
+    ArenaScope arena(e);
+    if (const int rc2 = append_device_descriptors(e, desc)) return rc2;
+  } else {
+    for (const ctvio::FactorDesc& d : desc)
+      e->img.push_back(HostImage{e->h_frame_t[d.slot_i / ctvio_engine::kFrameCap], e->h_frame_t[d.slot_j / ctvio_engine::kFrameCap],
+                                 0, 0, {0, 0}, {0, 0}, d.lm, d.marg});
+    e->img_desc.insert(e->img_desc.end(), desc.begin(), desc.end());
   }
   e->structure_dirty = true;
-  return CTVIO_OK;
+  return rc;
 }
 
 int ctvio_ingest_imu(ctvio_handle e, int32_t n, const void* records, int32_t stride, int32_t off_gyro, int32_t off_accel,

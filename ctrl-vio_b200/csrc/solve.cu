@@ -56,9 +56,10 @@ int shard_check_ownership(ctvio_engine* e) {
   if (e->world <= 1 || e->shard_checked) return CTVIO_OK;
   cudaStream_t st = e->stream;
   std::vector<double> owned(size_t(std::max(e->nL, 1)), 0.0);
-  for (const HostImage& o : e->img) owned[o.lm] = 1.0;
   CUDA_OK(e->d_rho_sync.reserve(2 * size_t(std::max(e->nL, 1))));
-  CUDA_OK(cudaMemcpyAsync(e->d_rho_sync.p, owned.data(), owned.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  // owned: the landmarks with a factor on this rank (hi > 0 in the built structure)
+  CUDA_OK(cudaMemsetAsync(e->d_rho_sync.p, 0, owned.size() * sizeof(double), st));
+  if (const int rc = owned_flags_device(e, e->d_rho_sync.p, nullptr)) return rc;
   std::string err;
   if (!ctvio::comm_allreduce_sum(e->nccl_comm, e->d_rho_sync.p, owned.size(), st, &err)) return fail(CTVIO_ERR_NCCL, err);
   CUDA_OK(cudaMemcpyAsync(owned.data(), e->d_rho_sync.p, owned.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -76,9 +77,8 @@ int shard_sync_inv_depths(ctvio_engine* e) {
   if (e->world <= 1 || e->nL == 0) return CTVIO_OK;
   cudaStream_t st = e->stream;
   CUDA_OK(e->d_rho_sync.reserve(2 * size_t(e->nL)));
-  std::vector<uint8_t> owned(e->nL, 0);
-  for (const HostImage& o : e->img) owned[o.lm] = 1;
-  CUDA_OK(e->d_owned.upload(owned, st));
+  CUDA_OK(e->d_owned.reserve(size_t(e->nL)));
+  if (const int rc = owned_flags_device(e, nullptr, e->d_owned.p)) return rc;
   double* rho = e->x[e->cur].rho.p;
   e->launches += ctvio::launch_rho_pack(rho, e->d_owned.p, e->d_rho_sync.p, e->nL, st);
   std::string err;
@@ -293,7 +293,7 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
   // It pays at C2 / C5 sizes but was measured slower per LM step at 100 k observations and more, with identical kernels
   // while host timestamps showed the host ahead of the device - cause not found; the round trip it hides is a small
   // part of such a step anyway.  CTVIO_SPECULATION=always / never overrides the size test.
-  bool spec_size_ok = e->img.size() <= 20000;
+  bool spec_size_ok = e->n_img() <= 20000;
   if (const char* sp = std::getenv("CTVIO_SPECULATION")) {
     if (std::strcmp(sp, "always") == 0) spec_size_ok = true;
     if (std::strcmp(sp, "never") == 0) spec_size_ok = false;

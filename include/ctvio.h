@@ -209,6 +209,21 @@ int ctvio_eval_imu_factors(ctvio_handle h, int32_t want_jacobians, double* r, in
  * at the current state.  counts4 = {image, imu, bias, prior}; err_sum18 = image[2] | imu[6] | bias[6] | pad[4];
  * prior_err_sum (may be NULL) receives the n sums of the active prior. */
 int ctvio_residual_summary(ctvio_handle h, int32_t* counts4, double* err_sum18, double* prior_err_sum);
+/* The structure the engine built for the current factor set (prepare's frame-pair order, work lists and landmark
+ * layout), host-built or device-built alike, so that tests can compare the two builds.  The structure is built first
+ * when the factor set changed.  out: int64 slab, *len: its capacity in int64 on entry, the length needed on return
+ * (out == NULL: query only).  Layout:
+ *   header[16]  n factors, n_desc (n, or 0 for factors with host payload), n_items, nL, n_schur_items, n_entries, np,
+ *               n_marg (-1 before a ctvio_marginalize that built its blocks), 0...
+ *   desc[n_desc][4] (slot_i, slot_j, landmark, marg; sorted) | orig[n] (sorted position -> caller index)
+ *   | K1 items[n_items][4] (start, count, wi0, wj0) | lo[nL] | hi[nL] | woff[nL + 1]
+ *   | K4 items[n_schur_items][4] (ti, tj, first, count) | entries[n_entries][5] (l, lo, hi, 0, woff)
+ *   | active[np + nL]
+ *   | pos_cam[np] | pos_lm[nL] | marg_img[n_marg]      -- only when n_marg >= 0
+ * Traffic of the device-built structure (factors from ctvio_add_image_features_from_table): the add itself reads
+ * nothing back; the build reads back one count block of 32 + 4 * ceil(n_knots / 32) bytes; ctvio_marginalize reads
+ * back 8 + 4 * ceil(n_knots / 32) bytes for its image blocks.  This probe's own read-back is not counted. */
+int ctvio_debug_structure(ctvio_handle h, int64_t* out, int64_t* len);
 /* total cost 0.5*sum rho(|r|^2) of all factors incl. bias + prior at the current state */
 int ctvio_eval_cost(ctvio_handle h, double* cost);
 /* Schur-form normal equations at the current state: camera block H_cc (np x np, row-major, symmetric),
@@ -375,8 +390,13 @@ int ctvio_triangulate_window_from_table(ctvio_handle h, double init_depth, int32
  *   (trajectory_manager.cpp:206-236, :359-385) over the last window's landmarks: one factor per (landmark, observation
  *   other than the anchor), landmark-major, in window order within a landmark.  With marg_oldest != 0 a factor is flagged
  *   for marginalization when its anchor is the window's oldest slot and the landmark's resident inverse depth is > 0 at
- *   the time of the call.  The factors join the same path as ctvio_add_image_features_from_slots: the 16-byte
- *   descriptors are read back (counted in ctvio_transfer_stats) for the host's structure build; the payload stays resident.
+ *   the time of the call.  The 16-byte descriptors are appended to the factor set's device-side list and nothing is
+ *   read back: the next solve builds the structure (frame-pair groups, work lists, landmark layout, active mask) on the
+ *   device, bit for bit what the host builds for the same factors added through ctvio_add_image_features_from_slots,
+ *   and reads back only its count block (see ctvio_debug_structure).  Slot-named factors may be added before or after
+ *   in the same factor set; they join the device-side list in caller order.  Several calls between two
+ *   ctvio_clear_factors append.  Errors found by that build are those of the host build: CTVIO_ERR_TIME_RANGE when a
+ *   frame time's padded knot window leaves the spline, CTVIO_ERR_INVALID for a landmark out of range.
  *   Errors: CTVIO_ERR_STATE without a window since the last add / slide, when the resident inverse-depth count differs
  *   from the window's landmark count, or when image factors with host payload are present. */
 int ctvio_add_image_features_from_table(ctvio_handle h, int32_t marg_oldest, int32_t* n_factors);
