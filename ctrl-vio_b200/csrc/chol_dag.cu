@@ -32,14 +32,6 @@ namespace ctvio {
 
 namespace {
 
-__device__ __forceinline__ int ld_acquire(const int* p) {
-  int v;
-  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_release(int* p, int v) {
-  asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
 // ---- self-validating words: packets of the diagonal factorisations travel WITHOUT flag + fence ----
 // A packet word is either the sentinel (a negative quiet NaN with a payload no arithmetic produces) or final data; 8-byte
 // accesses are single-copy atomic, so a consumer spins on the data itself: ONE L2 round trip per hop instead of
@@ -109,16 +101,16 @@ __device__ __forceinline__ double sentinel_value() { return __longlong_as_double
 // all threads of the CTA: wait until *flag == epoch (thread 0 spins), then make the producer's data visible
 __device__ __forceinline__ void wait_flag(const int* flag, int epoch) {
   if (threadIdx.x == 0) {
-    while (ld_acquire(flag) != epoch) {}
+    spin_until_gpu(flag, epoch);
   }
   __syncthreads();
 }
 // two flags at once: two polling threads in different warps, one barrier
 __device__ __forceinline__ void wait_flags2(const int* f1, const int* f2, int epoch) {
   if (threadIdx.x == 0) {
-    while (ld_acquire(f1) != epoch) {}
+    spin_until_gpu(f1, epoch);
   } else if (threadIdx.x == 32) {
-    while (ld_acquire(f2) != epoch) {}
+    spin_until_gpu(f2, epoch);
   }
   __syncthreads();
 }
@@ -127,7 +119,7 @@ __device__ __forceinline__ void post_flag(int* flag, int epoch) {
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence();
-    st_release(flag, epoch);
+    st_release_gpu(flag, epoch);
   }
 }
 
@@ -476,7 +468,7 @@ __global__ void __launch_bounds__(256, 1) chol_dag_kernel(CholDagArgs a) {
     __syncthreads();
     cluster_arrive();
   }
-  // everything above touches this CTA's shared memory only; M and rhs come from schur_tile_kernel
+  // everything above touches this CTA's shared memory only; M and rhs come from reduced_system_kernel
   pdl_wait();
   pdl_launch_dependents();
   // speculated step behind a rejected / terminating one: nothing has been sent or reset yet, and the host takes the

@@ -335,8 +335,10 @@ int prepare(ctvio_engine* e) {
       CUDA_OK(e->d_schur_list.upload(flat, st));
       CUDA_OK(e->d_schur_items.upload(items, st));
     }
-    CUDA_OK(e->d_lis.reserve(e->nL));
-    CUDA_OK(e->d_lc.reserve(e->nL));
+    if (reduced_system_flags_len(e->npad) > e->d_m_flags.cap) {
+      CUDA_OK(e->d_m_flags.reserve(reduced_system_flags_len(e->npad)));
+      CUDA_OK(cudaMemsetAsync(e->d_m_flags.p, 0, e->d_m_flags.cap * sizeof(int32_t), e->stream));
+    }
     if (chol_dag_flags_len(e->npad) > e->d_chol_flags.cap) {
       CUDA_OK(e->d_chol_flags.reserve(chol_dag_flags_len(e->npad)));
       CUDA_OK(cudaMemsetAsync(e->d_chol_flags.p, 0, e->d_chol_flags.cap * sizeof(int32_t), e->stream));
@@ -535,7 +537,7 @@ LinearLaunch linear_launch(ctvio_engine* e, int nb) {
   a.schur_list = e->d_schur_list.p;
   a.schur_items = e->d_schur_items.p;
   a.n_schur_items = e->n_schur_items;
-  a.lis = e->d_lis.p; a.lc = e->d_lc.p;
+  a.m_flags = e->d_m_flags.p;
   a.cmask = e->d_cmask.p;
   a.active = e->d_active.p;
   a.sc = e->d_sc.p; a.sl = e->d_sl.p;
@@ -554,7 +556,7 @@ LinearLaunch linear_launch(ctvio_engine* e, int nb) {
 }
 
 // one pass over all residual blocks at state buffer xb into normal-equation buffer nb
-// reset_cost = false: cost_eval was already zeroed by scale_copy_kernel of the same LM step
+// reset_cost = false: cost_eval was already zeroed by reduced_system_kernel of the same LM step
 void evaluate(ctvio_engine* e, int xb, int nb, bool full, bool reset_cost) {
   cudaStream_t st = e->stream;
   if (full) {
@@ -1293,11 +1295,12 @@ int ctvio_selfcheck_solver(ctvio_handle e, int32_t reps, int32_t* mismatches, do
 // Layout, np = 6 (nK + nB) + 1, npad = np rounded up to 64, all row-major doubles:
 //   header[16]  np, npad, nL, K4 work items, gd, dHd, dir_max, chol_fail, 0...
 //   A[np][np] (upper triangle valid, unscaled) | gc[np] | hl[nL] | gl[nL] | W[nL][np] (dense; wld in column np - 1)
-//   | cmask[np] (1 = constant) | sc[np] | sl[nL] | hh[nL]           -- what K4 reads (hh: written by K4's first kernel)
+//   | cmask[np] (1 = constant) | sc[np] | sl[nL] | hh[nL]           -- what K4 reads (hh: written by K4)
 //   | M[npad][npad] (lower triangle valid) | rhs[npad]             -- K4's output, before K5 factors M in place
 //   | y[npad]                                                         -- K5
 //   | dc[np] | dl[nL]                                                 -- K6
-int ctvio_debug_lm_step(ctvio_handle e, double radius, double* out, int64_t* len) {
+// poison != 0: M and rhs are filled with NaN before K4 runs, so that an entry K4 fails to write shows in the output.
+int ctvio_debug_lm_step_poison(ctvio_handle e, double radius, double* out, int64_t* len, int32_t poison) {
   if (!e || !len || !(radius > 0.0)) return fail(CTVIO_ERR_INVALID, "bad argument");
   cudaSetDevice(e->cfg.device);
   int rc = prepare(e);
@@ -1318,6 +1321,7 @@ int ctvio_debug_lm_step(ctvio_handle e, double radius, double* out, int64_t* len
   LinearLaunch lin = linear_launch(e, cur);
   launch_jacobi_scale(lin, st);
   reset_tickets(e);
+  if (poison) CUDA_OK(cudaMemsetAsync(lin.M, 0xff, (npad * npad + npad) * sizeof(double), st));  // M | rhs: all-ones NaN
   launch_reduced_system(lin, radius, st);
   double* o = out + 16;
   double* A = o; o += np * np;
@@ -1378,6 +1382,9 @@ int ctvio_debug_lm_step(ctvio_handle e, double radius, double* out, int64_t* len
   out[0] = double(np); out[1] = double(npad); out[2] = double(nL); out[3] = double(e->n_schur_items);
   out[4] = s.gd; out[5] = s.dHd; out[6] = s.dir_max; out[7] = double(s.chol_fail);
   return CTVIO_OK;
+}
+int ctvio_debug_lm_step(ctvio_handle e, double radius, double* out, int64_t* len) {
+  return ctvio_debug_lm_step_poison(e, radius, out, len, 0);
 }
 
 int ctvio_measure_fp64_tflops(ctvio_handle e, double* tflops) {

@@ -180,7 +180,6 @@ struct ctvio_engine {
   DevBuf<SchurEntry> d_schur_list;
   DevBuf<int64_t> d_woff;
   DevBuf<SchurTileItem> d_schur_items;
-  DevBuf<double> d_lis, d_lc;
   int n_schur_items = 0, n_schur_entries = 0;
   int64_t w_len = 0;                        // length of the compact W array (woff[nL])
   DevBuf<uint8_t> d_cmask, d_active;
@@ -197,7 +196,7 @@ struct ctvio_engine {
   size_t off_gc = 0, off_hl = 0, off_gl = 0, off_wld = 0, off_W = 0;
   // linear system
   DevBuf<double> d_M, d_Linv, d_y, d_sc, d_sl, d_hh, d_dc, d_dl, d_rho_sync, d_chol_part;
-  DevBuf<int32_t> d_chol_flags;
+  DevBuf<int32_t> d_chol_flags, d_m_flags;  // tile flags of K5 and of K4 (reduced_system_kernel)
   DevBuf<uint8_t> d_owned;
   DevBuf<double> d_shard_pack, d_shard_scal;  // sharded mode: packed all-reduce buffer, scalar all-gather buffer
   int npad = 0, linv_npad = -1;

@@ -130,7 +130,7 @@ struct LmScalars {
 // writes it directly, the host spins on `seq` instead of paying a device-to-host copy plus a stream synchronisation
 // Step decision of the LM driver, taken on the device by the last kernel of a step (gradient_norm_kernel) so that the
 // linear solve of the NEXT step can be enqueued before the host has seen this step's scalars (pipelined driver,
-// engine.cu): the speculated scale_copy_kernel reads `radius_next` from device memory.
+// engine.cu): the speculated reduced_system_kernel reads `radius_next` from device memory.
 struct LmDecision {
   double radius_next;         // trust-region radius after an accepted step (Ceres 1.14 trust_region_minimizer.cc)
   double model_cost_change;   // -g'd - d'Hd / 2
@@ -183,19 +183,27 @@ inline int device_sm_count() {
 // Blocks are dispatched in index order, so a waiting CTA's predecessors are always resident or done (no deadlock).
 // The serialised flush costs time (K1 runs several times longer at C2); it is a verification / regression mode, off by default.
 #if defined(__CUDACC__)
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_gpu(int* p, int v) {
+  asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ void spin_until_gpu(const int* p, int v) {
+  while (ld_acquire_gpu(p) != v) {}
+}
 __device__ __forceinline__ void det_ticket_wait(const int* ticket, int my) {
   if (!ticket) return;
-  if (threadIdx.x == 0) {
-    int v;
-    do { asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(ticket) : "memory"); } while (v != my);
-  }
+  if (threadIdx.x == 0) spin_until_gpu(ticket, my);
   __syncthreads();
 }
 __device__ __forceinline__ void det_ticket_done(int* ticket, int my) {
   if (!ticket) return;
   __threadfence();   // this thread's atomics are performed before the ticket moves on
   __syncthreads();
-  if (threadIdx.x == 0) asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(ticket), "r"(my + 1) : "memory");
+  if (threadIdx.x == 0) st_release_gpu(ticket, my + 1);
 }
 // programmatic dependent launch (see launch_chained): both are no-ops in a kernel that was launched without it
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -291,8 +299,7 @@ struct LinearLaunch {
   const SchurEntry* schur_list; // concatenated per-tile landmark lists
   const SchurTileItem* schur_items;
   int32_t n_schur_items;
-  double* lis;                  // [nL] sl / sqrt(hh): scale of the landmark's coupling row (written by scale_copy_kernel)
-  double* lc;                   // [nL] lis * g_l
+  int32_t* m_flags;             // [reduced_system_flags_len] K4: tile (ti, tj) of M written (epoch valued, zeroed once)
   const uint8_t* cmask;
   const uint8_t* active;        // [np + nL]
   double* sc;                   // [np] Jacobi scale
@@ -323,6 +330,7 @@ int launch_lm_step(const LinearLaunch& a, double radius, cudaStream_t s);
 // the three stages of launch_lm_step, separately launchable for measurement
 // radius_dev != null: the radius is read from device memory (first double of an LmDecision)
 int launch_reduced_system(const LinearLaunch& a, double radius, cudaStream_t s, const double* radius_dev = nullptr);
+size_t reduced_system_flags_len(int npad);  // ints of LinearLaunch::m_flags
 int launch_factor_solve(const LinearLaunch& a, cudaStream_t s);
 // tile-DAG variant (chol_dag.cu): usable when every tile gets its own SM
 bool chol_dag_supported(int npad, int n_sm);
@@ -337,7 +345,7 @@ int launch_step_vectors(const LinearLaunch& a, cudaStream_t s);
 // of constant / padding dims are added after the all-reduce by launch_shard_unpack, marginalize.h)
 int launch_extract_diag(const LinearLaunch& a, cudaStream_t s);
 int launch_jacobi_scale_from_diag(const LinearLaunch& a, cudaStream_t s);
-// reset = false: the accumulator was already zeroed by scale_copy_kernel of the same LM step
+// reset = false: the accumulator was already zeroed by reduced_system_kernel of the same LM step
 // pub != nullptr: after the norm the whole scalar block is copied to *pub (mapped host memory) and pub->seq = seq
 int launch_gradient_norm(const LinearLaunch& a, const StatePtrs& st, int fix_ld, double ld_lower, double ld_upper,
                          cudaStream_t s, bool reset = true, LmPublished* pub = nullptr, unsigned long long seq = 0,

@@ -3,7 +3,7 @@
 // Replaces what Ceres does inside ceres::Solve for one trust-region step
 // (trajectory_estimator.cpp:367-408 -> Ceres 1.14 levenberg_marquardt_strategy.cc +
 // SPARSE_NORMAL_CHOLESKY; Ceres is not part of the reference repository):
-//   K4  scale_copy + schur     reduced camera system  M = S A S + D^2 - sum_l w_l w_l' / h_l
+//   K4  reduced_system         reduced camera system  M = S A S + D^2 - sum_l w_l w_l' / h_l
 //   K5  (chol_dag.cu, chol_coop.cu) dense Cholesky (NB = 64) + block triangular solves
 //   K6  backsub / quad / apply landmark back-substitution, model cost change, x (+) delta, norms
 // The Schur complement is owner-computes by OUTPUT tile: every 64x64 tile of the lower triangle of M gets the list of
@@ -11,6 +11,7 @@
 // windows still fill the GPU; a CTA builds the scaled rows of 32 landmarks at a time in shared memory and reduces
 // them with fp64 tensor-core tiles (m8n8k4), then flushes its tile once.
 #include <algorithm>
+#include <atomic>
 
 #include "dmma_tiles.cuh"
 #include <cstddef>
@@ -49,99 +50,177 @@ int launch_jacobi_scale(const LinearLaunch& a, cudaStream_t s) {
   return 1;
 }
 
-// M = S A S + clamp(diag)/radius on the full (padded, symmetric) matrix; rhs = S g
-__global__ void scale_copy_kernel(LinearLaunch a, double radius, const double* __restrict__ radius_dev) {
-  // (nothing worth starting early: every output depends on the radius gradient_norm_kernel decides, and on the
-  // accumulators it reads before this kernel may reset them)
+// ------------------------------------------------------------------------------------------------
+// K4: the damped, scaled reduced camera system M = S A S + D^2 - sum_l w_l w_l' / h_l and rhs = S g_c - sum_l w_l c_l,
+// in ONE launch.  Blocks [0, T (T + 1) / 2) are BASE CTAs, one per 64x64 tile (ti >= tj) of the lower triangle: each
+// writes its tile of S A S + damping (identity / zero on constant and padding dims) and, on the diagonal, its block of
+// rhs, then publishes the tile with an epoch-valued release flag.  The remaining blocks are ITEM CTAs, one per
+// SchurTileItem: a part of the landmark list of one tile, reduced 32 landmarks at a time on DMMA and subtracted from the
+// tile with fp64 RED atomics once the tile's base CTA has published it.  Only the lower tiles are written (the diagonal
+// tiles in full); K5 reads nothing else.
+//
+// Ordering: an item CTA spins only on the flags of base CTAs, whose block indices are all lower than its own.  Blocks
+// are dispatched in index order, so those base CTAs are resident or done when the item CTA spins, and a base CTA waits
+// for nothing but the preceding kernel (pdl_wait): no deadlock (the argument det_ticket_wait relies on).  Deterministic
+// mode: the item CTAs flush in item order, so the atomics land in the order of the item list.
+// Before pdl_wait a CTA reads only what was written two or more launches back (A, g_c, W, the landmark diagonals and
+// gradients, the Jacobi scales, the work lists): the radius, the go flag and the per-step accumulators belong to the
+// preceding gradient_norm_kernel.
+constexpr int kSchurKC = 32;   // landmarks per shared-memory operand chunk
+constexpr int kBaseTS = kCholNB + 1;  // row stride of a base CTA's tile of A (odd: its column reads are conflict-free)
+static_assert(kCholNB * kBaseTS <= 2 * kSchurKC * kTS, "the base tile lives in the item operands' shared memory");
+
+__host__ __device__ __forceinline__ int lower_tile_index(int ti, int tj) { return ti * (ti + 1) / 2 + tj; }
+size_t reduced_system_flags_len(int npad) {
+  const int T = npad / kCholNB;
+  return size_t(lower_tile_index(T, 0));
+}
+
+// per-landmark prologue of the Schur complement: damped diagonal hh and the scale is = sl / sqrt(hh) of the coupling row
+__device__ __forceinline__ double landmark_hh(double sl, double hl, double radius) {
+  const double hs = sl * sl * hl;
+  return hl > 0.0 ? hs + fmin(fmax(hs, kMinLmDiag), kMaxLmDiag) / radius : 0.0;
+}
+__device__ __forceinline__ double landmark_is(double hh, double sl) { return hh > 0.0 ? rsqrt(hh) * sl : 0.0; }
+
+// base CTA b: tile (ti, tj) of S A S + clamp(diag) / radius, rhs = S g_c on the diagonal
+__device__ __forceinline__ void reduced_base_block(const LinearLaunch& a, int b, double radius, const double* radius_dev,
+                                                   int epoch, double* Ts, double* scR, double* scC, uint8_t* cmR,
+                                                   uint8_t* cmC) {
+  const int tid = threadIdx.x;
+  int ti = 0;
+  while (lower_tile_index(ti + 1, 0) <= b) ++ti;
+  const int tj = b - lower_tile_index(ti, 0);
+  const int npad = a.npad, np = a.dims.np;
+  const int r0 = kCholNB * ti, c0 = kCholNB * tj;
+  // the tile's block of A, read row-wise from the upper triangle: Ts[x][y] = A[c0 + x][r0 + y]
+  // (M[r][c] = A[c][r] below the diagonal; diagonal tiles use Ts[x][y] for x <= y)
+#pragma unroll
+  for (int k = 0; k < kCholNB * kCholNB / 256; ++k) {
+    const int e = tid + 256 * k, x = e / kCholNB, y = e % kCholNB;
+    Ts[x * kBaseTS + y] = (c0 + x < np && r0 + y < np) ? a.ne.A[size_t(c0 + x) * np + r0 + y] : 0.0;
+  }
+  // the first landmark of this thread's share of the hh prologue below
+  const int nbase = lower_tile_index(npad / kCholNB, 0), l0 = b * 256 + tid;
+  const double sl0 = l0 < a.dims.nL ? a.sl[l0] : 0.0, hl0 = l0 < a.dims.nL ? a.ne.hl[l0] : 0.0;
+  double rg = 0.0;
+  if (tid < kCholNB) {
+    const int i = r0 + tid, j = c0 + tid;
+    scR[tid] = i < np ? a.sc[i] : 0.0;
+    cmR[tid] = i < np ? a.cmask[i] : 1;
+    scC[tid] = j < np ? a.sc[j] : 0.0;
+    cmC[tid] = j < np ? a.cmask[j] : 1;
+    if (ti == tj && i < np) rg = a.ne.gc[i];
+  }
+  __syncthreads();
   pdl_wait();
   pdl_launch_dependents();
   if (radius_dev) radius = *radius_dev;  // speculated step: decided by the previous step's gradient_norm_kernel
-  const int npad = a.npad, np = a.dims.np;
-  const size_t idx = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (idx < size_t(a.dims.nL)) {
-    // per-landmark prologue of the Schur complement: damped diagonal and the scale of the coupling row
-    const int l = int(idx);
-    const double sl = a.sl[l], hl = a.ne.hl[l];
-    const double hs = sl * sl * hl;
-    const double hh = hl > 0.0 ? hs + fmin(fmax(hs, kMinLmDiag), kMaxLmDiag) / radius : 0.0;
-    const double is = hh > 0.0 ? rsqrt(hh) * sl : 0.0;
-    a.hh[l] = hh;
-    a.lis[l] = is;
-    a.lc[l] = is * a.ne.gl[l];
-  }
-  if (idx >= size_t(npad) * npad) return;
-  const int i = int(idx / npad), j = int(idx % npad);
-  double m;
   const double ident = a.sharded ? 0.0 : 1.0;  // sharded: identity rows are set after the all-reduce
-  if (i < np && j < np) {
-    if (a.cmask[i] || a.cmask[j]) {
-      m = (i == j) ? ident : 0.0;
-    } else {
-      const double v = (i <= j) ? a.ne.A[size_t(i) * np + j] : a.ne.A[size_t(j) * np + i];
-      m = a.sc[i] * v * a.sc[j];
-      if (i == j) {
-        if (a.sharded) a.diagA[i] = v;  // unscaled local diagonal, summed over ranks with M
-        else m += fmin(fmax(m, kMinLmDiag), kMaxLmDiag) / radius;
+  double* tile = a.M + size_t(r0) * npad + c0;
+#pragma unroll 4
+  for (int k = 0; k < kCholNB * kCholNB / 256; ++k) {
+    const int e = tid + 256 * k, rr = e / kCholNB, cc = e % kCholNB;
+    const int i = r0 + rr, j = c0 + cc;
+    double m;
+    if (i < np && j < np) {
+      if (cmR[rr] || cmC[cc]) {
+        m = (i == j) ? ident : 0.0;
+      } else {
+        const double v = (i <= j) ? Ts[rr * kBaseTS + cc] : Ts[cc * kBaseTS + rr];
+        m = scR[rr] * v * scC[cc];
+        if (i == j) {
+          if (a.sharded) a.diagA[i] = v;  // unscaled local diagonal, summed over ranks with M
+          else m += fmin(fmax(m, kMinLmDiag), kMaxLmDiag) / radius;
+        }
       }
+    } else {
+      m = (i == j) ? ident : 0.0;
+      if (a.sharded && i == j) a.diagA[i] = 0.0;
     }
-  } else {
-    m = (i == j) ? ident : 0.0;
-    if (a.sharded && i == j) a.diagA[i] = 0.0;
+    if (a.sharded && i == j && i < np && cmR[rr]) a.diagA[i] = 0.0;
+    tile[size_t(rr) * npad + cc] = m;
   }
-  if (a.sharded && i == j && i < np && a.cmask[i]) a.diagA[i] = 0.0;
-  a.M[idx] = m;
-  if (j == 0) {
-    a.rhs[i] = (i < np && !a.cmask[i]) ? a.sc[i] * a.ne.gc[i] : 0.0;
-    if (i == 0) {
-      // per-step accumulators of the kernels that follow in this LM step (no separate memsets on the stream)
-      a.scal->gd = 0.0;
-      a.scal->dHd = 0.0;
-      a.scal->dir_max = 0.0;
-      a.scal->chol_fail = 0;
-      a.scal->step_norm2 = 0.0;
-      a.scal->x_norm2 = 0.0;
-      a.scal->cost_eval = 0.0;
-      a.scal->gmax = 0.0;
-    }
+  if (ti == tj && tid < kCholNB) a.rhs[r0 + tid] = (r0 + tid < np && !cmR[tid]) ? scR[tid] * rg : 0.0;
+  __syncthreads();
+  if (tid == 0) {
+    __threadfence();
+    st_release_gpu(a.m_flags + b, epoch);
+  }
+  // the landmark diagonals (step_apply_kernel reads them), and the per-step accumulators of the kernels that follow in
+  // this LM step (no separate memsets on the stream); nothing in this launch reads either
+  if (l0 < a.dims.nL) a.hh[l0] = landmark_hh(sl0, hl0, radius);
+  for (int l = l0 + nbase * 256; l < a.dims.nL; l += nbase * 256) a.hh[l] = landmark_hh(a.sl[l], a.ne.hl[l], radius);
+  if (b == 0 && tid == 0) {
+    a.scal->gd = 0.0;
+    a.scal->dHd = 0.0;
+    a.scal->dir_max = 0.0;
+    a.scal->chol_fail = 0;
+    a.scal->step_norm2 = 0.0;
+    a.scal->x_norm2 = 0.0;
+    a.scal->cost_eval = 0.0;
+    a.scal->gmax = 0.0;
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// K4: Schur complement, one part of one output tile per CTA
-constexpr int kSchurKC = 32;  // landmarks per shared-memory operand chunk
-// scaled coupling rows of landmark chunk [c0, c0 + 32) restricted to the tile's blocks -> registers
-// (thread = (landmark k, 8 consecutive dims)); cl = {c_l, v_l[line delay], first-block flag}
-__device__ __forceinline__ void schur_fetch(const LinearLaunch& a, const SchurTileItem& it, int c0, int k, int dseg,
-                                            const double* scA, const double* scB, double sc_ld, bool diag, double va[8],
-                                            double vb[8], double cl[3]) {
+// landmark k of chunk [c0, c0 + 32) of an item (thread = (landmark k, 8 consecutive dims)): its coupling row restricted
+// to the tile's blocks and its scalars, as loaded; nothing here depends on the trust-region radius
+struct SchurRow {
+  double va[8], vb[8];
+  double sl, hl, gl, wld;
+  int32_t lo, hi;  // the landmark's knot-dim range; lo < 0: no landmark in this slot
+};
+__device__ __forceinline__ void schur_load(const LinearLaunch& a, const SchurTileItem& it, int c0, int k, int dseg, bool diag,
+                                           SchurRow& r) {
 #pragma unroll
-  for (int e = 0; e < 8; ++e) va[e] = vb[e] = 0.0;
-  cl[0] = cl[1] = cl[2] = 0.0;
+  for (int e = 0; e < 8; ++e) r.va[e] = r.vb[e] = 0.0;
+  r.lo = -1;
   if (c0 + k >= it.count) return;
   const SchurEntry en = a.schur_list[it.first + c0 + k];
-  const double is = a.lis[en.l];
   const double* Wl = a.ne.W + en.woff - en.lo;
   const int ga0 = kCholNB * it.ti + dseg, gb0 = kCholNB * it.tj + dseg;
-  cl[0] = a.lc[en.l];
-  cl[1] = is * a.ne.wld[en.l] * sc_ld;
-  cl[2] = en.lo / kCholNB == it.ti ? 1.0 : 0.0;  // exactly one diagonal tile counts the landmark's ld-ld / ld-rhs terms
+  r.lo = en.lo;
+  r.hi = en.hi;
+  r.sl = a.sl[en.l];
+  r.hl = a.ne.hl[en.l];
+  r.gl = a.ne.gl[en.l];
+  r.wld = a.ne.wld[en.l];
   if (ga0 + 8 > en.lo && ga0 < en.hi) {
 #pragma unroll
     for (int e = 0; e < 8; ++e)
-      if (ga0 + e >= en.lo && ga0 + e < en.hi) va[e] = is * Wl[ga0 + e] * scA[dseg + e];
+      if (ga0 + e >= en.lo && ga0 + e < en.hi) r.va[e] = Wl[ga0 + e];
   }
   if (!diag && gb0 + 8 > en.lo && gb0 < en.hi) {
 #pragma unroll
     for (int e = 0; e < 8; ++e)
-      if (gb0 + e >= en.lo && gb0 + e < en.hi) vb[e] = is * Wl[gb0 + e] * scB[dseg + e];
+      if (gb0 + e >= en.lo && gb0 + e < en.hi) r.vb[e] = Wl[gb0 + e];
+  }
+}
+// -> the scaled rows v = is W_l S in place, and cl = {c_l = is g_l, v_l[line delay], first-block flag}
+__device__ __forceinline__ void schur_scale(const SchurTileItem& it, int dseg, const double* scA, const double* scB,
+                                            double sc_ld, bool diag, double radius, SchurRow& r, double cl[3]) {
+  cl[0] = cl[1] = cl[2] = 0.0;
+  if (r.lo < 0) return;
+  const double is = landmark_is(landmark_hh(r.sl, r.hl, radius), r.sl);
+  const int ga0 = kCholNB * it.ti + dseg, gb0 = kCholNB * it.tj + dseg;
+  cl[0] = is * r.gl;
+  cl[1] = is * r.wld * sc_ld;
+  cl[2] = r.lo / kCholNB == it.ti ? 1.0 : 0.0;  // exactly one diagonal tile counts the landmark's ld-ld / ld-rhs terms
+#pragma unroll
+  for (int e = 0; e < 8; ++e)
+    if (ga0 + e >= r.lo && ga0 + e < r.hi) r.va[e] = is * r.va[e] * scA[dseg + e];
+  if (!diag) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e)
+      if (gb0 + e >= r.lo && gb0 + e < r.hi) r.vb[e] = is * r.vb[e] * scB[dseg + e];
   }
 }
 
-__global__ void __launch_bounds__(256, 2) schur_tile_kernel(LinearLaunch a) {
-  __shared__ __align__(16) double At[kSchurKC * kTS];
-  __shared__ __align__(16) double Bt[kSchurKC * kTS];
-  __shared__ double scA[kCholNB], scB[kCholNB], cvec[3][kSchurKC];
-  const SchurTileItem it = a.schur_items[blockIdx.x];
+// item CTA: part `item` of the landmark list of one output tile
+__device__ __forceinline__ void reduced_item_block(const LinearLaunch& a, int item, double radius, const double* radius_dev,
+                                                   int epoch, double* At, double* Bt, double* scA, double* scB,
+                                                   double (*cvec)[kSchurKC]) {
+  const SchurTileItem it = a.schur_items[item];
   const int tid = threadIdx.x;
   const Lane L = lane_of(tid);
   const int np = a.dims.np, npad = a.npad, ild = a.dims.idx_ld;
@@ -152,29 +231,32 @@ __global__ void __launch_bounds__(256, 2) schur_tile_kernel(LinearLaunch a) {
     scB[tid] = (gb < np && !a.cmask[gb]) ? a.sc[gb] : 0.0;
   }
   const double sc_ld = a.cmask[ild] ? 0.0 : a.sc[ild];
-  const int go = a.go ? *a.go : 1;  // (issued together with the loads above; written two launches back)
+  const int k = tid >> 3, dseg = (tid & 7) * 8;
+  SchurRow row;
+  schur_load(a, it, 0, k, dseg, diag, row);  // the first chunk's loads fly through the wait
   __syncthreads();
-  pdl_wait();  // lis, lc and M come from scale_copy_kernel
+  pdl_wait();
   pdl_launch_dependents();
+  const int go = a.go ? *a.go : 1;
+  if (radius_dev) radius = *radius_dev;  // (one round trip for both loads)
   if (!go) return;  // speculated step behind a rejected / terminating one
   Frag acc;
   frag_zero(acc);
   // diagonal tiles also own, for their block: rhs -= sum_l v_l c_l and the line-delay row M[ld][block] -= sum_l v_l vld_l;
   // lanes 0..31 of warp 0 (one landmark slot each) collect the ld-ld and ld-rhs terms of the landmarks starting here
   double racc = 0.0, lacc = 0.0, ll = 0.0, lr = 0.0;
-  const int k = tid >> 3, dseg = (tid & 7) * 8;
-  double va[8], vb[8], cl[3];
-  schur_fetch(a, it, 0, k, dseg, scA, scB, sc_ld, diag, va, vb, cl);
   for (int c0 = 0; c0 < it.count; c0 += kSchurKC) {
+    double cl[3];
+    schur_scale(it, dseg, scA, scB, sc_ld, diag, radius, row, cl);
 #pragma unroll
     for (int e = 0; e < 8; e += 2) {
-      *reinterpret_cast<double2*>(At + k * kTS + dseg + e) = make_double2(va[e], va[e + 1]);
-      if (!diag) *reinterpret_cast<double2*>(Bt + k * kTS + dseg + e) = make_double2(vb[e], vb[e + 1]);
+      *reinterpret_cast<double2*>(At + k * kTS + dseg + e) = make_double2(row.va[e], row.va[e + 1]);
+      if (!diag) *reinterpret_cast<double2*>(Bt + k * kTS + dseg + e) = make_double2(row.vb[e], row.vb[e + 1]);
     }
     if ((tid & 7) == 0) { cvec[0][k] = cl[0]; cvec[1][k] = cl[1]; cvec[2][k] = cl[2]; }
     __syncthreads();
     // the next chunk's global loads fly while the tensor cores chew on this one
-    if (c0 + kSchurKC < it.count) schur_fetch(a, it, c0 + kSchurKC, k, dseg, scA, scB, sc_ld, diag, va, vb, cl);
+    if (c0 + kSchurKC < it.count) schur_load(a, it, c0 + kSchurKC, k, dseg, diag, row);
     tile_gemm_dmma<false, kSchurKC>(At, diag ? At : Bt, acc, L);
     if (diag) {
       if (tid < kCholNB) {
@@ -193,8 +275,16 @@ __global__ void __launch_bounds__(256, 2) schur_tile_kernel(LinearLaunch a) {
     }
     __syncthreads();
   }
-  // flush: M_tile -= acc (several parts may share a tile: fp64 RED atomics), rhs_block -= racc
-  det_ticket_wait(a.det_ticket, blockIdx.x);
+  // flush: M_tile -= acc (several parts may share a tile: fp64 RED atomics), rhs_block -= racc, once the base CTAs of the
+  // tiles written here have published them: the tile itself and, for a diagonal tile, the line-delay row's tiles
+  {
+    const int tl = ild / kCholNB;
+    if (tid == 0) spin_until_gpu(a.m_flags + lower_tile_index(it.ti, it.tj), epoch);
+    else if (diag && tid == 32) spin_until_gpu(a.m_flags + lower_tile_index(tl, it.ti), epoch);
+    else if (diag && tid == 64) spin_until_gpu(a.m_flags + lower_tile_index(tl, tl), epoch);
+    __syncthreads();
+  }
+  det_ticket_wait(a.det_ticket, item);
   double* tile = a.M + size_t(kCholNB) * it.ti * npad + kCholNB * it.tj;
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
@@ -218,7 +308,17 @@ __global__ void __launch_bounds__(256, 2) schur_tile_kernel(LinearLaunch a) {
       }
     }
   }
-  det_ticket_done(a.det_ticket, blockIdx.x);
+  det_ticket_done(a.det_ticket, item);
+}
+
+__global__ void __launch_bounds__(256, 2) reduced_system_kernel(LinearLaunch a, double radius,
+                                                                const double* __restrict__ radius_dev, int epoch) {
+  __shared__ __align__(16) double opnd[2 * kSchurKC * kTS];  // item: At | Bt; base: the tile of A
+  __shared__ double scA[kCholNB], scB[kCholNB], cvec[3][kSchurKC];
+  __shared__ uint8_t cmA[kCholNB], cmB[kCholNB];
+  const int nbase = lower_tile_index(a.npad / kCholNB, 0);
+  if (int(blockIdx.x) < nbase) reduced_base_block(a, blockIdx.x, radius, radius_dev, epoch, opnd, scA, scB, cmA, cmB);
+  else reduced_item_block(a, blockIdx.x - nbase, radius, radius_dev, epoch, opnd, opnd + kSchurKC * kTS, scA, scB, cvec);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -343,15 +443,13 @@ int launch_jacobi_scale_from_diag(const LinearLaunch& a, cudaStream_t s) {
 }
 
 int launch_reduced_system(const LinearLaunch& a, double radius, cudaStream_t s, const double* radius_dev) {
-  int launches = 0;
-  const size_t total = std::max(size_t(a.npad) * a.npad, size_t(a.dims.nL));
-  launch_chained(a.pdl, scale_copy_kernel, dim3(unsigned((total + 255) / 256)), dim3(256), 0, s, a, radius, radius_dev);
-  ++launches;
-  if (a.n_schur_items > 0) {
-    launch_chained(a.pdl, schur_tile_kernel, dim3(a.n_schur_items), dim3(256), 0, s, a);
-    ++launches;
-  }
-  return launches;
+  // process-wide unique, never 0 (flag buffers start zeroed): a tile flag never holds the epoch of a launch before it
+  static std::atomic<unsigned> epoch_src{0};
+  const int epoch = int(epoch_src.fetch_add(1, std::memory_order_relaxed) % 0x7ffffffeu) + 1;
+  const int nbase = lower_tile_index(a.npad / kCholNB, 0);
+  launch_chained(a.pdl, reduced_system_kernel, dim3(unsigned(nbase + a.n_schur_items)), dim3(256), 0, s, a, radius,
+                 radius_dev, epoch);
+  return 1;
 }
 
 int launch_step_vectors(const LinearLaunch& a, cudaStream_t s) {

@@ -49,9 +49,9 @@ int shard_consensus(ctvio_engine* e, int local_rc) {
   return CTVIO_OK;
 }
 
-// sharded mode: the landmark prologue (hh, lis, lc) and the per-landmark Schur terms are formed from rank-local sums, so
-// all observations of one landmark must live on ONE rank.  Checked once per structure change with one all-reduce of the
-// per-landmark owner counts.
+// sharded mode: the landmark prologue (hh, the scale of the coupling row) and the per-landmark Schur terms are formed
+// from rank-local sums, so all observations of one landmark must live on ONE rank.  Checked once per structure change
+// with one all-reduce of the per-landmark owner counts.
 int shard_check_ownership(ctvio_engine* e) {
   if (e->world <= 1 || e->shard_checked) return CTVIO_OK;
   cudaStream_t st = e->stream;
@@ -329,7 +329,7 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
       // everything enqueued so far has completed (scalars were read back): the clear overlaps lm_step; with speculated
       // kernels in flight it is done in stream order by evaluate()
       if (!spec_in_flight) prezero_slab(e, cand_ne);
-      // (scale_copy_kernel of lm_step zeroes step_norm2 / x_norm2 / cost_eval / gmax: no memsets on the stream)
+      // (reduced_system_kernel of lm_step zeroes step_norm2 / x_norm2 / cost_eval / gmax: no memsets on the stream)
       rc = lm_step(e, cur_ne, radius, apply_launch(e, cur, cand, 1.0), pipelined);
       if (rc) return rc;
     }
@@ -340,7 +340,7 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
       const LmDecideArgs da{e->d_dec.p, x_cost, radius, min_relative_decrease, max_radius,
                             parameter_tolerance, function_tolerance, gradient_tolerance, min_radius};
       gradient_norm(e, cand, cand_ne, false, true, &da);
-      // (no stream operation between this kernel and the speculated scale_copy_kernel: it would cost the two kernels
+      // (no stream operation between this kernel and the speculated reduced_system_kernel: it would cost the two kernels
       // their programmatic dependent launch; ev1 is recorded after the loop, DESIGN §4)
       // ---- speculate: step iter + 1 from (cand, cand_ne), radius from the device-side decision ----
       spec_ready = false;
