@@ -99,7 +99,7 @@ ABI_SYMBOLS = [
     "clear_factors", "add_image_features", "add_imu_measurements", "add_bias_factors", "set_prior",
     "solve", "gauge_realign", "marginalize", "get_prior", "adopt_prior",
     "save_state", "restore_state",
-    "eval_image_factors", "eval_imu_factors", "residual_summary", "eval_cost", "normal_equations",
+    "eval_image_factors", "eval_imu_factors", "residual_summary", "eval_cost", "normal_equations", "covariance",
     "query_trajectory", "triangulate",
     "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior", "ingest_feature_cloud", "add_image_features_from_slots",
     "ingest_imu", "add_imu_from_table", "transfer_stats", "profile_kernels", "measure_fp64_tflops", "measure_fp64_tensor_tflops",
@@ -111,13 +111,14 @@ ABI_SYMBOLS = [
 
 
 # entry points a checker library (the CPU oracle mirrors the ABI under `ctvo_`) need not provide: multi-GPU plumbing and
-# the device-residency / wire-format calls, which have no CPU meaning
+# the device-residency / wire-format calls, which have no CPU meaning, and the covariance, which the tests form from the
+# oracle's normal equations instead
 DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enable_prior", "extend_knots_to", "slide_window", "remap_landmarks",
                        "ingest_feature_cloud", "add_image_features_from_slots", "ingest_imu", "add_imu_from_table",
                        "transfer_stats", "residual_summary", "triangulate_window", "check_keyframe",
                        "slide_window_second_new", "feature_table_add", "feature_table_window", "triangulate_window_from_table",
                        "add_image_features_from_table", "feature_table_slide", "feature_table_landmarks",
-                       "feature_table_map", "feature_table_slide_reanchor", "debug_structure")
+                       "feature_table_map", "feature_table_slide_reanchor", "debug_structure", "covariance")
 
 
 def _addr(a):
@@ -377,6 +378,17 @@ class Estimator:
         cost = C.c_double()
         self.lib.call("normal_equations", self.h, _dp(H), _dp(g), _dp(hl), _dp(gl), C.byref(cost))
         return H, g, hl, gl, cost.value
+
+    def Covariance(self, want_cc=True, want_rho=True):
+        """ceres::Covariance of the camera-side block and the inverse depths at the current state (ctvio_covariance):
+        (cov_cc [np, np] or None, var_rho [n_lm] or None, rcond).  Raises CtvioError on a rank-deficient window, with
+        rcond in the message."""
+        npd = self.np_dim
+        cc = np.zeros((npd, npd)) if want_cc else None
+        vr = np.zeros(self.n_lm) if want_rho else None
+        rcond = C.c_double()
+        self.lib.call("covariance", self.h, _dp(cc), _dp(vr), C.byref(rcond))
+        return cc, vr, rcond.value
 
     def QueryTrajectory(self, t):
         t = _i64(t); n = t.shape[0]

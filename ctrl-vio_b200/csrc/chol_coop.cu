@@ -269,12 +269,14 @@ extern "C" int ctvio_debug_latency(int nthreads, long long* out6) {
 }
 #endif
 
-int launch_factor_solve(const LinearLaunch& a, cudaStream_t s) {
+int launch_factor_solve(const LinearLaunch& a, cudaStream_t s, bool* tile_dag) {
   // CTVIO_CHOL=coop forces the barrier kernel (A/B measurements, tests/...::test_barrier_cholesky_fallback_*); read on
   // every call (a getenv costs nanoseconds against the kernel) so that one process can exercise both paths
   const char* env = std::getenv("CTVIO_CHOL");
   const int mode = (env && std::string(env) == "coop") ? 1 : 0;
-  if (mode == 0 && a.chol_part && a.chol_flags && chol_dag_supported(a.npad, device_sm_count())) return launch_chol_dag(a, s);
+  if (mode == 0 && a.chol_part && a.chol_flags && chol_dag_supported(a.npad, device_sm_count()))
+    return launch_chol_dag(a, s, tile_dag);
+  if (tile_dag) *tile_dag = false;
   return launch_chol_coop(a, s);
 }
 

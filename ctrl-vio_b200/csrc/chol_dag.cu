@@ -755,7 +755,7 @@ int launch_chol_dag_init(double* linv_buf, double* part_buf, int npad, cudaStrea
   return 2;
 }
 
-int launch_chol_dag(const LinearLaunch& l, cudaStream_t s) {
+int launch_chol_dag(const LinearLaunch& l, cudaStream_t s, bool* tile_dag) {
   static PerDeviceOnce once;
   static std::atomic<unsigned> epoch_src{0};
   if (once.first()) cudaFuncSetAttribute(chol_dag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kCholDagSmem));
@@ -813,6 +813,7 @@ int launch_chol_dag(const LinearLaunch& l, cudaStream_t s) {
     if (cerr == cudaSuccess) {
       cluster_state.store(1, std::memory_order_relaxed);
       g_dag_cluster_launches.fetch_add(1, std::memory_order_relaxed);
+      if (tile_dag) *tile_dag = true;
       return 1;
     }
     cudaGetLastError();
@@ -825,10 +826,19 @@ int launch_chol_dag(const LinearLaunch& l, cudaStream_t s) {
     // the flag protocol needs every CTA resident; if the runtime cannot promise that (MIG slice, fewer usable SMs than
     // reported, ...) the barrier kernel with its own, smaller grid is the safe path
     cudaGetLastError();
+    if (tile_dag) *tile_dag = false;
     return launch_chol_coop(l, s);
   }
   g_dag_plain_launches.fetch_add(1, std::memory_order_relaxed);
+  if (tile_dag) *tile_dag = true;
   return 1;
+}
+
+const double* chol_dag_last_packets(const double* linv_buf, int npad, unsigned chol_seq) {
+  // launch_chol_dag used parity (chol_seq - 1) & 1 and then advanced the counter; nothing resets those packets until the
+  // next launch of the other parity has ended
+  const size_t half = size_t(npad / kCholNB) * 4 * kPacketG;
+  return linv_buf + size_t(npad) * kCholNB + ((chol_seq - 1u) & 1u) * half;
 }
 
 // test / tools hook: launches of the tile-DAG kernel that ran with thread-block clusters so far

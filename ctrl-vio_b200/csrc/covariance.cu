@@ -1,0 +1,353 @@
+// ctvio_covariance: the marginal covariance of the window at the current state, from the factor of the LM step's own
+// reduced camera system (ceres::Covariance with its defaults, which the reference's trajectory_estimator.h:23 makes
+// available to its callers; Ceres is not part of the reference repository).
+//
+//   evaluation  K1-K3 with full Jacobians into the spare normal-equation buffer
+//   K4          reduced_system_kernel at radius +inf: no damping, S_s = D S D (D the Jacobi scale) with identity rows on
+//               the dims that get no covariance
+//   K5          the LM step's Cholesky (tile DAG or barrier kernel), S_s = L L'
+//   cov_*       L^-1 tile by tile, Sigma = D L^-T L^-1 D (the camera block of H^-1, by the Schur-complement identity), and
+//               the landmark inverse-depth variances 1 / h_l + v_l' Sigma v_l, v_l = W_l / h_l
+//
+// Every product of 64x64 tiles runs on the fp64 tensor path (mma.sync.m8n8k4.f64, full-tile instantiations only: no
+// DMMA under a run-time predicate, DESIGN §4).  No atomics: the result is bitwise reproducible for a given H.
+#include <cmath>
+#include <cstdio>
+
+#include "chol_tiles.cuh"
+#include "dmma_tiles.cuh"
+#include "engine_state.h"
+
+namespace ctvio {
+
+namespace {
+
+constexpr size_t kCovTileSmem = 2 * size_t(kTile) * sizeof(double);                          // two operand tiles
+constexpr size_t kCovDiagSmem = (4 * size_t(kPacket) + size_t(kTile)) * sizeof(double);      // 4 packets + the inverse
+
+// smem tile (row stride kTS) <- 64x64 row-major global block with row stride ld
+__device__ __forceinline__ void load_tile_rm(double* dst, const double* src, int ld, int tid) {
+  for (int e = tid; e < kCholNB * kCholNB / 2; e += 256) {
+    const int r = e >> 5, c = (e & 31) * 2;
+    *reinterpret_cast<double2*>(dst + r * kTS + c) = *reinterpret_cast<const double2*>(src + size_t(r) * ld + c);
+  }
+}
+
+// At[c][r] = L(ti, tj)[r][c], the A operand layout of tile_gemm_dmma, from K5's output in M
+__device__ __forceinline__ void load_factor_tile_t(double* At, const CovLaunch& c, int ti, int tj, int tid) {
+  const double* slot = c.M + size_t(ti) * kCholNB * c.npad + size_t(tj) * kCholNB;
+  if (c.tile_dag) load_tile_rm(At, slot, c.npad, tid);  // the DAG publishes its tiles transposed inside the slot
+  else load_tile_transposed(At, c.M, c.npad, ti * kCholNB, tj * kCholNB, tid);
+}
+
+// fragments -> global 64x64 tile (row stride ld)
+__device__ __forceinline__ void frag_store_global(double* dst, int ld, const Frag& f, const Lane& L) {
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt)
+      *reinterpret_cast<double2*>(dst + size_t(L.row(mt)) * ld + L.col(nt)) = make_double2(f.c[mt][nt][0], f.c[mt][nt][1]);
+}
+
+__device__ __forceinline__ double warp_min_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+__device__ __forceinline__ double warp_max_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+}  // namespace
+
+__global__ void cov_mask_kernel(const uint8_t* __restrict__ active, int np, uint8_t* __restrict__ cmask) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < np) cmask[i] = active[i] ? 0 : 1;
+}
+
+// CTA k: X(k,k) = L(k,k)^-1 (upper triangle zero) and the extreme pivots of block k.  The barrier kernel keeps the
+// inverse (Linv); the tile DAG keeps the block as four packets, inverted here as its own backward sweep does.
+__global__ void __launch_bounds__(256) cov_diag_inverse_kernel(CovLaunch c) {
+  extern __shared__ __align__(16) double cov_smem[];
+  double* Xi = cov_smem;
+  double* Pk = Xi + kTile;
+  __shared__ double red[2][8];
+  const int k = blockIdx.x, tid = threadIdx.x;
+  if (c.tile_dag) {
+    const double* src = c.packets + size_t(k) * 4 * kPacketG;
+    for (int e = tid; e < 4 * 16 * 40; e += 256) {  // [s][m][80] -> [s][m][kPS]
+      const int row = e / 40, col = (e - row * 40) * 2;
+      *reinterpret_cast<double2*>(Pk + row * kPS + col) = *reinterpret_cast<const double2*>(src + row * 80 + col);
+    }
+    __syncthreads();
+    inverse_from_packets(Pk, Xi, tid);
+    __syncthreads();
+  } else {
+    load_tile_rm(Xi, c.Linv + size_t(k) * kCholNB * kCholNB, kCholNB, tid);
+    __syncthreads();
+  }
+  double* dst = c.X + size_t(k) * kCholNB * c.npad + size_t(k) * kCholNB;
+  for (int e = tid; e < kCholNB * kCholNB / 2; e += 256) {
+    const int r = e >> 5, cc = (e & 31) * 2;
+    *reinterpret_cast<double2*>(dst + size_t(r) * c.npad + cc) = *reinterpret_cast<const double2*>(Xi + r * kTS + cc);
+  }
+  // 1 / L_ii = X_ii over the free dims of the block (constant and padding dims carry the identity)
+  double mn = INFINITY, mx = 0.0;
+  if (tid < kCholNB) {
+    const int g = k * kCholNB + tid;
+    if (g < c.np && !c.cmask[g]) mn = mx = Xi[tid * kTS + tid];
+  }
+  if (tid < kCholNB) {
+    mn = warp_min_d(mn);
+    mx = warp_max_d(mx);
+    if ((tid & 31) == 0) { red[0][tid >> 5] = mn; red[1][tid >> 5] = mx; }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    c.piv[2 * k] = fmin(red[0][0], red[0][1]);
+    c.piv[2 * k + 1] = fmax(red[1][0], red[1][1]);
+  }
+}
+
+// CTA j: block column j of X = L^-1, top to bottom: X(i,j) = -X(i,i) sum_{k=j}^{i-1} L(i,k) X(k,j), i > j.  Each step
+// reads the blocks of column j this CTA wrote before it (global memory, ordered by the CTA barrier).
+__global__ void __launch_bounds__(256) cov_column_kernel(CovLaunch c) {
+  extern __shared__ __align__(16) double cov_smem[];
+  double* At = cov_smem;
+  double* Bt = At + kTile;
+  const int j = blockIdx.x, tid = threadIdx.x, nb = c.npad / kCholNB;
+  const Lane L = lane_of(tid);
+#pragma unroll 1
+  for (int i = j + 1; i < nb; ++i) {
+    Frag t;
+    frag_zero(t);
+#pragma unroll 1
+    for (int k = j; k < i; ++k) {
+      load_factor_tile_t(At, c, i, k, tid);
+      load_tile_rm(Bt, c.X + size_t(k) * kCholNB * c.npad + size_t(j) * kCholNB, c.npad, tid);  // Bt[k'][n] = X(k,j)[k'][n]
+      __syncthreads();
+      tile_gemm_dmma<false>(At, Bt, t, L);
+      __syncthreads();
+    }
+    frag_store(Bt, t, L);
+    load_tile_transposed(At, c.X, c.npad, i * kCholNB, i * kCholNB, tid);  // At[c][r] = X(i,i)[r][c]
+    __syncthreads();
+    Frag x;
+    frag_zero(x);
+    tile_gemm_dmma<true>(At, Bt, x, L);
+    frag_store_global(c.X + size_t(i) * kCholNB * c.npad + size_t(j) * kCholNB, c.npad, x, L);
+    __syncthreads();
+  }
+}
+
+// CTA per lower tile (i, j): Sigma_s(i,j) = sum_{k >= i} X(k,i)' X(k,j), written as D Sigma_s D into both triangles of the
+// covariance, zero on the dims that get none.  A diagonal tile writes its lower half and mirrors it: exactly symmetric.
+__global__ void __launch_bounds__(256) cov_sigma_kernel(CovLaunch c) {
+  extern __shared__ __align__(16) double cov_smem[];
+  double* At = cov_smem;
+  double* Bt = At + kTile;
+  const int tid = threadIdx.x, nb = c.npad / kCholNB;
+  int i = 0;
+  while ((i + 1) * (i + 2) / 2 <= int(blockIdx.x)) ++i;
+  const int j = int(blockIdx.x) - i * (i + 1) / 2;
+  const Lane L = lane_of(tid);
+  Frag f;
+  frag_zero(f);
+#pragma unroll 1
+  for (int k = i; k < nb; ++k) {
+    const double* row = c.X + size_t(k) * kCholNB * c.npad;
+    load_tile_rm(At, row + size_t(i) * kCholNB, c.npad, tid);  // At[c][r] = X(k,i)[c][r]
+    if (i != j) load_tile_rm(Bt, row + size_t(j) * kCholNB, c.npad, tid);
+    __syncthreads();
+    tile_gemm_dmma<false>(At, i != j ? Bt : At, f, L);
+    __syncthreads();
+  }
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int r = L.row(mt), cc = L.col(nt) + e;
+        const int gi = i * kCholNB + r, gj = j * kCholNB + cc;
+        if (gi >= c.np || gj >= c.np || (i == j && cc > r)) continue;
+        const double v = (c.cmask[gi] || c.cmask[gj]) ? 0.0 : c.sc[gi] * f.c[mt][nt][e] * c.sc[gj];
+        c.cov[size_t(gi) * c.np + gj] = v;
+        c.cov[size_t(gj) * c.np + gi] = v;
+      }
+}
+
+// one warp per landmark: var_l = 1 / h_l + (w_l' Sigma w_l) / h_l^2 over its coupling row [lo, hi) + the line delay;
+// lane b takes the columns b, b + 32, ... of every row, then one fixed shuffle tree: bitwise reproducible
+__global__ void __launch_bounds__(256) landmark_variance_kernel(LandmarkVarLaunch v) {
+  const int lane = threadIdx.x & 31;
+  const int l = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (l >= v.nL) return;
+  const double hl = v.ne.hl[l];
+  if (!v.active[v.np + l]) {
+    if (lane == 0) v.var[l] = 0.0;
+    return;
+  }
+  if (!(hl > 0.0)) {  // a landmark with factors but no information: H is singular
+    if (lane == 0) { v.var[l] = 0.0; v.scal->chol_fail = 1; }
+    return;
+  }
+  const int lo = v.lm.lo[l], n = v.lm.hi[l] - lo, ld = v.idx_ld;
+  const double* Wl = v.ne.W + v.lm.woff[l];
+  const double wld = v.ne.wld[l];
+  double acc = 0.0;
+#pragma unroll 1
+  for (int a = 0; a <= n; ++a) {
+    const int ga = a < n ? lo + a : ld;
+    const double wa = a < n ? Wl[a] : wld;
+    const double* row = v.cov + size_t(ga) * v.np;
+    double s = 0.0;
+    for (int b = lane; b <= n; b += 32) s = fma(row[b < n ? lo + b : ld], b < n ? Wl[b] : wld, s);
+    acc = fma(wa, s, acc);
+  }
+  acc = warp_sum_d(acc);
+  if (lane == 0) v.var[l] = 1.0 / hl + acc / (hl * hl);
+}
+
+// one warp: the extreme pivots over the blocks, rcond, and the scalar block with rcond to mapped host memory
+__global__ void cov_publish_kernel(const double* __restrict__ piv, int nb, const LmScalars* scal, LmPublished* pub,
+                                   unsigned long long seq) {
+  const int lane = threadIdx.x;
+  double mn = INFINITY, mx = 0.0;
+  for (int b = lane; b < nb; b += 32) { mn = fmin(mn, piv[2 * b]); mx = fmax(mx, piv[2 * b + 1]); }
+  mn = warp_min_d(mn);
+  mx = warp_max_d(mx);
+  if (lane != 0) return;
+  // X_ii = 1 / L_ii: min L / max L = min X / max X.  No free dim at all: nothing can be singular
+  const double ratio = mx > 0.0 ? mn / mx : 1.0;
+  __threadfence();
+  pub->s = *scal;
+  pub->rcond = ratio * ratio;
+  __threadfence_system();
+  *reinterpret_cast<volatile unsigned long long*>(&pub->seq) = seq;
+}
+
+int launch_cov_mask(const uint8_t* active, int np, uint8_t* cmask, cudaStream_t s) {
+  cov_mask_kernel<<<(np + 255) / 256, 256, 0, s>>>(active, np, cmask);
+  return 1;
+}
+
+int launch_cov_inverse(const CovLaunch& c, cudaStream_t s) {
+  static PerDeviceOnce once;
+  if (once.first()) {
+    cudaFuncSetAttribute(cov_diag_inverse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kCovDiagSmem));
+    cudaFuncSetAttribute(cov_column_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kCovTileSmem));
+    cudaFuncSetAttribute(cov_sigma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kCovTileSmem));
+  }
+  const int nb = c.npad / kCholNB;
+  cov_diag_inverse_kernel<<<nb, 256, kCovDiagSmem, s>>>(c);
+  int n = 1;
+  if (nb > 1) {
+    cov_column_kernel<<<nb - 1, 256, kCovTileSmem, s>>>(c);
+    ++n;
+  }
+  cov_sigma_kernel<<<nb * (nb + 1) / 2, 256, kCovTileSmem, s>>>(c);
+  return n + 1;
+}
+
+int launch_landmark_variance(const LandmarkVarLaunch& v, cudaStream_t s) {
+  if (v.nL == 0) return 0;
+  landmark_variance_kernel<<<(v.nL + 7) / 8, 256, 0, s>>>(v);
+  return 1;
+}
+
+int launch_cov_publish(const double* piv, int nb, const LmScalars* scal, LmPublished* pub, unsigned long long seq,
+                       cudaStream_t s) {
+  cov_publish_kernel<<<1, 32, 0, s>>>(piv, nb, scal, pub, seq);
+  return 1;
+}
+
+}  // namespace ctvio
+
+extern "C" int ctvio_covariance(ctvio_handle e, double* cov_cc, double* var_rho, double* rcond) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_covariance: not available in sharded mode");
+  cudaSetDevice(e->cfg.device);
+  int rc = prepare(e);
+  if (rc) return rc;
+  cudaStream_t st = e->stream;
+  const ProblemDims d = e->dims();
+  const size_t np = size_t(d.np), nL = size_t(e->nL), npad = size_t(e->npad), nb = npad / kCholNB;
+  auto& w = e->cws;
+  CUDA_OK(w.sc.reserve(np));
+  CUDA_OK(w.sl.reserve(nL));
+  CUDA_OK(w.cmask.reserve(np));
+  CUDA_OK(w.X.reserve(npad * npad));
+  CUDA_OK(w.piv.reserve(2 * nb));
+  CUDA_OK(w.cov.reserve(np * np));
+  CUDA_OK(w.var.reserve(nL));
+  CUDA_OK(w.scal.reserve(1));
+  // the call leaves no trace in the LM driver's state: its scalar block is saved here and restored at the end, the
+  // normal equations go to the buffer the next solve clears before use, and the Jacobi scales / mask are this call's own
+  CUDA_OK(cudaMemcpyAsync(w.scal.p, e->d_scal.p, sizeof(LmScalars), cudaMemcpyDeviceToDevice, st));
+  ensure_table(e);
+  const int nbuf = e->cur ^ 1;
+  evaluate(e, e->cur, nbuf, true);
+  LinearLaunch lin = linear_launch(e, nbuf);
+  lin.sc = w.sc.p;
+  lin.sl = w.sl.p;
+  lin.cmask = w.cmask.p;
+  e->launches += launch_jacobi_scale(lin, st);
+  e->launches += launch_cov_mask(e->d_active.p, d.np, w.cmask.p, st);
+  if (e->deterministic) cudaMemsetAsync(e->d_ticket.p, 0, 2 * sizeof(int32_t), st);
+  // radius +inf: clamp(diag) / radius vanishes, and so does the landmark damping
+  e->launches += launch_reduced_system(lin, INFINITY, st);
+  bool tile_dag = false;
+  e->launches += launch_factor_solve(lin, st, &tile_dag);
+  CovLaunch c;
+  c.np = d.np; c.npad = int(npad); c.nL = e->nL; c.idx_ld = d.idx_ld;
+  c.M = lin.M;
+  c.Linv = e->d_Linv.p;
+  c.packets = tile_dag ? chol_dag_last_packets(e->d_Linv.p, int(npad), e->chol_seq) : nullptr;
+  c.tile_dag = tile_dag ? 1 : 0;
+  c.cmask = w.cmask.p;
+  c.sc = w.sc.p;
+  c.X = w.X.p; c.piv = w.piv.p; c.cov = w.cov.p;
+  e->launches += launch_cov_inverse(c, st);
+  LandmarkVarLaunch v;
+  v.np = d.np; v.nL = e->nL; v.idx_ld = d.idx_ld;
+  v.cov = w.cov.p;
+  v.ne = e->ne(nbuf);
+  v.lm = e->lml();
+  v.active = e->d_active.p;
+  v.var = w.var.p;
+  v.scal = e->d_scal.p;
+  e->launches += launch_landmark_variance(v, st);
+  e->launches += launch_cov_publish(w.piv.p, int(nb), e->d_scal.p, e->h_pub, ++e->pub_seq, st);
+  CUDA_OK(cudaMemcpyAsync(e->d_scal.p, w.scal.p, sizeof(LmScalars), cudaMemcpyDeviceToDevice, st));
+  rc = read_scalars(e, true);
+  const double rc_value = const_cast<const LmPublished*>(e->h_pub)->rcond;
+  const bool failed = e->h_scal->chol_fail != 0;
+  CUDA_OK(cudaStreamSynchronize(st));  // (the restore behind the published block)
+  if (rc) return rc;
+  if (rcond) *rcond = rc_value;
+  // Ceres' default min_reciprocal_condition_number; the estimate is the pivot ratio, see include/ctvio.h
+  if (failed || !(rc_value >= 1e-14)) {
+    char msg[96];
+    std::snprintf(msg, sizeof(msg), "ctvio_covariance: rank deficient (rcond %.3e%s)", rc_value,
+                  failed ? ", non-positive pivot" : "");
+    return fail(CTVIO_ERR_STATE, msg);
+  }
+  if (cov_cc) {
+    CUDA_OK(cudaMemcpyAsync(cov_cc, w.cov.p, np * np * sizeof(double), cudaMemcpyDeviceToHost, st));
+    e->d2h_bytes += np * np * sizeof(double);
+  }
+  if (var_rho && nL) {
+    CUDA_OK(cudaMemcpyAsync(var_rho, w.var.p, nL * sizeof(double), cudaMemcpyDeviceToHost, st));
+    e->d2h_bytes += nL * sizeof(double);
+  }
+  CUDA_OK(cudaStreamSynchronize(st));
+  return CTVIO_OK;
+}

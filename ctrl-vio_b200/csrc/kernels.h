@@ -150,7 +150,7 @@ struct LmPublished {
   LmScalars s;
   LmDecision dec;
   unsigned long long seq;
-  unsigned long long pad;
+  double rcond;  // written by ctvio_covariance only: pivot ratio of the factored reduced system
 };
 constexpr int kLmSumScalars = 6;  // cost_eval, gd, dHd, step_norm2, x_norm2, err_sum: plain sums over landmark shards
 
@@ -331,14 +331,47 @@ int launch_lm_step(const LinearLaunch& a, double radius, cudaStream_t s);
 // radius_dev != null: the radius is read from device memory (first double of an LmDecision)
 int launch_reduced_system(const LinearLaunch& a, double radius, cudaStream_t s, const double* radius_dev = nullptr);
 size_t reduced_system_flags_len(int npad);  // ints of LinearLaunch::m_flags
-int launch_factor_solve(const LinearLaunch& a, cudaStream_t s);
+// tile_dag (may be null): set to whether the tile-DAG kernel ran (else the barrier kernel) - the two leave the factor in
+// different layouts (CholDagArgs::M in chol_dag.cu, the header of chol_coop.cu)
+int launch_factor_solve(const LinearLaunch& a, cudaStream_t s, bool* tile_dag = nullptr);
 // tile-DAG variant (chol_dag.cu): usable when every tile gets its own SM
 bool chol_dag_supported(int npad, int n_sm);
 size_t chol_dag_part_len(int npad);
 size_t chol_dag_flags_len(int npad);
 size_t chol_dag_lpub_len(int npad);  // doubles of LinearLaunch::Linv: [block inverses of the barrier kernel | 2 packet buffers]
 int launch_chol_dag_init(double* linv_buf, double* part_buf, int npad, cudaStream_t s);  // message buffers <- sentinels, once per allocation
-int launch_chol_dag(const LinearLaunch& a, cudaStream_t s);
+int launch_chol_dag(const LinearLaunch& a, cudaStream_t s, bool* tile_dag = nullptr);
+// the packet buffer (packets [nb][4][16][80], layout in chol_tiles.cuh) of the last tile-DAG launch on this engine
+const double* chol_dag_last_packets(const double* linv_buf, int npad, unsigned chol_seq);
+
+// ---- marginal covariance (covariance.cu, ctvio_covariance) ----------------------------------------
+struct CovLaunch {
+  int32_t np, npad, nL, idx_ld;
+  const double* M;         // K5's factor: strictly-lower tiles of L (transposed inside the slot if tile_dag)
+  const double* Linv;      // barrier kernel: [nb][64][64] inverses of the diagonal blocks of L
+  const double* packets;   // tile-DAG kernel: the packets of its diagonal factorisations
+  int32_t tile_dag;
+  const uint8_t* cmask;    // [np] 1 = no covariance (held constant, or touched by no factor)
+  const double* sc;        // [np] Jacobi scale the reduced system was formed with
+  double* X;               // [npad][npad] L^-1, lower tiles
+  double* piv;             // [nb][2] min / max of 1 / L_ii over the block's free dims
+  double* cov;             // [np][np] camera-side covariance, both triangles
+};
+int launch_cov_mask(const uint8_t* active, int np, uint8_t* cmask, cudaStream_t s);  // cmask = !active over [0, np)
+int launch_cov_inverse(const CovLaunch& c, cudaStream_t s);  // X, piv, cov
+struct LandmarkVarLaunch {
+  int32_t np, nL, idx_ld;
+  const double* cov;
+  NormalEqPtrs ne;
+  LandmarkLayout lm;
+  const uint8_t* active;   // [np + nL]
+  double* var;             // [nL]
+  LmScalars* scal;         // chol_fail is set when a landmark with a factor has h_l <= 0
+};
+int launch_landmark_variance(const LandmarkVarLaunch& v, cudaStream_t s);
+// rcond = (min / max of the pivots)^2 from piv, then the scalar block + rcond to *pub with sequence number seq
+int launch_cov_publish(const double* piv, int nb, const LmScalars* scal, LmPublished* pub, unsigned long long seq,
+                       cudaStream_t s);
 int launch_chol_coop(const LinearLaunch& a, cudaStream_t s);
 int launch_step_vectors(const LinearLaunch& a, cudaStream_t s);
 // sharded mode: the iteration-0 Jacobi scale from the all-reduced camera diagonal (the LM damping and identity rows

@@ -257,6 +257,20 @@ class TrajectoryEstimator {
     return out;
   }
 
+  // what ceres::Covariance (trajectory_estimator.h:23) computes for the camera-side blocks and the inverse depths, at
+  // the current state (see ctvio_covariance): cov_cc [np][np] row-major in ctvio_normal_equations' column order,
+  // var_rho [n_landmarks]; either may be null.  Returns rcond; throws ctvio_host::Error on a rank-deficient window.
+  double GetCovariance(std::vector<double>* cov_cc, std::vector<double>* var_rho) {
+    upload();
+    const size_t np = 6 * (trajectory_->numKnots() + bias_nodes_.size()) + 1;
+    if (cov_cc) cov_cc->assign(np * np, 0.0);
+    if (var_rho) var_rho->assign(landmarks_.size(), 0.0);
+    double rcond = 0.0;
+    check(ctvio_covariance(h_, cov_cc ? cov_cc->data() : nullptr, var_rho ? var_rho->data() : nullptr, &rcond),
+          "ctvio_covariance");
+    return rcond;
+  }
+
   // TrajectoryManager::double2vector (trajectory_manager.cpp:485-516): R0 row-major, t0; knots >= min_idx
   void GaugeRealign(int min_idx, const double R0[9], const double t0[3]) {
     check(ctvio_gauge_realign(h_, min_idx, R0, t0), "ctvio_gauge_realign");

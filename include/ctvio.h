@@ -229,6 +229,30 @@ int ctvio_eval_cost(ctvio_handle h, double* cost);
 /* Schur-form normal equations at the current state: camera block H_cc (np x np, row-major, symmetric),
  * g_c (np), per-landmark h_l, g_l (n_landmarks each).  np = 6*n_knots + 6*n_bias + 1. */
 int ctvio_normal_equations(ctvio_handle h, double* Hcc, double* gc, double* hl, double* gl, double* cost);
+/* ctvio_covariance - marginal covariance of the window at the current state (ceres::Covariance with its defaults,
+ *   apply_loss_function = true, which trajectory_estimator.h:23 makes available to the reference's callers).
+ *   The matrix: H = J'J of the current factor set (image factors with the cauchy_solve loss applied as the solve
+ *   applies it, IMU, bias and the active prior), the Gauss-Newton matrix the solve builds, without damping and without
+ *   Jacobi scaling, in the tangent space of ctvio_normal_equations (3 columns per rotation).
+ *   cov_cc (np x np, row-major, may be NULL): the camera-side block of H^-1, columns ordered as ctvio_normal_equations'
+ *     H_cc, np = 6*n_knots + 6*n_bias + 1.  It is S^-1, S the landmark-reduced system (Schur-complement identity); the
+ *     full inverse is never formed.  Exactly symmetric.
+ *   var_rho (n_landmarks, may be NULL): the diagonal of H^-1 at the inverse depths, 1/h_l + v_l' S^-1 v_l with
+ *     v_l = W_l / h_l, W_l the landmark's coupling row (its knot / bias range and the line delay).
+ *   Dimensions the solve holds constant (knots <= fixed_knot_index, lock_traj, lock_wb, lock_ab, fix_ld) and dimensions
+ *   no factor touches have zero rows and columns; a landmark no factor touches has variance 0 (Ceres returns zero
+ *   covariance for constant blocks).
+ *   rcond (may be NULL) = (min_i L_ii / max_i L_ii)^2, L the Cholesky factor of the Jacobi-scaled S over its free
+ *   dimensions.  The call fails with CTVIO_ERR_STATE ("rank deficient") and writes nothing but rcond when the
+ *   factorisation meets a non-positive or non-finite pivot, when a landmark with factors has h_l <= 0, or when
+ *   rcond < 1e-14.  The threshold is Ceres' default min_reciprocal_condition_number, but the test is this pivot-ratio
+ *   estimate, not Ceres' own rank test.  A window without a prior or fixed knots is always rank deficient (yaw and
+ *   translation are unobservable).
+ *   No side effects: state, prior, factor set and the LM driver's scalars are unchanged; a solve after the call is
+ *   bitwise the solve without it in deterministic mode.  ctvio_transfer_stats counts the outputs copied (only those
+ *   requested).
+ *   Errors: CTVIO_ERR_STATE before the state is set and in sharded mode. */
+int ctvio_covariance(ctvio_handle h, double* cov_cc, double* var_rho, double* rcond);
 
 /* ---- spline query service (SURVEY §8f-2: Trajectory::poseNs / GetIMUState, spline/trajectory.cpp:27-55) ----
  * batch R(t), p(t), body angular velocity, world linear velocity and acceleration. Any output may be NULL. */
