@@ -100,7 +100,7 @@ ABI_SYMBOLS = [
     "solve", "gauge_realign", "marginalize", "get_prior", "adopt_prior",
     "save_state", "restore_state",
     "eval_image_factors", "eval_imu_factors", "residual_summary", "eval_cost", "normal_equations", "covariance",
-    "query_trajectory", "triangulate",
+    "pose_covariance", "query_trajectory", "triangulate",
     "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior", "ingest_feature_cloud", "add_image_features_from_slots",
     "ingest_imu", "add_imu_from_table", "transfer_stats", "profile_kernels", "measure_fp64_tflops", "measure_fp64_tensor_tflops",
     "selfcheck_solver", "nccl_unique_id", "comm_init", "triangulate_window", "check_keyframe", "slide_window_second_new",
@@ -111,14 +111,15 @@ ABI_SYMBOLS = [
 
 
 # entry points a checker library (the CPU oracle mirrors the ABI under `ctvo_`) need not provide: multi-GPU plumbing and
-# the device-residency / wire-format calls, which have no CPU meaning, and the covariance, which the tests form from the
+# the device-residency / wire-format calls, which have no CPU meaning, and the covariances, which the tests form from the
 # oracle's normal equations instead
 DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enable_prior", "extend_knots_to", "slide_window", "remap_landmarks",
                        "ingest_feature_cloud", "add_image_features_from_slots", "ingest_imu", "add_imu_from_table",
                        "transfer_stats", "residual_summary", "triangulate_window", "check_keyframe",
                        "slide_window_second_new", "feature_table_add", "feature_table_window", "triangulate_window_from_table",
                        "add_image_features_from_table", "feature_table_slide", "feature_table_landmarks",
-                       "feature_table_map", "feature_table_slide_reanchor", "debug_structure", "covariance")
+                       "feature_table_map", "feature_table_slide_reanchor", "debug_structure", "covariance",
+                       "pose_covariance")
 
 
 def _addr(a):
@@ -389,6 +390,17 @@ class Estimator:
         rcond = C.c_double()
         self.lib.call("covariance", self.h, _dp(cc), _dp(vr), C.byref(rcond))
         return cc, vr, rcond.value
+
+    def PoseCovariance(self, t, gauge_knot_index=-1, camera_frame=False):
+        """Covariance of (dtheta, dp, domega, dv) at the times t (ctvio_pose_covariance): (cov [n, 12, 12], rcond).
+        Knots <= gauge_knot_index are held constant for this call only; camera_frame=True gives the camera's pose and
+        velocity.  Raises CtvioError on a rank-deficient window, with rcond in the message."""
+        t = _i64(np.atleast_1d(t)); n = t.shape[0]
+        cov = np.zeros((n, 12, 12))
+        rcond = C.c_double()
+        self.lib.call("pose_covariance", self.h, C.c_int32(n), _lp(t), C.c_int32(int(gauge_knot_index)),
+                      C.c_int32(int(bool(camera_frame))), _dp(cov), C.byref(rcond))
+        return cov, rcond.value
 
     def QueryTrajectory(self, t):
         t = _i64(t); n = t.shape[0]

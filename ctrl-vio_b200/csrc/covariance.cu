@@ -11,6 +11,9 @@
 //
 // Every product of 64x64 tiles runs on the fp64 tensor path (mma.sync.m8n8k4.f64, full-tile instantiations only: no
 // DMMA under a run-time predicate, DESIGN §4).  No atomics: the result is bitwise reproducible for a given H.
+//
+// ctvio_pose_covariance forms the same Sigma (with an optional gauge of its own in the mask) and projects it to the
+// pose and velocity at each query time on the device (pose_cov_kernel, 12 x 24 Jacobians, plain fp64 fma chains).
 #include <cmath>
 #include <cstdio>
 
@@ -67,9 +70,9 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 
 }  // namespace
 
-__global__ void cov_mask_kernel(const uint8_t* __restrict__ active, int np, uint8_t* __restrict__ cmask) {
+__global__ void cov_mask_kernel(const uint8_t* __restrict__ active, int np, int n_gauge, uint8_t* __restrict__ cmask) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < np) cmask[i] = active[i] ? 0 : 1;
+  if (i < np) cmask[i] = (active[i] && i >= n_gauge) ? 0 : 1;
 }
 
 // CTA k: X(k,k) = L(k,k)^-1 (upper triangle zero) and the extreme pivots of block k.  The barrier kernel keeps the
@@ -234,8 +237,8 @@ __global__ void cov_publish_kernel(const double* __restrict__ piv, int nb, const
   *reinterpret_cast<volatile unsigned long long*>(&pub->seq) = seq;
 }
 
-int launch_cov_mask(const uint8_t* active, int np, uint8_t* cmask, cudaStream_t s) {
-  cov_mask_kernel<<<(np + 255) / 256, 256, 0, s>>>(active, np, cmask);
+int launch_cov_mask(const uint8_t* active, int np, int n_gauge, uint8_t* cmask, cudaStream_t s) {
+  cov_mask_kernel<<<(np + 255) / 256, 256, 0, s>>>(active, np, n_gauge, cmask);
   return 1;
 }
 
@@ -269,12 +272,69 @@ int launch_cov_publish(const double* piv, int nb, const LmScalars* scal, LmPubli
   return 1;
 }
 
+// One warp per query time: C = (J Sigma_sub) J' with J = J(t) (12 x 24, PoseJacobian) and Sigma_sub the 24 x 24 block of
+// the window covariance at the dims of knots s..s+3, which are contiguous (6s .. 6s + 23).  Every lane evaluates the
+// spline (the same values in all lanes) and lanes 0..23 write one column of J each; the products are fixed-order fma
+// chains, one output entry per lane, no atomics.  The lower triangle is formed and mirrored: exactly symmetric.
+constexpr int kPoseCovWarps = 4;
+__global__ void __launch_bounds__(32 * kPoseCovWarps) pose_cov_kernel(PoseCovLaunch a) {
+  __shared__ double sJ[kPoseCovWarps][12 * 24], sS[kPoseCovWarps][24 * 24], sT[kPoseCovWarps][12 * 24];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int n = blockIdx.x * kPoseCovWarps + w;
+  if (n >= a.n) return;
+  double* J = sJ[w];
+  double* S = sS[w];
+  double* T = sT[w];
+  int32_t s;
+  double u;
+  spline_index(a.sp, a.t[n], s, u);
+  const double* src = a.cov + size_t(6 * s) * a.np + 6 * s;
+  for (int e = lane; e < 24 * 24; e += 32) S[e] = src[size_t(e / 24) * a.np + e % 24];
+  PoseJacobian pj;
+  pose_jacobian<kPStride>(a.sp, a.st.q, a.st.p, a.st.tab, s, u, pj);
+  if (lane < 24) {
+    double col[12];
+    pose_jacobian_column(pj, a.camera_frame != 0, a.R_CI, a.p_CI, lane, col);
+#pragma unroll
+    for (int i = 0; i < 12; ++i) J[i * 24 + lane] = col[i];
+  }
+  __syncwarp();
+  for (int e = lane; e < 12 * 24; e += 32) {  // T = J Sigma_sub
+    const int i = e / 24, b = e % 24;
+    double acc = 0.0;
+#pragma unroll 8
+    for (int k = 0; k < 24; ++k) acc = fma(J[i * 24 + k], S[k * 24 + b], acc);
+    T[e] = acc;
+  }
+  __syncwarp();
+  double* out = a.out + size_t(n) * 144;
+  for (int e = lane; e < 78; e += 32) {  // C[i][j] = T[i] . J[j], i >= j
+    int i = 0;
+    while ((i + 1) * (i + 2) / 2 <= e) ++i;
+    const int j = e - i * (i + 1) / 2;
+    double acc = 0.0;
+#pragma unroll 8
+    for (int k = 0; k < 24; ++k) acc = fma(T[i * 24 + k], J[j * 24 + k], acc);
+    out[i * 12 + j] = acc;
+    out[j * 12 + i] = acc;
+  }
+}
+
+int launch_pose_cov(const PoseCovLaunch& a, cudaStream_t s) {
+  if (a.n <= 0) return 0;
+  pose_cov_kernel<<<(a.n + kPoseCovWarps - 1) / kPoseCovWarps, 32 * kPoseCovWarps, 0, s>>>(a);
+  return 1;
+}
+
 }  // namespace ctvio
 
-extern "C" int ctvio_covariance(ctvio_handle e, double* cov_cc, double* var_rho, double* rcond) {
-  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
-  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_covariance: not available in sharded mode");
-  cudaSetDevice(e->cfg.device);
+namespace {
+
+// Sigma of the window at the current state into cws.cov and the inverse-depth variances into cws.var, with the knots
+// <= gauge_knot held constant on top of what the options hold constant (-1: the options alone).  Returns CTVIO_OK, an
+// error of the evaluation, or CTVIO_ERR_STATE "<who>: rank deficient"; *rcond (may be null) is written in these last two
+// cases only.  Ends with the stream synchronised.
+int form_covariance(ctvio_engine* e, int gauge_knot, const char* who, double* rcond) {
   int rc = prepare(e);
   if (rc) return rc;
   cudaStream_t st = e->stream;
@@ -300,7 +360,7 @@ extern "C" int ctvio_covariance(ctvio_handle e, double* cov_cc, double* var_rho,
   lin.sl = w.sl.p;
   lin.cmask = w.cmask.p;
   e->launches += launch_jacobi_scale(lin, st);
-  e->launches += launch_cov_mask(e->d_active.p, d.np, w.cmask.p, st);
+  e->launches += launch_cov_mask(e->d_active.p, d.np, 6 * (gauge_knot + 1), w.cmask.p, st);
   if (e->deterministic) cudaMemsetAsync(e->d_ticket.p, 0, 2 * sizeof(int32_t), st);
   // radius +inf: clamp(diag) / radius vanishes, and so does the landmark damping
   e->launches += launch_reduced_system(lin, INFINITY, st);
@@ -335,11 +395,25 @@ extern "C" int ctvio_covariance(ctvio_handle e, double* cov_cc, double* var_rho,
   if (rcond) *rcond = rc_value;
   // Ceres' default min_reciprocal_condition_number; the estimate is the pivot ratio, see include/ctvio.h
   if (failed || !(rc_value >= 1e-14)) {
-    char msg[96];
-    std::snprintf(msg, sizeof(msg), "ctvio_covariance: rank deficient (rcond %.3e%s)", rc_value,
+    char msg[128];
+    std::snprintf(msg, sizeof(msg), "%s: rank deficient (rcond %.3e%s)", who, rc_value,
                   failed ? ", non-positive pivot" : "");
     return fail(CTVIO_ERR_STATE, msg);
   }
+  return CTVIO_OK;
+}
+
+}  // namespace
+
+extern "C" int ctvio_covariance(ctvio_handle e, double* cov_cc, double* var_rho, double* rcond) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_covariance: not available in sharded mode");
+  cudaSetDevice(e->cfg.device);
+  int rc = form_covariance(e, -1, "ctvio_covariance", rcond);
+  if (rc) return rc;
+  cudaStream_t st = e->stream;
+  const size_t np = size_t(e->dims().np), nL = size_t(e->nL);
+  auto& w = e->cws;
   if (cov_cc) {
     CUDA_OK(cudaMemcpyAsync(cov_cc, w.cov.p, np * np * sizeof(double), cudaMemcpyDeviceToHost, st));
     e->d2h_bytes += np * np * sizeof(double);
@@ -348,6 +422,46 @@ extern "C" int ctvio_covariance(ctvio_handle e, double* cov_cc, double* var_rho,
     CUDA_OK(cudaMemcpyAsync(var_rho, w.var.p, nL * sizeof(double), cudaMemcpyDeviceToHost, st));
     e->d2h_bytes += nL * sizeof(double);
   }
+  CUDA_OK(cudaStreamSynchronize(st));
+  return CTVIO_OK;
+}
+
+extern "C" int ctvio_pose_covariance(ctvio_handle e, int32_t n, const int64_t* t_ns, int32_t gauge_knot_index,
+                                     int32_t camera_frame, double* cov12, double* rcond) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (n < 0 || (n > 0 && (!t_ns || !cov12))) return fail(CTVIO_ERR_INVALID, "ctvio_pose_covariance: bad argument");
+  if (camera_frame != 0 && camera_frame != 1) return fail(CTVIO_ERR_INVALID, "ctvio_pose_covariance: camera_frame must be 0 or 1");
+  if (gauge_knot_index < -1 || gauge_knot_index >= e->nK)
+    return fail(CTVIO_ERR_INVALID, "ctvio_pose_covariance: gauge_knot_index outside -1 .. n_knots - 1");
+  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_pose_covariance: not available in sharded mode");
+  if (n == 0) return CTVIO_OK;
+  if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
+  for (int32_t i = 0; i < n; ++i) {  // the range ctvio_query_trajectory accepts
+    int32_t s;
+    double u;
+    if (!spline_index(e->sp, t_ns[i], s, u)) return fail(CTVIO_ERR_TIME_RANGE, "ctvio_pose_covariance: a time outside the spline");
+  }
+  cudaSetDevice(e->cfg.device);
+  int rc = form_covariance(e, gauge_knot_index, "ctvio_pose_covariance", rcond);
+  if (rc) return rc;
+  cudaStream_t st = e->stream;
+  auto& w = e->cws;
+  CUDA_OK(w.t.reserve(size_t(n)));
+  CUDA_OK(w.pose.reserve(144 * size_t(n)));
+  CUDA_OK(cudaMemcpyAsync(w.t.p, t_ns, size_t(n) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  e->h2d_bytes += size_t(n) * sizeof(int64_t);
+  PoseCovLaunch a;
+  a.st = e->x[e->cur].ptrs();
+  a.sp = e->sp;
+  a.R_CI = e->rig.R_CI;
+  a.p_CI = e->rig.p_CI;
+  a.n = n; a.np = e->dims().np; a.camera_frame = camera_frame;
+  a.t = w.t.p;
+  a.cov = w.cov.p;
+  a.out = w.pose.p;
+  e->launches += launch_pose_cov(a, st);
+  CUDA_OK(cudaMemcpyAsync(cov12, w.pose.p, 144 * size_t(n) * sizeof(double), cudaMemcpyDeviceToHost, st));
+  e->d2h_bytes += 144 * size_t(n) * sizeof(double);
   CUDA_OK(cudaStreamSynchronize(st));
   return CTVIO_OK;
 }

@@ -357,7 +357,8 @@ struct CovLaunch {
   double* piv;             // [nb][2] min / max of 1 / L_ii over the block's free dims
   double* cov;             // [np][np] camera-side covariance, both triangles
 };
-int launch_cov_mask(const uint8_t* active, int np, uint8_t* cmask, cudaStream_t s);  // cmask = !active over [0, np)
+// cmask = !active over [0, np), and 1 on the first n_gauge dims (knots held constant for one call only)
+int launch_cov_mask(const uint8_t* active, int np, int n_gauge, uint8_t* cmask, cudaStream_t s);
 int launch_cov_inverse(const CovLaunch& c, cudaStream_t s);  // X, piv, cov
 struct LandmarkVarLaunch {
   int32_t np, nL, idx_ld;
@@ -372,6 +373,18 @@ int launch_landmark_variance(const LandmarkVarLaunch& v, cudaStream_t s);
 // rcond = (min / max of the pivots)^2 from piv, then the scalar block + rcond to *pub with sequence number seq
 int launch_cov_publish(const double* piv, int nb, const LmScalars* scal, LmPublished* pub, unsigned long long seq,
                        cudaStream_t s);
+// ctvio_pose_covariance: one warp per time, out[n][12][12] = J(t) Sigma_sub J(t)' (PoseJacobian, spline_eval.cuh)
+struct PoseCovLaunch {
+  StatePtrs st;
+  SplineParams sp;
+  M3 R_CI;
+  V3 p_CI;
+  int32_t n, np, camera_frame;
+  const int64_t* t;        // [n], inside the spline (checked by the caller)
+  const double* cov;       // [np][np] the window covariance
+  double* out;             // [n][144]
+};
+int launch_pose_cov(const PoseCovLaunch& a, cudaStream_t s);
 int launch_chol_coop(const LinearLaunch& a, cudaStream_t s);
 int launch_step_vectors(const LinearLaunch& a, cudaStream_t s);
 // sharded mode: the iteration-0 Jacobi scale from the all-reduced camera diagonal (the LM damping and identity rows

@@ -549,4 +549,94 @@ CTVIO_HD void eval_imu(const SplineParams& sp, const RigParams& rig, const doubl
   imu_jacobian_half<true, 1>(rig, tab, s, st, put(9));
 }
 
+// ------------------------------- pose covariance ------------------------------------------------
+// d omega(t) / d delta_{s+k} (right tangent) of the body angular velocity eval_side returns: VelocityBody with its
+// Jacobian (so3_spline_view.h:401-426).  These are the gyro rows of imu_jacobian_half<false, H> before imu_info:
+// X_I = lam_{I+1} P_I hat(om_I) Jr(-lam_{I+1} d_I) + dl_{I+1} P_{I+1} (P_0 = E_2 E_1 E_0, P_1 = E_2 E_1, P_2 = E_2,
+// P_3 = I, om_I the partial sums of the omega recursion), block k = X_{k-1} JrInv_{k-1} - X_k JrInv_k^T.
+CTVIO_HD void omega_jacobian(const SplineParams& sp, const KnotPair* tab, int32_t s, double u, M3 Jw[4]) {
+  double lam[4], dl[4];
+  cum_coeffs(u, lam);
+  cum_dcoeffs(u, sp.inv_dt, dl);
+  V3 phi[3], om[4];
+  Q4 E[3];
+  om[0] = V3{0, 0, 0};
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    const KnotPair& kp = tab[s + j];
+    const V3 d = V3{kp.d[0], kp.d[1], kp.d[2]};
+    phi[j] = lam[j + 1] * d;
+    const double th = fabs(lam[j + 1]) * kp.theta;
+    E[j] = so3_exp_theta(neg(phi[j]), th * th, th);
+    om[j + 1] = so3_rotate(E[j], om[j]) + dl[j + 1] * d;
+  }
+  M3 P[4];
+  P[3] = m3_identity();
+  P[2] = so3_matrix(E[2]);
+  P[1] = so3_matrix(so3_mul(E[2], E[1]));
+  P[0] = so3_matrix(so3_mul(so3_mul(E[2], E[1]), E[0]));
+  M3 X[3];
+  X[0] = m3_scale(dl[1], P[1]);
+#pragma unroll
+  for (int I = 1; I < 3; ++I) {
+    const M3 t = m3_mul(m3_mul_hat(P[I], om[I]), right_jacobian(neg(phi[I])));
+#pragma unroll
+    for (int e = 0; e < 9; ++e) X[I].m[e] = lam[I + 1] * t.m[e] + dl[I + 1] * P[I + 1].m[e];
+  }
+  M3 JI[3];
+#pragma unroll
+  for (int j = 0; j < 3; ++j)
+#pragma unroll
+    for (int e = 0; e < 9; ++e) JI[j].m[e] = tab[s + j].jrinv[e];
+  Jw[0] = m3_scale(-1.0, m3_mul_bt(X[0], JI[0]));
+  Jw[1] = m3_sub(m3_mul(X[0], JI[0]), m3_mul_bt(X[1], JI[1]));
+  Jw[2] = m3_sub(m3_mul(X[1], JI[1]), m3_mul_bt(X[2], JI[2]));
+  Jw[3] = m3_mul(X[2], JI[2]);
+}
+
+// The 12 x 24 Jacobian of the pose and velocity at one time, J(t) = d (dtheta, dp, domega, dv) / d (delta_k, dP_k),
+// k = 0..3 over the knots s..s+3 (column 6k + r: r < 3 the rotation of knot k, r >= 3 its position, the order of the
+// window's tangent space).  dtheta is the right perturbation R(t) -> R(t) Exp(dtheta), dp, dv are world-frame, domega
+// is body-frame.
+struct PoseJacobian {
+  SideEval ev;    // R, p, J[k] (dtheta rows), c[k] (dp rows), omega, vel
+  M3 Jw[4];       // domega rows
+  double c1[4];   // dv rows: first-derivative weights
+};
+
+template <int PS>
+CTVIO_HD void pose_jacobian(const SplineParams& sp, const double* q, const double* p, const KnotPair* tab, int32_t s,
+                            double u, PoseJacobian& o) {
+  eval_side<true, PS>(sp, q, p, tab, s, u, o.ev);
+  omega_jacobian(sp, tab, s, u, o.Jw);
+  plain_coeffs<1>(u, sp.inv_dt, o.c1);
+}
+
+// Column col (0..23) of J(t).  camera = true: of the camera pose R_c = R R_CI, p_c = p + R p_CI instead, with
+//   dtheta_c = R_CI' dtheta, dp_c = dp - R [p_CI]x dtheta, domega_c = R_CI' domega,
+//   dv_c = dv - R [omega x p_CI]x dtheta - R [p_CI]x domega.
+CTVIO_HD void pose_jacobian_column(const PoseJacobian& J, bool camera, const M3& R_CI, V3 p_CI, int col, double out[12]) {
+  const int k = col / 6, r = col % 6;
+  V3 th{0, 0, 0}, dp{0, 0, 0}, dw{0, 0, 0}, dv{0, 0, 0};
+  if (r < 3) {
+    th = V3{J.ev.J[k].m[r], J.ev.J[k].m[3 + r], J.ev.J[k].m[6 + r]};
+    dw = V3{J.Jw[k].m[r], J.Jw[k].m[3 + r], J.Jw[k].m[6 + r]};
+  } else {
+    const V3 e = V3{r == 3 ? 1.0 : 0.0, r == 4 ? 1.0 : 0.0, r == 5 ? 1.0 : 0.0};
+    dp = J.ev.c[k] * e;
+    dv = J.c1[k] * e;
+  }
+  if (camera) {
+    const V3 Rth = m3_vec(J.ev.R, th), Rdw = m3_vec(J.ev.R, dw);
+    dp = dp + cross(Rth, m3_vec(J.ev.R, p_CI));                                   // -R [p_CI]x th = R (th x p_CI)
+    dv = dv + cross(Rth, m3_vec(J.ev.R, cross(J.ev.omega, p_CI))) + cross(Rdw, m3_vec(J.ev.R, p_CI));
+    th = m3_tvec(R_CI, th);
+    dw = m3_tvec(R_CI, dw);
+  }
+  out[0] = th.x; out[1] = th.y; out[2] = th.z;
+  out[3] = dp.x; out[4] = dp.y; out[5] = dp.z;
+  out[6] = dw.x; out[7] = dw.y; out[8] = dw.z;
+  out[9] = dv.x; out[10] = dv.y; out[11] = dv.z;
+}
+
 }  // namespace ctvio

@@ -271,6 +271,18 @@ class TrajectoryEstimator {
     return rcond;
   }
 
+  // the covariance of the pose and velocity at n times t (ns), from the window covariance (see ctvio_pose_covariance):
+  // cov12 [n][12][12] row-major over (dtheta, dp, domega, dv), of the body or (camera_frame) of the camera.  Knots
+  // <= gauge_knot_index are held constant for this call only (-1: the options alone).  Returns rcond; throws
+  // ctvio_host::Error on a rank-deficient window.
+  double GetPoseCovariance(int n, const int64_t* t, int gauge_knot_index, bool camera_frame, double* cov12) {
+    upload();
+    double rcond = 0.0;
+    check(ctvio_pose_covariance(h_, n, t, gauge_knot_index, camera_frame ? 1 : 0, cov12, &rcond),
+          "ctvio_pose_covariance");
+    return rcond;
+  }
+
   // TrajectoryManager::double2vector (trajectory_manager.cpp:485-516): R0 row-major, t0; knots >= min_idx
   void GaugeRealign(int min_idx, const double R0[9], const double t0[3]) {
     check(ctvio_gauge_realign(h_, min_idx, R0, t0), "ctvio_gauge_realign");

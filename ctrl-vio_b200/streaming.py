@@ -23,7 +23,7 @@ import time
 import numpy as np
 
 from . import synthetic as syn
-from .binding import BLK_BA, BLK_BG, BLK_LD, BLK_POS, BLK_RHO, BLK_ROT, Estimator, PriorData
+from .binding import BLK_BA, BLK_BG, BLK_LD, BLK_POS, BLK_RHO, BLK_ROT, CtvioError, Estimator, PriorData
 
 KF_DT_NS = 50_000_000       # 20 Hz keyframes
 WINDOW_SIZE = 10            # visual_odometry/parameters.h:8
@@ -654,9 +654,20 @@ class ResidentRunner(StreamingRunner):
     anchored in the leaving frame are re-anchored instead of dropped; the record gains n_reanchored.  On C5 the solve
     diverges in window 8: as in the reference, every MARGIN_OLD marginalizes all factors of the landmarks anchored in the
     oldest frame, so a re-anchored landmark's observations enter the prior again at every slide (DESIGN §6).
-    Default (False): FeatureTableSlide after the window's slide, as before."""
+    Default (False): FeatureTableSlide after the window's slide, as before.
 
-    def __init__(self, lib, seq, triangulate=False, device_features=False, publish_map=False, reanchor=False, **kw):
+    publish_covariance=True: right after GaugeRealign and before the marginalization, inside the timed region, the
+    covariance of the camera pose and velocity the reference publishes as its TF (odometry_manager.cpp:287-288, at
+    maxTimeNs() - 50 ms) comes from the device (PoseCovariance with camera_frame=True).  The main solve fixes no knots,
+    so the call holds knots 0..3 (the window's first segment) constant as its own gauge.  The 12 x 12 matrix is kept on
+    last_pose_cov and the record gains pose_cov_rcond and ms_pose_cov; a window the call finds rank deficient records
+    pose_cov_rcond = nan, its message as pose_cov_error, and keeps last_pose_cov = None."""
+
+    POSE_COV_LAG_NS = 50_000_000
+    POSE_COV_GAUGE_KNOT = 3
+
+    def __init__(self, lib, seq, triangulate=False, device_features=False, publish_map=False, reanchor=False,
+                 publish_covariance=False, **kw):
         if device_features and not triangulate:
             raise ValueError("device_features requires triangulate=True: new landmarks enter with inverse depth -1")
         if publish_map and not device_features:
@@ -668,7 +679,9 @@ class ResidentRunner(StreamingRunner):
         self.device_features = device_features
         self.publish_map = publish_map
         self.reanchor = reanchor
+        self.publish_covariance = publish_covariance
         self.last_map = None
+        self.last_pose_cov = None
         self.triangulate_probe = None
         if self.clouds is None:
             self.clouds = FrameClouds(seq)
@@ -835,6 +848,17 @@ class ResidentRunner(StreamingRunner):
         summ = e.Solve(self.iters)
         t_solved = time.perf_counter()
         e.GaugeRealign(nowk, R0, t0_)
+        pose_cov = None
+        if self.publish_covariance:                    # the covariance of the published camera pose, before the slide
+            t_cov = time.perf_counter()
+            try:
+                self.last_pose_cov, rc = e.PoseCovariance([max_t - self.POSE_COV_LAG_NS],
+                                                          gauge_knot_index=self.POSE_COV_GAUGE_KNOT, camera_frame=True)
+                pose_cov = dict(pose_cov_rcond=rc)
+            except CtvioError as err:
+                self.last_pose_cov = None
+                pose_cov = dict(pose_cov_rcond=float("nan"), pose_cov_error=str(err))
+            pose_cov["ms_pose_cov"] = 1e3 * (time.perf_counter() - t_cov)
         if marg:
             n_out = C_int32(); nb_out = C_int32()
             e.lib.call("marginalize", e.h, byref(n_out), byref(nb_out))
@@ -877,6 +901,8 @@ class ResidentRunner(StreamingRunner):
                    h2d_bytes=h2d, d2h_bytes=d2h)
         if decision is not None:
             rec.update(decision)
+        if pose_cov is not None:
+            rec.update(pose_cov)
         if self.device_features:
             # n_new_lm: the window's landmarks without a depth yet (-1), which are exactly the ones TriangulateWindow wrote
             rec.update(n_triangulated=n_tri, n_fallback=n_fb, n_new_lm=n_tri + n_fb, n_removed=n_removed)

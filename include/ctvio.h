@@ -253,6 +253,29 @@ int ctvio_normal_equations(ctvio_handle h, double* Hcc, double* gc, double* hl, 
  *   requested).
  *   Errors: CTVIO_ERR_STATE before the state is set and in sharded mode. */
 int ctvio_covariance(ctvio_handle h, double* cov_cc, double* var_rho, double* rcond);
+/* ctvio_pose_covariance - covariance of the pose and velocity at n times, from the window covariance of
+ *   ctvio_covariance (same H, same rcond test and failure mode, same absence of side effects); the np x np matrix
+ *   stays on the device.
+ *   cov12[n][12][12] (row-major, exactly symmetric): the covariance of what ctvio_query_trajectory returns, in its
+ *     order: dtheta (3, R(t) -> R(t) Exp(dtheta), the right / body perturbation of the knots), dp (3, world position),
+ *     domega (3, body angular velocity), dv (3, world linear velocity).  It is J(t) Sigma_sub J(t)', Sigma_sub the
+ *     24 x 24 block of the window covariance at the rotation and position dims of the four knots of t's segment, J(t)
+ *     the spline's Jacobian with respect to them.
+ *   camera_frame = 1: of the camera instead, R_c = R R_CI, p_c = p + R p_CI (the convention of
+ *     ctvio_feature_table_map): dtheta_c = R_CI' dtheta, dp_c = dp - R [p_CI]x dtheta, domega_c = R_CI' domega,
+ *     dv_c = dv - R [omega x p_CI]x dtheta - R [p_CI]x domega.
+ *   gauge_knot_index: knots with index <= gauge_knot_index are held constant for this call only, on top of what the
+ *     options hold constant (SetFixedIndex applied to the covariance problem alone); -1: the options alone.  A window
+ *     whose solve fixes no knots (fixed_knot_index = -1) is rank deficient without it.
+ *   A time whose four knots are all constant gets an exact zero matrix.
+ *   rcond (may be NULL): as ctvio_covariance; on CTVIO_ERR_STATE "rank deficient" only rcond is written.
+ *   Errors, checked before anything is launched, with nothing written: CTVIO_ERR_INVALID for a null handle, n < 0,
+ *   a NULL t_ns or cov12 with n > 0, camera_frame not 0 or 1, gauge_knot_index outside -1 .. n_knots - 1;
+ *   CTVIO_ERR_STATE in sharded mode or before the knots are set; CTVIO_ERR_TIME_RANGE for a time
+ *   ctvio_query_trajectory does not accept.  n = 0 returns CTVIO_OK and launches nothing.
+ *   ctvio_transfer_stats counts 8 n bytes up and 1152 n bytes down. */
+int ctvio_pose_covariance(ctvio_handle h, int32_t n, const int64_t* t_ns, int32_t gauge_knot_index,
+                          int32_t camera_frame, double* cov12, double* rcond);
 
 /* ---- spline query service (SURVEY §8f-2: Trajectory::poseNs / GetIMUState, spline/trajectory.cpp:27-55) ----
  * batch R(t), p(t), body angular velocity, world linear velocity and acceleration. Any output may be NULL. */
