@@ -578,18 +578,20 @@ class Estimator:
 
     def DebugStructure(self):
         """the structure the engine built for the current factor set (ctvio_debug_structure), as int64 arrays: desc
-        (n_desc x 4), orig, items (x 4), lo, hi, woff, schur_items (x 4), entries (x 5), active, and after a
-        marginalization that built its blocks pos_cam, pos_lm, marg_img (else None)."""
+        (n_desc x 4), orig, items (x 4), lo, hi, woff, schur_items (x 4), entries (x 5), active, after a
+        marginalization that built its blocks pos_cam, pos_lm, marg_img (else None), and imu_items (x 4: start, count,
+        start knot, bias node)."""
         n = C.c_int64(0)
         self.lib.call("debug_structure", self.h, None, C.byref(n))
         out = np.zeros(n.value, np.int64)
         self.lib.call("debug_structure", self.h, _lp(out), C.byref(n))
         hdr = out[:16]
-        n_f, n_desc, n_items, nL, n_si, n_e, np_, n_marg = (int(x) for x in hdr[:8])
+        n_f, n_desc, n_items, nL, n_si, n_e, np_, n_marg, n_imu = (int(x) for x in hdr[:9])
         parts = [("desc", (n_desc, 4)), ("orig", (n_f,)), ("items", (n_items, 4)), ("lo", (nL,)), ("hi", (nL,)),
                  ("woff", (nL + 1,)), ("schur_items", (n_si, 4)), ("entries", (n_e, 5)), ("active", (np_ + nL,))]
         if n_marg >= 0:
             parts += [("pos_cam", (np_,)), ("pos_lm", (nL,)), ("marg_img", (n_marg,))]
+        parts += [("imu_items", (n_imu, 4))]
         res, o = {"pos_cam": None, "pos_lm": None, "marg_img": None}, 16
         for name, shape in parts:
             k = int(np.prod(shape))

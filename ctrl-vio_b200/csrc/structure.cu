@@ -561,7 +561,8 @@ extern "C" int ctvio_debug_structure(ctvio_handle e, int64_t* out, int64_t* len)
   const size_t ni = size_t(e->n_items), nsi = size_t(e->n_schur_items), ne = size_t(e->n_schur_entries);
   const size_t nm = e->n_marg_img >= 0 ? size_t(e->n_marg_img) : 0;
   const size_t marg_len = e->n_marg_img >= 0 ? np + nL + nm : 0;
-  const size_t need = 16 + 4 * n_desc + n + 4 * ni + 3 * nL + 1 + 4 * nsi + 5 * ne + np + nL + marg_len;
+  const size_t nii = size_t(e->n_imu_items);
+  const size_t need = 16 + 4 * n_desc + n + 4 * ni + 3 * nL + 1 + 4 * nsi + 5 * ne + np + nL + marg_len + 4 * nii;
   const int64_t cap = *len;
   *len = int64_t(need);
   if (!out) return CTVIO_OK;
@@ -574,6 +575,7 @@ extern "C" int ctvio_debug_structure(ctvio_handle e, int64_t* out, int64_t* len)
   std::vector<SchurTileItem> sitems(nsi);
   std::vector<SchurEntry> entries(ne);
   std::vector<uint8_t> active(np + nL);
+  std::vector<ImuItem> imu_items(nii);
   auto get = [&](auto& v, const void* src) {
     return v.empty() ? cudaSuccess : cudaMemcpyAsync(v.data(), src, v.size() * sizeof(v[0]), cudaMemcpyDeviceToHost, st);
   };
@@ -581,10 +583,11 @@ extern "C" int ctvio_debug_structure(ctvio_handle e, int64_t* out, int64_t* len)
   CUDA_OK(get(lo, e->d_lo.p)); CUDA_OK(get(hi, e->d_hi.p)); CUDA_OK(get(woff, e->d_woff.p));
   CUDA_OK(get(sitems, e->d_schur_items.p)); CUDA_OK(get(entries, e->d_schur_list.p)); CUDA_OK(get(active, e->d_active.p));
   CUDA_OK(get(pos_cam, e->mws.pos_cam.p)); CUDA_OK(get(pos_lm, e->mws.pos_lm.p)); CUDA_OK(get(marg, e->mws.marg_img.p));
+  CUDA_OK(get(imu_items, e->d_imu_items.p));
   CUDA_OK(cudaStreamSynchronize(st));
   std::memset(out, 0, 16 * sizeof(int64_t));
   out[0] = int64_t(n); out[1] = int64_t(n_desc); out[2] = int64_t(ni); out[3] = int64_t(nL); out[4] = int64_t(nsi);
-  out[5] = int64_t(ne); out[6] = int64_t(np); out[7] = e->n_marg_img;
+  out[5] = int64_t(ne); out[6] = int64_t(np); out[7] = e->n_marg_img; out[8] = int64_t(nii);
   int64_t* o = out + 16;
   for (const auto& x : desc) { *o++ = x.slot_i; *o++ = x.slot_j; *o++ = x.lm; *o++ = x.marg; }
   for (int32_t x : orig) *o++ = x;
@@ -598,5 +601,6 @@ extern "C" int ctvio_debug_structure(ctvio_handle e, int64_t* out, int64_t* len)
   for (int32_t x : pos_cam) *o++ = x;
   for (int32_t x : pos_lm) *o++ = x;
   for (int32_t x : marg) *o++ = x;
+  for (const auto& x : imu_items) { *o++ = x.start; *o++ = x.count; *o++ = x.s; *o++ = x.node; }
   return CTVIO_OK;
 }

@@ -214,12 +214,13 @@ int ctvio_residual_summary(ctvio_handle h, int32_t* counts4, double* err_sum18, 
  * when the factor set changed.  out: int64 slab, *len: its capacity in int64 on entry, the length needed on return
  * (out == NULL: query only).  Layout:
  *   header[16]  n factors, n_desc (n, or 0 for factors with host payload), n_items, nL, n_schur_items, n_entries, np,
- *               n_marg (-1 before a ctvio_marginalize that built its blocks), 0...
+ *               n_marg (-1 before a ctvio_marginalize that built its blocks), n_imu_items, 0...
  *   desc[n_desc][4] (slot_i, slot_j, landmark, marg; sorted) | orig[n] (sorted position -> caller index)
  *   | K1 items[n_items][4] (start, count, wi0, wj0) | lo[nL] | hi[nL] | woff[nL + 1]
  *   | K4 items[n_schur_items][4] (ti, tj, first, count) | entries[n_entries][5] (l, lo, hi, 0, woff)
  *   | active[np + nL]
  *   | pos_cam[np] | pos_lm[nL] | marg_img[n_marg]      -- only when n_marg >= 0
+ *   | K2 items[n_imu_items][4] (start, count, s, node): runs of IMU samples in sorted order
  * Traffic of the device-built structure (factors from ctvio_add_image_features_from_table): the add itself reads
  * nothing back; the build reads back one count block of 32 + 4 * ceil(n_knots / 32) bytes; ctvio_marginalize reads
  * back 8 + 4 * ceil(n_knots / 32) bytes for its image blocks.  This probe's own read-back is not counted. */
