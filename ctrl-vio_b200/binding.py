@@ -100,13 +100,13 @@ ABI_SYMBOLS = [
     "solve", "gauge_realign", "marginalize", "get_prior", "adopt_prior",
     "save_state", "restore_state",
     "eval_image_factors", "eval_imu_factors", "residual_summary", "eval_cost", "normal_equations", "covariance",
-    "pose_covariance", "query_trajectory", "triangulate",
+    "pose_covariance", "point_covariance", "query_trajectory", "triangulate",
     "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior", "ingest_feature_cloud", "add_image_features_from_slots",
     "ingest_imu", "add_imu_from_table", "transfer_stats", "profile_kernels", "measure_fp64_tflops", "measure_fp64_tensor_tflops",
     "selfcheck_solver", "nccl_unique_id", "comm_init", "triangulate_window", "check_keyframe", "slide_window_second_new",
     "feature_table_add", "feature_table_window", "triangulate_window_from_table", "add_image_features_from_table",
     "feature_table_slide", "feature_table_landmarks", "feature_table_map", "feature_table_slide_reanchor",
-    "debug_structure",
+    "debug_structure", "feature_table_point_covariance",
 ]
 
 
@@ -119,7 +119,7 @@ DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enab
                        "slide_window_second_new", "feature_table_add", "feature_table_window", "triangulate_window_from_table",
                        "add_image_features_from_table", "feature_table_slide", "feature_table_landmarks",
                        "feature_table_map", "feature_table_slide_reanchor", "debug_structure", "covariance",
-                       "pose_covariance")
+                       "pose_covariance", "point_covariance", "feature_table_point_covariance")
 
 
 def _addr(a):
@@ -402,6 +402,19 @@ class Estimator:
                       C.c_int32(int(bool(camera_frame))), _dp(cov), C.byref(rcond))
         return cov, rcond.value
 
+    def PointCovariance(self, landmark, t, bearing, gauge_knot_index=-1):
+        """Covariance of the world points of landmarks anchored at the times t with the bearings (x, y)
+        (ctvio_point_covariance): (cov [n, 3, 3], rcond).  Knots <= gauge_knot_index are held constant for this call
+        only.  Raises CtvioError on a rank-deficient window, with rcond in the message."""
+        lm = _i32(np.atleast_1d(landmark)); t = _i64(np.atleast_1d(t)); b = _f64(bearing, (-1, 2))
+        n = lm.shape[0]
+        assert t.shape[0] == n and b.shape[0] == n
+        cov = np.zeros((n, 3, 3))
+        rcond = C.c_double()
+        self.lib.call("point_covariance", self.h, C.c_int32(n), _ip(lm), _lp(t), _dp(b), C.c_int32(int(gauge_knot_index)),
+                      _dp(cov), C.byref(rcond))
+        return cov, rcond.value
+
     def QueryTrajectory(self, t):
         t = _i64(t); n = t.shape[0]
         q = np.zeros((n, 4)); p = np.zeros((n, 3)); w = np.zeros((n, 3)); v = np.zeros((n, 3)); a = np.zeros((n, 3))
@@ -535,6 +548,16 @@ class Estimator:
         ids, anchor, used = (np.zeros(max(n, 0), np.int32) for _ in range(3))
         self.lib.call("feature_table_landmarks", self.h, C.c_int32(n), _ip(ids), _ip(anchor), _ip(used))
         return ids, anchor, used
+
+    def FeatureTablePointCovariance(self, gauge_knot_index=-1):
+        """PointCovariance of every landmark of the last window, anchored as the feature table holds it
+        (ctvio_feature_table_point_covariance): (cov [n_lm, 3, 3], rcond) in the window's numbering."""
+        n = self.n_lm
+        cov = np.zeros((n, 3, 3))
+        rcond = C.c_double()
+        self.lib.call("feature_table_point_covariance", self.h, C.c_int32(n), C.c_int32(int(gauge_knot_index)), _dp(cov),
+                      C.byref(rcond))
+        return cov, rcond.value
 
     # capacity of FeatureTableMap's point arrays: every entry the table can hold (16 slots x 1024 features)
     MAP_CAPACITY = 16 * 1024

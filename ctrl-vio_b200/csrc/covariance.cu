@@ -14,6 +14,8 @@
 //
 // ctvio_pose_covariance forms the same Sigma (with an optional gauge of its own in the mask) and projects it to the
 // pose and velocity at each query time on the device (pose_cov_kernel, 12 x 24 Jacobians, plain fp64 fma chains).
+// ctvio_point_covariance and ctvio_feature_table_point_covariance project it, with the landmark-knot cross terms
+// -Sigma W_l' / h_l and the variance of rho_l, to anchored landmarks' world points (point_cov_kernel, 3 x 25 Jacobians).
 #include <cmath>
 #include <cstdio>
 
@@ -66,6 +68,15 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+
+// lane's part of sum_b row[col_b] w_b over a landmark's coupling row: its n knot dims lo .. lo + n - 1, then the line
+// delay (b = n).  Lane b takes b, b + 32, ... in order; the caller finishes with one fixed shuffle tree.
+__device__ __forceinline__ double coupling_dot_part(const double* row, int lo, int n, int ld, const double* Wl, double wld,
+                                                    int lane) {
+  double s = 0.0;
+  for (int b = lane; b <= n; b += 32) s = fma(row[b < n ? lo + b : ld], b < n ? Wl[b] : wld, s);
+  return s;
 }
 
 }  // namespace
@@ -210,10 +221,7 @@ __global__ void __launch_bounds__(256) landmark_variance_kernel(LandmarkVarLaunc
   for (int a = 0; a <= n; ++a) {
     const int ga = a < n ? lo + a : ld;
     const double wa = a < n ? Wl[a] : wld;
-    const double* row = v.cov + size_t(ga) * v.np;
-    double s = 0.0;
-    for (int b = lane; b <= n; b += 32) s = fma(row[b < n ? lo + b : ld], b < n ? Wl[b] : wld, s);
-    acc = fma(wa, s, acc);
+    acc = fma(wa, coupling_dot_part(v.cov + size_t(ga) * v.np, lo, n, ld, Wl, wld, lane), acc);
   }
   acc = warp_sum_d(acc);
   if (lane == 0) v.var[l] = 1.0 / hl + acc / (hl * hl);
@@ -326,6 +334,94 @@ int launch_pose_cov(const PoseCovLaunch& a, cudaStream_t s) {
   return 1;
 }
 
+// One warp per point: C = (G Sigma_25) G' with G = d P / d (knots s..s+3, rho_l) (3 x 25, point_jacobian_column) and
+// Sigma_25 the joint covariance of the segment's 24 knot dims (6s .. 6s + 23) and rho_l:
+//   [[Sigma_sub, c], [c', var_l]],  c = -(Sigma_{6s.., row} W_l') / h_l over the coupling row landmark_variance_kernel walks.
+// A landmark without factors has rho constant: c = 0 and var_l = 0.  An inverse depth that is not > 0 and finite leaves
+// the point undefined: NaN.  Fixed-order fma chains and shuffle trees, no atomics; the lower triangle is mirrored.
+constexpr int kPointCovWarps = 4;
+__global__ void __launch_bounds__(32 * kPointCovWarps) point_cov_kernel(PointCovLaunch a) {
+  __shared__ double sG[kPointCovWarps][3 * 25], sS[kPointCovWarps][25 * 25], sT[kPointCovWarps][3 * 25];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int n = blockIdx.x * kPointCovWarps + w;
+  if (n >= a.n) return;
+  double* G = sG[w];
+  double* S = sS[w];
+  double* T = sT[w];
+  int l;
+  int64_t t;
+  double x, y;
+  if (a.landmark) {
+    l = a.landmark[n];
+    t = a.t[n];
+    x = a.bearing[2 * n];
+    y = a.bearing[2 * n + 1];
+  } else {  // the anchor observation: the first entry of the landmark's CSR row
+    l = n;
+    const int o = a.obs_offset[l], slot = a.obs_slot[o];
+    const FrameFeature f = a.table[size_t(slot) * a.frame_cap + a.obs_idx[o]];
+    t = a.frame_t[slot];
+    x = f.x;
+    y = f.y;
+  }
+  double* out = a.out + size_t(n) * 9;
+  const double rho = a.st.rho[l];
+  if (!(rho > 0.0) || !isfinite(rho)) {
+    if (lane < 9) out[lane] = NAN;
+    return;
+  }
+  int32_t s;
+  double u;
+  spline_index(a.sp, t, s, u);
+  const double* src = a.cov + size_t(6 * s) * a.np + 6 * s;
+  for (int e = lane; e < 24 * 24; e += 32) S[(e / 24) * 25 + e % 24] = src[size_t(e / 24) * a.np + e % 24];
+  const double hl = a.ne.hl[l];
+  if (a.active[a.np + l] && hl > 0.0) {  // (h_l <= 0 with factors fails the covariance before this kernel runs)
+    const int lo = a.lm.lo[l], nw = a.lm.hi[l] - lo;
+    const double* Wl = a.ne.W + a.lm.woff[l];
+    const double wld = a.ne.wld[l];
+#pragma unroll 1
+    for (int r = 0; r < 24; ++r) {
+      const double c = warp_sum_d(coupling_dot_part(a.cov + size_t(6 * s + r) * a.np, lo, nw, a.idx_ld, Wl, wld, lane));
+      if (lane == 0) S[r * 25 + 24] = S[24 * 25 + r] = -c / hl;
+    }
+  } else if (lane < 24) {
+    S[lane * 25 + 24] = S[24 * 25 + lane] = 0.0;
+  }
+  if (lane == 0) S[24 * 25 + 24] = a.var[l];
+  PoseJacobian pj;
+  pose_jacobian<kPStride>(a.sp, a.st.q, a.st.p, a.st.tab, s, u, pj);
+  if (lane < 25) {
+    double col[3];
+    point_jacobian_column(pj, a.R_CI, a.p_CI, x, y, rho, lane, col);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) G[i * 25 + lane] = col[i];
+  }
+  __syncwarp();
+  for (int e = lane; e < 3 * 25; e += 32) {  // T = G Sigma_25
+    const int i = e / 25, b = e % 25;
+    double acc = 0.0;
+#pragma unroll 5
+    for (int k = 0; k < 25; ++k) acc = fma(G[i * 25 + k], S[k * 25 + b], acc);
+    T[e] = acc;
+  }
+  __syncwarp();
+  if (lane < 6) {  // C[i][j] = T[i] . G[j], i >= j
+    const int i = lane < 1 ? 0 : lane < 3 ? 1 : 2, j = lane - i * (i + 1) / 2;
+    double acc = 0.0;
+#pragma unroll 5
+    for (int k = 0; k < 25; ++k) acc = fma(T[i * 25 + k], G[j * 25 + k], acc);
+    out[i * 3 + j] = acc;
+    out[j * 3 + i] = acc;
+  }
+}
+
+int launch_point_cov(const PointCovLaunch& a, cudaStream_t s) {
+  if (a.n <= 0) return 0;
+  point_cov_kernel<<<(a.n + kPointCovWarps - 1) / kPointCovWarps, 32 * kPointCovWarps, 0, s>>>(a);
+  return 1;
+}
+
 }  // namespace ctvio
 
 namespace {
@@ -403,6 +499,31 @@ int form_covariance(ctvio_engine* e, int gauge_knot, const char* who, double* rc
   return CTVIO_OK;
 }
 
+// point_cov_kernel over the a.n points whose inputs a names, right after form_covariance on the same stream; the n x 9
+// result to cov9.  Ends with the stream synchronised.
+int point_covariance(ctvio_engine* e, PointCovLaunch& a, double* cov9) {
+  cudaStream_t st = e->stream;
+  auto& w = e->cws;
+  const ProblemDims d = e->dims();
+  CUDA_OK(w.pose.reserve(9 * size_t(a.n)));
+  a.st = e->x[e->cur].ptrs();
+  a.sp = e->sp;
+  a.R_CI = e->rig.R_CI;
+  a.p_CI = e->rig.p_CI;
+  a.np = d.np; a.idx_ld = d.idx_ld;
+  a.cov = w.cov.p;
+  a.var = w.var.p;
+  a.ne = e->ne(e->cur ^ 1);  // the buffer form_covariance evaluated into
+  a.lm = e->lml();
+  a.active = e->d_active.p;
+  a.out = w.pose.p;
+  e->launches += launch_point_cov(a, st);
+  CUDA_OK(cudaMemcpyAsync(cov9, w.pose.p, 9 * size_t(a.n) * sizeof(double), cudaMemcpyDeviceToHost, st));
+  e->d2h_bytes += 9 * size_t(a.n) * sizeof(double);
+  CUDA_OK(cudaStreamSynchronize(st));
+  return CTVIO_OK;
+}
+
 }  // namespace
 
 extern "C" int ctvio_covariance(ctvio_handle e, double* cov_cc, double* var_rho, double* rcond) {
@@ -464,4 +585,73 @@ extern "C" int ctvio_pose_covariance(ctvio_handle e, int32_t n, const int64_t* t
   e->d2h_bytes += 144 * size_t(n) * sizeof(double);
   CUDA_OK(cudaStreamSynchronize(st));
   return CTVIO_OK;
+}
+
+extern "C" int ctvio_point_covariance(ctvio_handle e, int32_t n, const int32_t* landmark, const int64_t* t_anchor_ns,
+                                      const double* bearing_xy, int32_t gauge_knot_index, double* cov9, double* rcond) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (n < 0 || (n > 0 && (!landmark || !t_anchor_ns || !bearing_xy || !cov9)))
+    return fail(CTVIO_ERR_INVALID, "ctvio_point_covariance: bad argument");
+  for (int32_t i = 0; i < n; ++i)
+    if (landmark[i] < 0 || landmark[i] >= e->nL) return fail(CTVIO_ERR_INVALID, "ctvio_point_covariance: landmark out of range");
+  if (gauge_knot_index < -1 || gauge_knot_index >= e->nK)
+    return fail(CTVIO_ERR_INVALID, "ctvio_point_covariance: gauge_knot_index outside -1 .. n_knots - 1");
+  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_point_covariance: not available in sharded mode");
+  if (n == 0) return CTVIO_OK;
+  if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
+  for (int32_t i = 0; i < n; ++i) {  // the range ctvio_query_trajectory accepts
+    int32_t s;
+    double u;
+    if (!spline_index(e->sp, t_anchor_ns[i], s, u))
+      return fail(CTVIO_ERR_TIME_RANGE, "ctvio_point_covariance: an anchor time outside the spline");
+  }
+  cudaSetDevice(e->cfg.device);
+  int rc = form_covariance(e, gauge_knot_index, "ctvio_point_covariance", rcond);
+  if (rc) return rc;
+  cudaStream_t st = e->stream;
+  auto& w = e->cws;
+  CUDA_OK(w.lm.reserve(size_t(n)));
+  CUDA_OK(w.t.reserve(size_t(n)));
+  CUDA_OK(w.pose.reserve(11 * size_t(n)));  // outputs, then the bearings
+  CUDA_OK(cudaMemcpyAsync(w.lm.p, landmark, size_t(n) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(w.t.p, t_anchor_ns, size_t(n) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(w.pose.p + 9 * size_t(n), bearing_xy, 2 * size_t(n) * sizeof(double), cudaMemcpyHostToDevice, st));
+  e->h2d_bytes += 28 * size_t(n);
+  PointCovLaunch a = {};
+  a.n = n;
+  a.landmark = w.lm.p;
+  a.t = w.t.p;
+  a.bearing = w.pose.p + 9 * size_t(n);
+  return point_covariance(e, a, cov9);
+}
+
+extern "C" int ctvio_feature_table_point_covariance(ctvio_handle e, int32_t n_landmarks, int32_t gauge_knot_index,
+                                                    double* cov9, double* rcond) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (gauge_knot_index < -1 || gauge_knot_index >= e->nK)
+    return fail(CTVIO_ERR_INVALID, "ctvio_feature_table_point_covariance: gauge_knot_index outside -1 .. n_knots - 1");
+  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_feature_table_point_covariance: not available in sharded mode");
+  auto& ft = e->ft;
+  if (!ft.window_current) return fail(CTVIO_ERR_STATE, "no feature-table window since the last add / slide");
+  if (e->nL != ft.n_lm) return fail(CTVIO_ERR_STATE, "the resident inverse depths no longer follow the table's numbering");
+  if (n_landmarks != ft.n_lm)
+    return fail(CTVIO_ERR_INVALID, "ctvio_feature_table_point_covariance: n_landmarks differs from the window's landmark count");
+  if (n_landmarks > 0 && !cov9) return fail(CTVIO_ERR_INVALID, "ctvio_feature_table_point_covariance: null argument");
+  if (n_landmarks == 0) return CTVIO_OK;
+  if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
+  for (int slot = 0; slot < ctvio_engine::kFrameSlots; ++slot) {  // every anchor is a held slot
+    int32_t s;
+    double u;
+    if ((ft.held >> slot & 1u) && !spline_index(e->sp, e->h_frame_t[slot], s, u))
+      return fail(CTVIO_ERR_TIME_RANGE, "ctvio_feature_table_point_covariance: a held frame time falls outside the spline");
+  }
+  cudaSetDevice(e->cfg.device);
+  int rc = form_covariance(e, gauge_knot_index, "ctvio_feature_table_point_covariance", rcond);
+  if (rc) return rc;
+  // the anchors come from the window's observation CSR and the frame table: nothing goes up
+  PointCovLaunch a = {};
+  a.n = n_landmarks;
+  a.obs_offset = ft.obs_offset.p; a.obs_slot = ft.obs_slot.p; a.obs_idx = ft.obs_idx.p;
+  a.table = e->d_frames.p; a.frame_t = e->d_frame_t.p; a.frame_cap = ctvio_engine::kFrameCap;
+  return point_covariance(e, a, cov9);
 }

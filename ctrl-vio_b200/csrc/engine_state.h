@@ -272,12 +272,14 @@ struct ctvio_engine {
     DevBuf<double> eig_scratch, Jrow, bs, A, b, Amm, V, ev, Vs, Ainv, T, Ap, bp, Ap2, V2, ev2, vb, J, r;
   } mws;
   // ctvio_covariance workspace (covariance.cu): Jacobi scales, mask, L^-1, pivots, outputs, the saved scalar block;
-  // ctvio_pose_covariance's query times and 12 x 12 outputs
+  // ctvio_pose_covariance's query times and 12 x 12 outputs; ctvio_point_covariance's landmarks, times (t) and
+  // [outputs 9 n | bearings 2 n] (pose)
   struct CovWs {
     DevBuf<double> sc, sl, X, piv, cov, var, pose;
     DevBuf<uint8_t> cmask;
     DevBuf<LmScalars> scal;
     DevBuf<int64_t> t;
+    DevBuf<int32_t> lm;
   } cws;
   int n_marg_img = -1;  // marginalized image factors of the last ctvio_marginalize (-1: pos_cam / pos_lm / marg_img not built)
 

@@ -385,6 +385,36 @@ struct PoseCovLaunch {
   double* out;             // [n][144]
 };
 int launch_pose_cov(const PoseCovLaunch& a, cudaStream_t s);
+// ctvio_point_covariance / ctvio_feature_table_point_covariance: one warp per point, out[n][3][3] = G Sigma_25 G' of the
+// world point of landmark l anchored at time t with bearing (x, y, 1) (point_jacobian_column, spline_eval.cuh), Sigma_25
+// the joint covariance of its segment's 24 knot dims and rho_l
+struct FrameFeature;  // frontend.h
+struct PointCovLaunch {
+  StatePtrs st;
+  SplineParams sp;
+  M3 R_CI;
+  V3 p_CI;
+  int32_t n, np, idx_ld;
+  // per point either the caller's arrays (landmark != null) ...
+  const int32_t* landmark; // [n] 0 .. nL - 1
+  const int64_t* t;        // [n] anchor times, inside the spline (checked by the caller)
+  const double* bearing;   // [n][2]
+  // ... or point l = landmark l of the feature table's window, its anchor the first entry of its observation CSR, the
+  // time the anchor slot's frame time (every held slot's time checked by the caller)
+  const int32_t* obs_offset;
+  const int32_t* obs_slot;
+  const int32_t* obs_idx;
+  const FrameFeature* table;  // [n_slots][frame_cap]
+  const int64_t* frame_t;     // [n_slots]
+  int32_t frame_cap;
+  const double* cov;       // [np][np] the window covariance
+  const double* var;       // [nL] the inverse-depth variances of the same call
+  NormalEqPtrs ne;         // the coupling rows the covariance was formed from
+  LandmarkLayout lm;
+  const uint8_t* active;   // [np + nL]
+  double* out;             // [n][9]
+};
+int launch_point_cov(const PointCovLaunch& a, cudaStream_t s);
 int launch_chol_coop(const LinearLaunch& a, cudaStream_t s);
 int launch_step_vectors(const LinearLaunch& a, cudaStream_t s);
 // sharded mode: the iteration-0 Jacobi scale from the all-reduced camera diagonal (the LM damping and identity rows

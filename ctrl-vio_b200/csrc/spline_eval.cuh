@@ -639,4 +639,25 @@ CTVIO_HD void pose_jacobian_column(const PoseJacobian& J, bool camera, const M3&
   out[9] = dv.x; out[10] = dv.y; out[11] = dv.z;
 }
 
+// ------------------------------- point covariance -----------------------------------------------
+// Column col (0..24) of G = d P / d (delta_k, dP_k, rho) for the world point of a landmark with inverse depth rho and
+// anchor bearing b = (x, y, 1), J evaluated at its anchor frame time (the point of ctvio_feature_table_map):
+//   P = R (m) + p,  m = R_CI b / rho + p_CI.
+// Columns 0..23 (the knots of the segment, pose_jacobian_column's order): -R [m]x dtheta + dp = R (dtheta x m) + dp from
+// the body dtheta and dp rows; column 24: d P / d rho = -R R_CI b / rho^2.
+CTVIO_HD void point_jacobian_column(const PoseJacobian& J, const M3& R_CI, V3 p_CI, double x, double y, double rho, int col,
+                                    double out[3]) {
+  const V3 c = m3_vec(R_CI, V3{x, y, 1.0});
+  V3 g;
+  if (col < 24) {
+    double pc[12];
+    pose_jacobian_column(J, false, R_CI, p_CI, col, pc);
+    const V3 m = (1.0 / rho) * c + p_CI;
+    g = m3_vec(J.ev.R, cross(V3{pc[0], pc[1], pc[2]}, m)) + V3{pc[3], pc[4], pc[5]};
+  } else {
+    g = (-1.0 / (rho * rho)) * m3_vec(J.ev.R, c);
+  }
+  out[0] = g.x; out[1] = g.y; out[2] = g.z;
+}
+
 }  // namespace ctvio

@@ -283,6 +283,19 @@ class TrajectoryEstimator {
     return rcond;
   }
 
+  // the covariance of the world points of n landmarks, each anchored at time t (ns) with the bearing (x, y, 1), from the
+  // window covariance and the landmark-knot cross terms (see ctvio_point_covariance): cov9 [n][3][3] row-major, world
+  // frame.  Knots <= gauge_knot_index are held constant for this call only (-1: the options alone).  Returns rcond;
+  // throws ctvio_host::Error on a rank-deficient window.
+  double GetPointCovariance(int n, const int32_t* landmark, const int64_t* t, const double* bearing_xy,
+                            int gauge_knot_index, double* cov9) {
+    upload();
+    double rcond = 0.0;
+    check(ctvio_point_covariance(h_, n, landmark, t, bearing_xy, gauge_knot_index, cov9, &rcond),
+          "ctvio_point_covariance");
+    return rcond;
+  }
+
   // TrajectoryManager::double2vector (trajectory_manager.cpp:485-516): R0 row-major, t0; knots >= min_idx
   void GaugeRealign(int min_idx, const double R0[9], const double t0[3]) {
     check(ctvio_gauge_realign(h_, min_idx, R0, t0), "ctvio_gauge_realign");

@@ -661,27 +661,40 @@ class ResidentRunner(StreamingRunner):
     maxTimeNs() - 50 ms) comes from the device (PoseCovariance with camera_frame=True).  The main solve fixes no knots,
     so the call holds knots 0..3 (the window's first segment) constant as its own gauge.  The 12 x 12 matrix is kept on
     last_pose_cov and the record gains pose_cov_rcond and ms_pose_cov; a window the call finds rank deficient records
-    pose_cov_rcond = nan, its message as pose_cov_error, and keeps last_pose_cov = None."""
+    pose_cov_rcond = nan, its message as pose_cov_error, and keeps last_pose_cov = None.
+
+    publish_map_covariance=True (requires publish_map=True): right after GaugeRealign, next to the pose covariance and
+    with the same gauge (knots 0..3), the covariance of every landmark's world point in the window's numbering comes
+    from the device (FeatureTablePointCovariance, ids from FeatureTableLandmarks).  After FeatureTableMap the matrices
+    are attached to the map points by feature id and kept on last_map_cov [n_points, 3, 3]: a point whose entry had no
+    number in the window, or was anchored in the leaving frame (re-anchored by reanchor=True), has no covariance and
+    gets NaN.  The record gains point_cov_rcond, ms_point_cov and n_map_points_without_cov; a window the call finds rank
+    deficient records point_cov_rcond = nan and its message as point_cov_error, and keeps last_map_cov = None.  With
+    publish_covariance as well, the window covariance is formed twice (once per call)."""
 
     POSE_COV_LAG_NS = 50_000_000
     POSE_COV_GAUGE_KNOT = 3
 
     def __init__(self, lib, seq, triangulate=False, device_features=False, publish_map=False, reanchor=False,
-                 publish_covariance=False, **kw):
+                 publish_covariance=False, publish_map_covariance=False, **kw):
         if device_features and not triangulate:
             raise ValueError("device_features requires triangulate=True: new landmarks enter with inverse depth -1")
         if publish_map and not device_features:
             raise ValueError("publish_map requires device_features=True: the map is read from the resident feature table")
         if reanchor and not device_features:
             raise ValueError("reanchor requires device_features=True: landmarks are re-anchored in the resident feature table")
+        if publish_map_covariance and not publish_map:
+            raise ValueError("publish_map_covariance requires publish_map=True: the covariances belong to the map's points")
         super().__init__(lib, seq, **kw)
         self.triangulate = triangulate
         self.device_features = device_features
         self.publish_map = publish_map
         self.reanchor = reanchor
         self.publish_covariance = publish_covariance
+        self.publish_map_covariance = publish_map_covariance
         self.last_map = None
         self.last_pose_cov = None
+        self.last_map_cov = None
         self.triangulate_probe = None
         if self.clouds is None:
             self.clouds = FrameClouds(seq)
@@ -859,6 +872,17 @@ class ResidentRunner(StreamingRunner):
                 self.last_pose_cov = None
                 pose_cov = dict(pose_cov_rcond=float("nan"), pose_cov_error=str(err))
             pose_cov["ms_pose_cov"] = 1e3 * (time.perf_counter() - t_cov)
+        point_cov = lm_cov = None
+        if self.publish_map_covariance:                # the covariances of the window's landmark points, before the slide
+            t_cov = time.perf_counter()
+            try:
+                cov, rc = e.FeatureTablePointCovariance(gauge_knot_index=self.POSE_COV_GAUGE_KNOT)
+                lm_ids, lm_anchor, _ = e.FeatureTableLandmarks()
+                lm_cov = (cov, lm_ids, lm_anchor)
+                point_cov = dict(point_cov_rcond=rc)
+            except CtvioError as err:
+                point_cov = dict(point_cov_rcond=float("nan"), point_cov_error=str(err))
+            point_cov["ms_point_cov"] = 1e3 * (time.perf_counter() - t_cov)
         if marg:
             n_out = C_int32(); nb_out = C_int32()
             e.lib.call("marginalize", e.h, byref(n_out), byref(nb_out))
@@ -880,6 +904,10 @@ class ResidentRunner(StreamingRunner):
             n_removed = e.FeatureTableSlide(self.slot_of[self.frames[0 if marg else -2]])
         if self.publish_map:                           # the landmark map and keyframe poses of the post-slide window
             self.last_map = e.FeatureTableMap(np.delete(frame_slots, 0 if marg else len(frame_slots) - 2), WINDOW_SIZE)
+        if self.publish_map_covariance:
+            self.last_map_cov = None if lm_cov is None else self._map_covariance(lm_cov, frame_slots[0 if marg else -2])
+            point_cov["n_map_points_without_cov"] = (len(self.last_map[1]) if self.last_map_cov is None else
+                                                     int(np.isnan(self.last_map_cov[:, 0, 0]).sum()))
         t_wall = time.perf_counter() - t_start
         h2d, d2h = (0, 0) if first else e.TransferStats(reset=True)
 
@@ -903,6 +931,8 @@ class ResidentRunner(StreamingRunner):
             rec.update(decision)
         if pose_cov is not None:
             rec.update(pose_cov)
+        if point_cov is not None:
+            rec.update(point_cov)
         if self.device_features:
             # n_new_lm: the window's landmarks without a depth yet (-1), which are exactly the ones TriangulateWindow wrote
             rec.update(n_triangulated=n_tri, n_fallback=n_fb, n_new_lm=n_tri + n_fb, n_removed=n_removed)
@@ -915,6 +945,19 @@ class ResidentRunner(StreamingRunner):
         self.records.append(rec)
         self.step_index += 1
         return rec
+
+    def _map_covariance(self, lm_cov, leaving_slot):
+        """[n_points, 3, 3]: the window's point covariances attached to last_map's points by feature id; NaN for a point
+        whose entry had no number in the window or was anchored in the leaving slot (re-anchored since)"""
+        cov, ids, anchor = lm_cov
+        keep = anchor != leaving_slot
+        of_id = dict(zip(ids[keep].tolist(), np.nonzero(keep)[0].tolist()))
+        out = np.full((len(self.last_map[1]), 3, 3), np.nan)
+        for k, i in enumerate(self.last_map[1].tolist()):
+            l = of_id.get(i)
+            if l is not None:
+                out[k] = cov[l]
+        return out
 
     def _observation_csr(self, frames, w, lm_global, slot_j, idx_j, frame_slots=None):
         """(obs_offset, obs_slot, obs_idx) of TriangulateWindow: per window landmark its anchor, then its observations

@@ -277,6 +277,25 @@ int ctvio_covariance(ctvio_handle h, double* cov_cc, double* var_rho, double* rc
  *   ctvio_transfer_stats counts 8 n bytes up and 1152 n bytes down. */
 int ctvio_pose_covariance(ctvio_handle h, int32_t n, const int64_t* t_ns, int32_t gauge_knot_index,
                           int32_t camera_frame, double* cov12, double* rcond);
+/* ctvio_point_covariance - covariance of the world points of n anchored landmarks, from the window covariance of
+ *   ctvio_covariance (same H, same gauge argument, same rcond test and failure mode, same absence of side effects);
+ *   neither the np x np matrix nor the landmark couplings leave the device.
+ *   Point k is landmark[k] (inverse depth rho) anchored at time t_anchor_ns[k] with the bearing
+ *   b = (bearing_xy[2k], bearing_xy[2k+1], 1):  P = R(t) (R_CI b / rho + p_CI) + p(t), the point
+ *   ctvio_feature_table_map publishes for an entry anchored in a frame at that time (the frame time, not a row time).
+ *   cov9[n][3][3] (row-major, world frame, exactly symmetric): G Sigma_25 G', G = dP / d(knots of t's segment, rho) and
+ *     Sigma_25 the joint covariance of those 24 knot dims and rho: the 24 x 24 block of the window covariance, the cross
+ *     column -Sigma W' / h of the landmark's coupling row W and diagonal h, and its variance from ctvio_covariance.
+ *   A landmark no factor touches has rho constant: only the pose part remains, and a point whose four knots and rho
+ *   are all constant gets an exact zero matrix.  A rho that is not > 0 and finite gives a matrix of NaNs.
+ *   rcond (may be NULL): as ctvio_covariance; on CTVIO_ERR_STATE "rank deficient" only rcond is written.
+ *   Errors, checked before anything is launched, with nothing written: CTVIO_ERR_INVALID for a null handle, n < 0,
+ *   a NULL array with n > 0, a landmark outside 0 .. n_landmarks - 1, gauge_knot_index outside -1 .. n_knots - 1;
+ *   CTVIO_ERR_STATE in sharded mode or before the knots are set; CTVIO_ERR_TIME_RANGE for an anchor time
+ *   ctvio_query_trajectory does not accept.  n = 0 returns CTVIO_OK and launches nothing.
+ *   ctvio_transfer_stats counts 28 n bytes up and 72 n bytes down. */
+int ctvio_point_covariance(ctvio_handle h, int32_t n, const int32_t* landmark, const int64_t* t_anchor_ns,
+                           const double* bearing_xy, int32_t gauge_knot_index, double* cov9, double* rcond);
 
 /* ---- spline query service (SURVEY §8f-2: Trajectory::poseNs / GetIMUState, spline/trajectory.cpp:27-55) ----
  * batch R(t), p(t), body angular velocity, world linear velocity and acceleration. Any output may be NULL. */
@@ -529,6 +548,24 @@ int ctvio_feature_table_landmarks(ctvio_handle h, int32_t n_landmarks, int32_t* 
 int ctvio_feature_table_map(ctvio_handle h, int32_t n_frames, const int32_t* frame_slots, int32_t window_size,
                             int32_t capacity, double* xyz_world, int32_t* feature_id, uint8_t* in_margin_cloud,
                             int32_t* n_points, double* cam_q_xyzw, double* cam_p_xyz);
+/* ctvio_feature_table_point_covariance - ctvio_point_covariance for every landmark of the feature table's last window,
+ *   in the numbering of ctvio_feature_table_window / ctvio_feature_table_landmarks: cov9[n_landmarks][3][3].  Landmark
+ *   l's anchor is the first entry of its observation CSR (anchor slot, feature index): the bearing is that feature's in
+ *   the frame table, the time the anchor slot's frame time.  rcond as ctvio_point_covariance.
+ *   When it applies to a map point: call it after the solve and ctvio_gauge_realign and before the slide (after the
+ *   slide H no longer matches the state).  A map entry that keeps its anchor and its number across the slide is the
+ *   same function of the same state in ctvio_feature_table_map: for it, the matrix of its number is the covariance of
+ *   the point the map publishes.  An entry re-anchored by ctvio_feature_table_slide_reanchor loses its number, and its
+ *   new point has no covariance from this call.
+ *   Errors, checked before anything is launched, with nothing written: CTVIO_ERR_INVALID for a null handle,
+ *   gauge_knot_index outside -1 .. n_knots - 1, n_landmarks other than the window's landmark count, or a NULL cov9
+ *   with n_landmarks > 0; CTVIO_ERR_STATE in sharded mode, without a window since the last add / slide, when the
+ *   resident inverse-depth count differs from the window's landmark count, or before the knots are set;
+ *   CTVIO_ERR_TIME_RANGE when the frame time of a slot the table holds falls outside the spline.  n_landmarks = 0
+ *   returns CTVIO_OK and launches nothing.
+ *   Nothing goes up; ctvio_transfer_stats counts 72 n_landmarks bytes down. */
+int ctvio_feature_table_point_covariance(ctvio_handle h, int32_t n_landmarks, int32_t gauge_knot_index, double* cov9,
+                                         double* rcond);
 
 /* bytes moved host<->device by the C-ABI calls since the last reset (state, factors, priors, index tables) */
 int ctvio_transfer_stats(ctvio_handle h, int64_t* h2d_bytes, int64_t* d2h_bytes, int32_t reset);
