@@ -100,7 +100,7 @@ ABI_SYMBOLS = [
     "solve", "gauge_realign", "marginalize", "get_prior", "adopt_prior",
     "save_state", "restore_state",
     "eval_image_factors", "eval_imu_factors", "residual_summary", "eval_cost", "normal_equations", "covariance",
-    "pose_covariance", "point_covariance", "query_trajectory", "triangulate",
+    "pose_covariance", "relative_pose_covariance", "point_covariance", "query_trajectory", "triangulate",
     "extend_knots_to", "slide_window", "remap_landmarks", "enable_prior", "ingest_feature_cloud", "add_image_features_from_slots",
     "ingest_imu", "add_imu_from_table", "transfer_stats", "profile_kernels", "measure_fp64_tflops", "measure_fp64_tensor_tflops",
     "selfcheck_solver", "nccl_unique_id", "comm_init", "triangulate_window", "check_keyframe", "slide_window_second_new",
@@ -119,7 +119,7 @@ DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enab
                        "slide_window_second_new", "feature_table_add", "feature_table_window", "triangulate_window_from_table",
                        "add_image_features_from_table", "feature_table_slide", "feature_table_landmarks",
                        "feature_table_map", "feature_table_slide_reanchor", "debug_structure", "covariance",
-                       "pose_covariance", "point_covariance", "feature_table_point_covariance")
+                       "pose_covariance", "relative_pose_covariance", "point_covariance", "feature_table_point_covariance")
 
 
 def _addr(a):
@@ -401,6 +401,21 @@ class Estimator:
         self.lib.call("pose_covariance", self.h, C.c_int32(n), _lp(t), C.c_int32(int(gauge_knot_index)),
                       C.c_int32(int(bool(camera_frame))), _dp(cov), C.byref(rcond))
         return cov, rcond.value
+
+    def RelativePoseCovariance(self, t_a, t_b, gauge_knot_index=-1, camera_frame=False, want_cross=False):
+        """Covariance of (dtheta_ab, dp_ab), the pose at t_b in the frame of the pose at t_a, for each pair
+        (ctvio_relative_pose_covariance): (cov [n, 6, 6], cross [n, 6, 6] or None, rcond).  cross (want_cross=True) is the
+        covariance of the two poses' (dtheta, dp), rows a and columns b.  Knots <= gauge_knot_index are held constant for
+        this call only; camera_frame=True gives the camera poses.  Raises CtvioError on a rank-deficient window, with
+        rcond in the message."""
+        ta = _i64(np.atleast_1d(t_a)); tb = _i64(np.atleast_1d(t_b)); n = ta.shape[0]
+        assert tb.shape[0] == n
+        cov = np.zeros((n, 6, 6))
+        cross = np.zeros((n, 6, 6)) if want_cross else None
+        rcond = C.c_double()
+        self.lib.call("relative_pose_covariance", self.h, C.c_int32(n), _lp(ta), _lp(tb), C.c_int32(int(gauge_knot_index)),
+                      C.c_int32(int(bool(camera_frame))), _dp(cov), _dp(cross), C.byref(rcond))
+        return cov, cross, rcond.value
 
     def PointCovariance(self, landmark, t, bearing, gauge_knot_index=-1):
         """Covariance of the world points of landmarks anchored at the times t with the bearings (x, y)

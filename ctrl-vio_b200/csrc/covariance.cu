@@ -14,6 +14,8 @@
 //
 // ctvio_pose_covariance forms the same Sigma (with an optional gauge of its own in the mask) and projects it to the
 // pose and velocity at each query time on the device (pose_cov_kernel, 12 x 24 Jacobians, plain fp64 fma chains).
+// ctvio_relative_pose_covariance projects it to the pose at t_b in the frame of the pose at t_a, over the union of the
+// two segments' knots, with the cross-covariance of the two poses (relative_pose_cov_kernel, 6 x 48 Jacobians).
 // ctvio_point_covariance and ctvio_feature_table_point_covariance project it, with the landmark-knot cross terms
 // -Sigma W_l' / h_l and the variance of rho_l, to anchored landmarks' world points (point_cov_kernel, 3 x 25 Jacobians).
 #include <cmath>
@@ -422,6 +424,100 @@ int launch_point_cov(const PointCovLaunch& a, cudaStream_t s) {
   return 1;
 }
 
+// One warp (one CTA) per pair: C = (G Sigma_U) G' with U the union of the knots of t_a's and t_b's segments (4 to 8
+// knots, m = 24 .. 48 dims, relative_union_knot), Sigma_U its block of the window covariance and G (6 x m) the
+// relative-pose Jacobian (relative_pose_jacobian_column over the two poses' dtheta / dp rows J_a, J_b, 6 x 24 each).
+// Shared knots get one column, so their terms cancel inside G rather than between two stacked 24-dim blocks.  The cross
+// block X = (J_a Sigma_ab) J_b' reads the same Sigma_U at the two segments' slots.  Every lane evaluates both splines (the
+// same values in all lanes); the products are fixed-order fma chains, one output entry per lane, no atomics; the lower
+// triangle of C is formed and mirrored: exactly symmetric.  26.5 KB of static shared memory per CTA.
+constexpr int kRelUnion = 48;
+__global__ void __launch_bounds__(32) relative_pose_cov_kernel(RelativePoseCovLaunch a) {
+  __shared__ double S[kRelUnion * kRelUnion], Ja[6 * 24], Jb[6 * 24], G[6 * kRelUnion], T[6 * kRelUnion], X[6 * 24];
+  const int lane = threadIdx.x, n = blockIdx.x;
+  const bool camera = a.camera_frame != 0;
+  int32_t sa, sb;
+  double ua, ub;
+  spline_index(a.sp, a.t_a[n], sa, ua);
+  spline_index(a.sp, a.t_b[n], sb, ub);
+  const int off = relative_union_offset(sa, sb), m = 6 * (4 + off);
+  const int fa = relative_union_first(sa, sb), fb = relative_union_first(sb, sa);
+  for (int e = lane; e < m * m; e += 32) {  // Sigma_U, row by row
+    const int i = e / m, j = e - i * m;
+    const int gi = 6 * relative_union_knot(sa, sb, i / 6) + i % 6, gj = 6 * relative_union_knot(sa, sb, j / 6) + j % 6;
+    S[e] = a.cov[size_t(gi) * a.np + gj];
+  }
+  M3 R[2];
+  V3 pos[2];
+#pragma unroll 1
+  for (int side = 0; side < 2; ++side) {  // a, then b: one PoseJacobian live at a time
+    PoseJacobian pj;
+    pose_jacobian<kPStride>(a.sp, a.st.q, a.st.p, a.st.tab, side ? sb : sa, side ? ub : ua, pj);
+    if (lane < 24) {
+      double col[12];
+      pose_jacobian_column(pj, camera, a.R_CI, a.p_CI, lane, col);
+      double* J = side ? Jb : Ja;
+#pragma unroll
+      for (int i = 0; i < 6; ++i) J[i * 24 + lane] = col[i];
+    }
+    frame_pose(pj, camera, a.R_CI, a.p_CI, R[side], pos[side]);
+  }
+  const RelativePose rel = relative_pose(R[0], pos[0], R[1], pos[1]);
+  __syncwarp();
+  for (int c = lane; c < m; c += 32) {
+    double g[6];
+    relative_pose_jacobian_column(rel, Ja, fa, Jb, fb, c, g);
+#pragma unroll
+    for (int i = 0; i < 6; ++i) G[i * m + c] = g[i];
+  }
+  __syncwarp();
+  for (int e = lane; e < 6 * m; e += 32) {  // T = G Sigma_U
+    const int i = e / m, b = e - i * m;
+    double acc = 0.0;
+#pragma unroll 6
+    for (int k = 0; k < m; ++k) acc = fma(G[i * m + k], S[k * m + b], acc);
+    T[e] = acc;
+  }
+  if (a.cross) {
+    for (int e = lane; e < 6 * 24; e += 32) {  // X = J_a Sigma_ab: rows at a's slots, columns at b's
+      const int i = e / 24, b = e % 24;
+      const double* Sab = S + size_t(6 * fa) * m + 6 * fb;
+      double acc = 0.0;
+#pragma unroll 8
+      for (int k = 0; k < 24; ++k) acc = fma(Ja[i * 24 + k], Sab[k * m + b], acc);
+      X[e] = acc;
+    }
+  }
+  __syncwarp();
+  double* out = a.out + size_t(n) * 36;
+  if (lane < 21) {  // C[i][j] = T[i] . G[j], i >= j
+    int i = 0;
+    while ((i + 1) * (i + 2) / 2 <= lane) ++i;
+    const int j = lane - i * (i + 1) / 2;
+    double acc = 0.0;
+#pragma unroll 6
+    for (int k = 0; k < m; ++k) acc = fma(T[i * m + k], G[j * m + k], acc);
+    out[i * 6 + j] = acc;
+    out[j * 6 + i] = acc;
+  }
+  if (a.cross) {
+    double* cx = a.cross + size_t(n) * 36;
+    for (int e = lane; e < 36; e += 32) {  // cross[i][j] = X[i] . J_b[j]
+      const int i = e / 6, j = e % 6;
+      double acc = 0.0;
+#pragma unroll 8
+      for (int k = 0; k < 24; ++k) acc = fma(X[i * 24 + k], Jb[j * 24 + k], acc);
+      cx[e] = acc;
+    }
+  }
+}
+
+int launch_relative_pose_cov(const RelativePoseCovLaunch& a, cudaStream_t s) {
+  if (a.n <= 0) return 0;
+  relative_pose_cov_kernel<<<a.n, 32, 0, s>>>(a);
+  return 1;
+}
+
 }  // namespace ctvio
 
 namespace {
@@ -583,6 +679,55 @@ extern "C" int ctvio_pose_covariance(ctvio_handle e, int32_t n, const int64_t* t
   e->launches += launch_pose_cov(a, st);
   CUDA_OK(cudaMemcpyAsync(cov12, w.pose.p, 144 * size_t(n) * sizeof(double), cudaMemcpyDeviceToHost, st));
   e->d2h_bytes += 144 * size_t(n) * sizeof(double);
+  CUDA_OK(cudaStreamSynchronize(st));
+  return CTVIO_OK;
+}
+
+extern "C" int ctvio_relative_pose_covariance(ctvio_handle e, int32_t n, const int64_t* t_a_ns, const int64_t* t_b_ns,
+                                              int32_t gauge_knot_index, int32_t camera_frame, double* cov6,
+                                              double* cross6, double* rcond) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (n < 0 || (n > 0 && (!t_a_ns || !t_b_ns || !cov6)))
+    return fail(CTVIO_ERR_INVALID, "ctvio_relative_pose_covariance: bad argument");
+  if (camera_frame != 0 && camera_frame != 1)
+    return fail(CTVIO_ERR_INVALID, "ctvio_relative_pose_covariance: camera_frame must be 0 or 1");
+  if (gauge_knot_index < -1 || gauge_knot_index >= e->nK)
+    return fail(CTVIO_ERR_INVALID, "ctvio_relative_pose_covariance: gauge_knot_index outside -1 .. n_knots - 1");
+  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_relative_pose_covariance: not available in sharded mode");
+  if (n == 0) return CTVIO_OK;
+  if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
+  for (int32_t i = 0; i < n; ++i) {  // the range ctvio_query_trajectory accepts
+    int32_t s;
+    double u;
+    if (!spline_index(e->sp, t_a_ns[i], s, u) || !spline_index(e->sp, t_b_ns[i], s, u))
+      return fail(CTVIO_ERR_TIME_RANGE, "ctvio_relative_pose_covariance: a time outside the spline");
+  }
+  cudaSetDevice(e->cfg.device);
+  int rc = form_covariance(e, gauge_knot_index, "ctvio_relative_pose_covariance", rcond);
+  if (rc) return rc;
+  cudaStream_t st = e->stream;
+  auto& w = e->cws;
+  const size_t nn = size_t(n), n_out = cross6 ? 72 : 36;
+  CUDA_OK(w.t.reserve(2 * nn));
+  CUDA_OK(w.pose.reserve(n_out * nn));  // cov6, then cross6
+  CUDA_OK(cudaMemcpyAsync(w.t.p, t_a_ns, nn * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(w.t.p + nn, t_b_ns, nn * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  e->h2d_bytes += 2 * nn * sizeof(int64_t);
+  RelativePoseCovLaunch a;
+  a.st = e->x[e->cur].ptrs();
+  a.sp = e->sp;
+  a.R_CI = e->rig.R_CI;
+  a.p_CI = e->rig.p_CI;
+  a.n = n; a.np = e->dims().np; a.camera_frame = camera_frame;
+  a.t_a = w.t.p;
+  a.t_b = w.t.p + nn;
+  a.cov = w.cov.p;
+  a.out = w.pose.p;
+  a.cross = cross6 ? w.pose.p + 36 * nn : nullptr;
+  e->launches += launch_relative_pose_cov(a, st);
+  CUDA_OK(cudaMemcpyAsync(cov6, a.out, 36 * nn * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (cross6) CUDA_OK(cudaMemcpyAsync(cross6, a.cross, 36 * nn * sizeof(double), cudaMemcpyDeviceToHost, st));
+  e->d2h_bytes += n_out * nn * sizeof(double);
   CUDA_OK(cudaStreamSynchronize(st));
   return CTVIO_OK;
 }

@@ -273,7 +273,7 @@ struct ctvio_engine {
   } mws;
   // ctvio_covariance workspace (covariance.cu): Jacobi scales, mask, L^-1, pivots, outputs, the saved scalar block;
   // ctvio_pose_covariance's query times and 12 x 12 outputs; ctvio_point_covariance's landmarks, times (t) and
-  // [outputs 9 n | bearings 2 n] (pose)
+  // [outputs 9 n | bearings 2 n] (pose); ctvio_relative_pose_covariance's [t_a | t_b] (t) and [cov6 | cross6] (pose)
   struct CovWs {
     DevBuf<double> sc, sl, X, piv, cov, var, pose;
     DevBuf<uint8_t> cmask;

@@ -385,6 +385,22 @@ struct PoseCovLaunch {
   double* out;             // [n][144]
 };
 int launch_pose_cov(const PoseCovLaunch& a, cudaStream_t s);
+// ctvio_relative_pose_covariance: one warp per pair, out[n][6][6] = G Sigma_U G' of the pose at t_b in the frame of the
+// pose at t_a, Sigma_U the block of the window covariance at the union of the two segments' knots
+// (relative_pose_jacobian_column, spline_eval.cuh), and cross[n][6][6] = J_a Sigma_ab J_b' of the two poses
+struct RelativePoseCovLaunch {
+  StatePtrs st;
+  SplineParams sp;
+  M3 R_CI;
+  V3 p_CI;
+  int32_t n, np, camera_frame;
+  const int64_t* t_a;      // [n], inside the spline (checked by the caller)
+  const int64_t* t_b;      // [n], inside the spline (checked by the caller)
+  const double* cov;       // [np][np] the window covariance
+  double* out;             // [n][36]
+  double* cross;           // [n][36] or null
+};
+int launch_relative_pose_cov(const RelativePoseCovLaunch& a, cudaStream_t s);
 // ctvio_point_covariance / ctvio_feature_table_point_covariance: one warp per point, out[n][3][3] = G Sigma_25 G' of the
 // world point of landmark l anchored at time t with bearing (x, y, 1) (point_jacobian_column, spline_eval.cuh), Sigma_25
 // the joint covariance of its segment's 24 knot dims and rho_l

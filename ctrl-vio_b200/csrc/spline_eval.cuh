@@ -660,4 +660,71 @@ CTVIO_HD void point_jacobian_column(const PoseJacobian& J, const M3& R_CI, V3 p_
   out[0] = g.x; out[1] = g.y; out[2] = g.z;
 }
 
+// ------------------------------- relative pose covariance ---------------------------------------
+// The pose whose perturbation the dtheta and dp rows of pose_jacobian_column describe: the body (R, p), or with camera
+// the camera (R R_CI, p + R p_CI).
+CTVIO_HD void frame_pose(const PoseJacobian& J, bool camera, const M3& R_CI, V3 p_CI, M3& R, V3& p) {
+  R = camera ? m3_mul(J.ev.R, R_CI) : J.ev.R;
+  p = camera ? J.ev.p + m3_vec(J.ev.R, p_CI) : J.ev.p;
+}
+
+// The pose of b in the frame of a: R_ab = R_a' R_b, p_ab = R_a' (p_b - p_a).  Its perturbation (dtheta_ab right,
+// R_ab -> R_ab Exp(dtheta_ab); dp_ab additive, in frame a) to first order in those of the two poses (dtheta right, dp
+// world):
+//   dtheta_ab = dtheta_b - R_ab' dtheta_a,   dp_ab = R_a' (dp_b - dp_a) + [p_ab]x dtheta_a.
+struct RelativePose {
+  M3 Ra, Rab;
+  V3 pab;
+};
+
+CTVIO_HD RelativePose relative_pose(const M3& Ra, V3 pa, const M3& Rb, V3 pb) {
+  RelativePose r;
+  r.Ra = Ra;
+  r.Rab = m3_mul(m3_transpose(Ra), Rb);
+  r.pab = m3_tvec(Ra, pb - pa);
+  return r;
+}
+
+// The union U of the knots of two segments sa and sb (four knots each), lo = min, hi = max: lo's four knots in slots
+// 0..3, hi's knots in slots off .. off + 3 with off = min(hi - lo, 4).  So U has 4 + off knots: contiguous (lo ..
+// hi + 3) when the segments overlap, lo .. lo + 3 then hi .. hi + 3 when they do not.
+CTVIO_HD int relative_union_offset(int32_t sa, int32_t sb) {
+  const int32_t d = sa > sb ? sa - sb : sb - sa;
+  return d < 4 ? int(d) : 4;
+}
+
+// the slot of segment s's first knot in its union with segment other
+CTVIO_HD int relative_union_first(int32_t s, int32_t other) { return s <= other ? 0 : relative_union_offset(s, other); }
+
+// the window knot of slot u of the union of sa and sb
+CTVIO_HD int32_t relative_union_knot(int32_t sa, int32_t sb, int u) {
+  const int32_t lo = sa < sb ? sa : sb, hi = sa < sb ? sb : sa;
+  const int off = relative_union_offset(sa, sb);
+  return u < off ? lo + u : hi + (u - off);
+}
+
+// Column col (0 .. 6 |U| - 1; slot col / 6, r = col % 6 as in pose_jacobian_column) of G = d (dtheta_ab, dp_ab) / d U.
+// Ja, Jb: the dtheta and dp rows ([6][24], row-major) of the two poses' Jacobians over their own segments, the first six
+// rows of pose_jacobian_column for the body or the camera; fa, fb: the slot of each segment's first knot in U
+// (relative_union_first).  A knot both segments share gets both contributions in the one column.
+CTVIO_HD void relative_pose_jacobian_column(const RelativePose& rel, const double* Ja, int fa, const double* Jb, int fb,
+                                            int col, double out[6]) {
+  const int u = col / 6, r = col % 6;
+  V3 tha{0, 0, 0}, pa{0, 0, 0}, thb{0, 0, 0}, pb{0, 0, 0};
+  if (u >= fa && u < fa + 4) {
+    const int c = 6 * (u - fa) + r;
+    tha = V3{Ja[c], Ja[24 + c], Ja[48 + c]};
+    pa = V3{Ja[72 + c], Ja[96 + c], Ja[120 + c]};
+  }
+  if (u >= fb && u < fb + 4) {
+    const int c = 6 * (u - fb) + r;
+    thb = V3{Jb[c], Jb[24 + c], Jb[48 + c]};
+    pb = V3{Jb[72 + c], Jb[96 + c], Jb[120 + c]};
+  }
+  const V3 th = thb - m3_tvec(rel.Rab, tha);
+  const V3 dp = m3_tvec(rel.Ra, pb - pa) + cross(rel.pab, tha);
+  out[0] = th.x; out[1] = th.y; out[2] = th.z;
+  out[3] = dp.x; out[4] = dp.y; out[5] = dp.z;
+}
+
 }  // namespace ctvio

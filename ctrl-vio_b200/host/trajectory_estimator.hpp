@@ -283,6 +283,20 @@ class TrajectoryEstimator {
     return rcond;
   }
 
+  // the covariance of the relative pose between t_a and t_b (ns) for n pairs, the pose at t_b in the frame of the pose
+  // at t_a, from the window covariance (see ctvio_relative_pose_covariance): cov6 [n][6][6] row-major over (dtheta_ab,
+  // dp_ab), of the body or (camera_frame) of the camera; cross6 [n][6][6] (may be null) the covariance of the two
+  // poses' (dtheta, dp), rows a and columns b.  Knots <= gauge_knot_index are held constant for this call only (-1: the
+  // options alone).  Returns rcond; throws ctvio_host::Error on a rank-deficient window.
+  double GetRelativePoseCovariance(int n, const int64_t* t_a, const int64_t* t_b, int gauge_knot_index, bool camera_frame,
+                                   double* cov6, double* cross6 = nullptr) {
+    upload();
+    double rcond = 0.0;
+    check(ctvio_relative_pose_covariance(h_, n, t_a, t_b, gauge_knot_index, camera_frame ? 1 : 0, cov6, cross6, &rcond),
+          "ctvio_relative_pose_covariance");
+    return rcond;
+  }
+
   // the covariance of the world points of n landmarks, each anchored at time t (ns) with the bearing (x, y, 1), from the
   // window covariance and the landmark-knot cross terms (see ctvio_point_covariance): cov9 [n][3][3] row-major, world
   // frame.  Knots <= gauge_knot_index are held constant for this call only (-1: the options alone).  Returns rcond;

@@ -670,13 +670,21 @@ class ResidentRunner(StreamingRunner):
     number in the window, or was anchored in the leaving frame (re-anchored by reanchor=True), has no covariance and
     gets NaN.  The record gains point_cov_rcond, ms_point_cov and n_map_points_without_cov; a window the call finds rank
     deficient records point_cov_rcond = nan and its message as point_cov_error, and keeps last_map_cov = None.  With
-    publish_covariance as well, the window covariance is formed twice (once per call)."""
+    publish_covariance as well, the window covariance is formed twice (once per call).
+
+    publish_odometry_covariance=True: right after GaugeRealign, next to the pose covariance and with the same gauge
+    (knots 0..3) and frame (the camera), the covariance of the relative camera pose of each consecutive keyframe pair
+    (kf[i], kf[i+1]) of the window, the odometry edges a pose graph fuses, comes from the device
+    (RelativePoseCovariance).  Unlike the absolute pose covariance it does not grow with the distance from the gauge.
+    The matrices are kept on last_rel_cov [n_frames - 1, 6, 6] and the record gains rel_cov_rcond and ms_rel_cov; a
+    window the call finds rank deficient records rel_cov_rcond = nan and its message as rel_cov_error, and keeps
+    last_rel_cov = None.  Each covariance call forms the window covariance anew."""
 
     POSE_COV_LAG_NS = 50_000_000
     POSE_COV_GAUGE_KNOT = 3
 
     def __init__(self, lib, seq, triangulate=False, device_features=False, publish_map=False, reanchor=False,
-                 publish_covariance=False, publish_map_covariance=False, **kw):
+                 publish_covariance=False, publish_map_covariance=False, publish_odometry_covariance=False, **kw):
         if device_features and not triangulate:
             raise ValueError("device_features requires triangulate=True: new landmarks enter with inverse depth -1")
         if publish_map and not device_features:
@@ -692,9 +700,11 @@ class ResidentRunner(StreamingRunner):
         self.reanchor = reanchor
         self.publish_covariance = publish_covariance
         self.publish_map_covariance = publish_map_covariance
+        self.publish_odometry_covariance = publish_odometry_covariance
         self.last_map = None
         self.last_pose_cov = None
         self.last_map_cov = None
+        self.last_rel_cov = None
         self.triangulate_probe = None
         if self.clouds is None:
             self.clouds = FrameClouds(seq)
@@ -872,6 +882,18 @@ class ResidentRunner(StreamingRunner):
                 self.last_pose_cov = None
                 pose_cov = dict(pose_cov_rcond=float("nan"), pose_cov_error=str(err))
             pose_cov["ms_pose_cov"] = 1e3 * (time.perf_counter() - t_cov)
+        rel_cov = None
+        if self.publish_odometry_covariance:           # the odometry edges between the window's keyframes, before the slide
+            t_cov = time.perf_counter()
+            try:
+                self.last_rel_cov, _, rc = e.RelativePoseCovariance(kf[:-1], kf[1:],
+                                                                    gauge_knot_index=self.POSE_COV_GAUGE_KNOT,
+                                                                    camera_frame=True)
+                rel_cov = dict(rel_cov_rcond=rc)
+            except CtvioError as err:
+                self.last_rel_cov = None
+                rel_cov = dict(rel_cov_rcond=float("nan"), rel_cov_error=str(err))
+            rel_cov["ms_rel_cov"] = 1e3 * (time.perf_counter() - t_cov)
         point_cov = lm_cov = None
         if self.publish_map_covariance:                # the covariances of the window's landmark points, before the slide
             t_cov = time.perf_counter()
@@ -933,6 +955,8 @@ class ResidentRunner(StreamingRunner):
             rec.update(pose_cov)
         if point_cov is not None:
             rec.update(point_cov)
+        if rel_cov is not None:
+            rec.update(rel_cov)
         if self.device_features:
             # n_new_lm: the window's landmarks without a depth yet (-1), which are exactly the ones TriangulateWindow wrote
             rec.update(n_triangulated=n_tri, n_fallback=n_fb, n_new_lm=n_tri + n_fb, n_removed=n_removed)

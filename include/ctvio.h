@@ -277,6 +277,33 @@ int ctvio_covariance(ctvio_handle h, double* cov_cc, double* var_rho, double* rc
  *   ctvio_transfer_stats counts 8 n bytes up and 1152 n bytes down. */
 int ctvio_pose_covariance(ctvio_handle h, int32_t n, const int64_t* t_ns, int32_t gauge_knot_index,
                           int32_t camera_frame, double* cov12, double* rcond);
+/* ctvio_relative_pose_covariance - covariance of the relative pose between two times for n pairs (t_a_ns[k],
+ *   t_b_ns[k]), the odometry edge between two keyframes, from the window covariance of ctvio_covariance (same H, same
+ *   gauge argument, same rcond test and failure mode, same absence of side effects); the np x np matrix stays on the
+ *   device.
+ *   The poses at t_a and t_b are those of ctvio_pose_covariance: of the body, or with camera_frame = 1 of the camera
+ *   (R_c = R R_CI, p_c = p + R p_CI), each perturbed as dtheta (right, R -> R Exp(dtheta)) and dp (world, additive).
+ *   The relative pose is R_ab = R_a' R_b, p_ab = R_a' (p_b - p_a), perturbed as dtheta_ab (right, R_ab -> R_ab
+ *   Exp(dtheta_ab)) and dp_ab (additive, in frame a):
+ *     dtheta_ab = dtheta_b - R_ab' dtheta_a,   dp_ab = R_a' (dp_b - dp_a) + [p_ab]x dtheta_a  (first order).
+ *   cov6[n][6][6] (row-major, exactly symmetric): the covariance of (dtheta_ab, dp_ab), G Sigma_U G' with U the union of
+ *     the knots of t_a's and t_b's segments (4 to 8 knots, not contiguous when the segments are 4 or more knots apart),
+ *     Sigma_U its block of the window covariance and G the relative-pose Jacobian with respect to those knots; a knot
+ *     of both segments has one column, the sum of both contributions.  Unlike the absolute pose covariance it does not
+ *     grow with the distance from the gauge, so it can weight an odometry edge.
+ *   cross6[n][6][6] (may be NULL): Cov((dtheta_a, dp_a), (dtheta_b, dp_b)), rows a and columns b, in the convention of
+ *     the first six rows and columns of ctvio_pose_covariance; with the two diagonal blocks of that call it gives the
+ *     joint 12 x 12 covariance of the two poses.
+ *   t_a > t_b and t_a == t_b are valid.  A pair whose knots are all constant gets exact zero matrices.
+ *   rcond (may be NULL): as ctvio_covariance; on CTVIO_ERR_STATE "rank deficient" only rcond is written.
+ *   Errors, checked before anything is launched, with nothing written: CTVIO_ERR_INVALID for a null handle, n < 0,
+ *   a NULL t_a_ns, t_b_ns or cov6 with n > 0, camera_frame not 0 or 1, gauge_knot_index outside -1 .. n_knots - 1;
+ *   CTVIO_ERR_STATE in sharded mode or before the knots are set; CTVIO_ERR_TIME_RANGE for a time
+ *   ctvio_query_trajectory does not accept.  n = 0 returns CTVIO_OK and launches nothing.
+ *   ctvio_transfer_stats counts 16 n bytes up and 288 n bytes down, 576 n with cross6. */
+int ctvio_relative_pose_covariance(ctvio_handle h, int32_t n, const int64_t* t_a_ns, const int64_t* t_b_ns,
+                                   int32_t gauge_knot_index, int32_t camera_frame, double* cov6, double* cross6,
+                                   double* rcond);
 /* ctvio_point_covariance - covariance of the world points of n anchored landmarks, from the window covariance of
  *   ctvio_covariance (same H, same gauge argument, same rcond test and failure mode, same absence of side effects);
  *   neither the np x np matrix nor the landmark couplings leave the device.
