@@ -90,6 +90,60 @@ class Summary(C.Structure):
         return d
 
 
+class ImageMsg(C.Structure):
+    """ctvio_image_msg (include/ctvio.h)."""
+
+    _fields_ = [("t_ns", C.c_int64), ("n_points", C.c_int32), ("reserved", C.c_int32)] + [
+        (n, C.c_void_p) for n in ("points_xyz", "ch_id", "ch_u", "ch_v", "ch_vx", "ch_vy")]
+
+
+class ImuMsgs(C.Structure):
+    """ctvio_imu_msgs (include/ctvio.h)."""
+
+    _fields_ = [("n", C.c_int32), ("stride_bytes", C.c_int32), ("off_gyro", C.c_int32), ("off_accel", C.c_int32),
+                ("data", C.c_void_p)]
+
+
+class CycleOptions(C.Structure):
+    """ctvio_cycle_options (include/ctvio.h)."""
+
+    _fields_ = [
+        ("window_size", C.c_int32), ("solve_iterations", C.c_int32), ("predictor_iterations", C.c_int32),
+        ("fix_ld", C.c_int32), ("min_parallax", C.c_double), ("init_depth", C.c_double), ("extend_ns", C.c_int64),
+        ("ld_lower", C.c_double), ("ld_upper", C.c_double), ("sigma_wb_discrete", C.c_double),
+        ("sigma_ab_discrete", C.c_double), ("reanchor", C.c_int32), ("publish_map", C.c_int32),
+        ("reserved", C.c_int32 * 4),
+    ]
+
+
+class CycleOutputs(C.Structure):
+    """ctvio_cycle_outputs (include/ctvio.h)."""
+
+    _fields_ = [("knot_capacity", C.c_int32), ("map_capacity", C.c_int32)] + [
+        (n, C.c_void_p) for n in ("q_xyzw", "p_xyz", "line_delay", "map_xyz", "map_feature_id", "map_in_margin_cloud",
+                                  "cam_q_xyzw", "cam_p_xyz")]
+
+
+class CycleResult(C.Structure):
+    """ctvio_cycle_result (include/ctvio.h)."""
+
+    _fields_ = [
+        ("marg_flag", C.c_int32), ("n_tracked", C.c_int32), ("parallax_num", C.c_int32), ("frame_slot", C.c_int32),
+        ("parallax_sum", C.c_double), ("n_frames", C.c_int32), ("n_knots", C.c_int32), ("knot_t0_ns", C.c_int64),
+        ("n_landmarks", C.c_int32), ("n_image_factors", C.c_int32), ("n_imu_factors", C.c_int32),
+        ("n_predictor_imu", C.c_int32), ("n_triangulated", C.c_int32), ("n_fallback", C.c_int32),
+        ("predictor", Summary), ("solve", Summary),
+        ("prior_dim", C.c_int32), ("n_removed", C.c_int32), ("n_reanchored", C.c_int32), ("n_map_points", C.c_int32),
+        ("n_margin_points", C.c_int32), ("n_knots_after", C.c_int32), ("host_ms", C.c_double),
+    ]
+
+    def as_dict(self):
+        d = {k: getattr(self, k) for k, _ in self._fields_ if k not in ("predictor", "solve")}
+        d["predictor"] = self.predictor.as_dict()
+        d["solve"] = self.solve.as_dict()
+        return d
+
+
 # every symbol include/ctvio.h declares (without prefix); used by the
 # export-completeness test and by the binder.
 ABI_SYMBOLS = [
@@ -106,7 +160,8 @@ ABI_SYMBOLS = [
     "selfcheck_solver", "nccl_unique_id", "comm_init", "triangulate_window", "check_keyframe", "slide_window_second_new",
     "feature_table_add", "feature_table_window", "triangulate_window_from_table", "add_image_features_from_table",
     "feature_table_slide", "feature_table_landmarks", "feature_table_map", "feature_table_slide_reanchor",
-    "debug_structure", "feature_table_point_covariance",
+    "debug_structure", "feature_table_point_covariance", "sync_stats", "cycle_default_options", "odometry_start",
+    "process_image", "debug_bias_weights",
 ]
 
 
@@ -119,7 +174,8 @@ DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enab
                        "slide_window_second_new", "feature_table_add", "feature_table_window", "triangulate_window_from_table",
                        "add_image_features_from_table", "feature_table_slide", "feature_table_landmarks",
                        "feature_table_map", "feature_table_slide_reanchor", "debug_structure", "covariance",
-                       "pose_covariance", "relative_pose_covariance", "point_covariance", "feature_table_point_covariance")
+                       "pose_covariance", "relative_pose_covariance", "point_covariance", "feature_table_point_covariance",
+                       "sync_stats", "cycle_default_options", "odometry_start", "process_image", "debug_bias_weights")
 
 
 def _addr(a):
@@ -613,6 +669,108 @@ class Estimator:
         a, b = C.c_int64(), C.c_int64()
         self.lib.call("transfer_stats", self.h, C.byref(a), C.byref(b), C.c_int32(int(reset)))
         return a.value, b.value
+
+    def SyncStats(self, reset=True):
+        """host waits on the device (stream synchronisations, published-scalar spins) since the last reset"""
+        a = C.c_int64()
+        self.lib.call("sync_stats", self.h, C.byref(a), C.c_int32(int(reset)))
+        return a.value
+
+    # --- the per-image odometry cycle ---------------------------------------------------------------------------
+    @staticmethod
+    def _image_msg(t_ns, message):
+        """(ImageMsg, keep-alive arrays) of a tracker message (points, id, u, v, vx, vy)"""
+        pts = np.ascontiguousarray(message[0], np.float32).reshape(-1, 3)
+        ch = [np.ascontiguousarray(x, np.float32).reshape(-1) for x in message[1:6]]
+        m = ImageMsg(t_ns=int(t_ns), n_points=pts.shape[0])
+        m.points_xyz, m.ch_id, m.ch_u, m.ch_v, m.ch_vx, m.ch_vy = (a.ctypes.data for a in [pts] + ch)
+        return m, [pts] + ch
+
+    @staticmethod
+    def _imu_msgs(records, off_gyro, off_accel):
+        if records is None:
+            return None, None
+        rec = np.ascontiguousarray(records)
+        n = rec.shape[0]
+        m = ImuMsgs(n=n, stride_bytes=rec.strides[0] if n else rec.dtype.itemsize, off_gyro=off_gyro, off_accel=off_accel,
+                    data=rec.ctypes.data if n else None)
+        return m, rec
+
+    def _cycle_outputs(self, want_knots, want_map, n_knots_cap):
+        out = CycleOutputs()
+        keep = {}
+        if want_knots:
+            keep["q"] = np.zeros((n_knots_cap, 4)); keep["p"] = np.zeros((n_knots_cap, 3)); keep["ld"] = np.zeros(1)
+            out.knot_capacity = n_knots_cap
+            out.q_xyzw, out.p_xyz, out.line_delay = keep["q"].ctypes.data, keep["p"].ctypes.data, keep["ld"].ctypes.data
+        if want_map:
+            cap = self.MAP_CAPACITY
+            keep["xyz"] = np.empty((cap, 3)); keep["ids"] = np.empty(cap, np.int32); keep["marg"] = np.empty(cap, np.uint8)
+            keep["cq"] = np.empty((16, 4)); keep["cp"] = np.empty((16, 3))
+            out.map_capacity = cap
+            out.map_xyz, out.map_feature_id, out.map_in_margin_cloud = (keep[k].ctypes.data for k in ("xyz", "ids", "marg"))
+            out.cam_q_xyzw, out.cam_p_xyz = keep["cq"].ctypes.data, keep["cp"].ctypes.data
+        return out, keep
+
+    @staticmethod
+    def _cycle_arrays(res, keep):
+        arrays = {}
+        if "q" in keep:
+            n = res.n_knots
+            arrays.update(q=keep["q"][:n].copy(), p=keep["p"][:n].copy(), line_delay=float(keep["ld"][0]))
+        if "xyz" in keep:
+            k, nf = res.n_map_points, res.n_frames - 1
+            arrays["map"] = (keep["xyz"][:k].copy(), keep["ids"][:k].copy(), keep["marg"][:k].astype(bool),
+                             keep["cq"][:nf].copy(), keep["cp"][:nf].copy())
+        return arrays
+
+    def OdometryStart(self, opt: CycleOptions, t0_ns, q, p, messages, frame_times, bg_ba, line_delay, imu_records=None,
+                      off_gyro=8, off_accel=32, marg_flag_override=-1, want_knots=True, want_map=True):
+        """ctvio_odometry_start: the initializer's window (knots from t0_ns, one tracker message and one bias node per
+        frame, the IMU records so far) solved as the first window.  Returns (result dict, arrays dict: q, p, line_delay
+        when want_knots; map = (xyz, ids, in_margin, cam_q, cam_p) when want_map)."""
+        q = _f64(q, (-1, 4)); p = _f64(p, (-1, 3)); b = _f64(bg_ba, (-1, 6))
+        msgs, keep_alive = [], []
+        for t, m in zip(frame_times, messages):
+            mm, ka = self._image_msg(t, m)
+            msgs.append(mm); keep_alive.append(ka)
+        frames = (ImageMsg * len(msgs))(*msgs)
+        imu, rec = self._imu_msgs(imu_records, off_gyro, off_accel)
+        out, keep = self._cycle_outputs(want_knots, want_map, q.shape[0])
+        res = CycleResult()
+        self.lib.call("odometry_start", self.h, C.byref(opt), C.c_int64(int(t0_ns)), C.c_int32(q.shape[0]), _dp(q), _dp(p),
+                      C.c_int32(len(msgs)), frames, _dp(b), C.c_double(line_delay), C.byref(imu) if imu is not None else None,
+                      C.c_int32(marg_flag_override), C.byref(out), C.byref(res))
+        self._after_cycle(res, opt)
+        return res.as_dict(), self._cycle_arrays(res, keep)
+
+    def ProcessImage(self, t_ns, message, imu_records=None, off_gyro=8, off_accel=32, marg_flag_override=-1,
+                     want_knots=True, want_map=True):
+        """ctvio_process_image: one image of the per-image cycle.  Returns (result dict, arrays dict) as OdometryStart."""
+        m, _ka = self._image_msg(t_ns, message)
+        imu, rec = self._imu_msgs(imu_records, off_gyro, off_accel)
+        # the extension adds at most extend_ns / dt + 1 knots
+        out, keep = self._cycle_outputs(want_knots, want_map, self.n_knots + 64)
+        res = CycleResult()
+        self.lib.call("process_image", self.h, C.byref(m), C.byref(imu) if imu is not None else None,
+                      C.c_int32(marg_flag_override), C.byref(out), C.byref(res))
+        self._after_cycle(res, None)
+        return res.as_dict(), self._cycle_arrays(res, keep)
+
+    def _after_cycle(self, res, opt):
+        # the engine's window after the slide (GetKnots / GetBiases / GetInvDepths read it)
+        self.n_knots = res.n_knots_after
+        self.n_bias = res.n_frames   # (the newest node stands for the next image)
+        self.n_lm = res.n_landmarks
+
+    def DebugBiasWeights(self, kf_times, sigma_wb, sigma_ab):
+        """(test support) the bias random-walk weights of ctvio_process_image for these keyframe times over the resident
+        IMU table: [n_kf - 1, 6]"""
+        kf = _i64(kf_times)
+        out = np.zeros((kf.shape[0] - 1, 6))
+        self.lib.call("debug_bias_weights", self.h, C.c_int32(kf.shape[0]), _lp(kf), C.c_double(sigma_wb),
+                      C.c_double(sigma_ab), _dp(out))
+        return out
 
     def DebugStructure(self):
         """the structure the engine built for the current factor set (ctvio_debug_structure), as int64 arrays: desc

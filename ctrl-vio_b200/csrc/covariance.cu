@@ -582,7 +582,7 @@ int form_covariance(ctvio_engine* e, int gauge_knot, const char* who, double* rc
   rc = read_scalars(e, true);
   const double rc_value = const_cast<const LmPublished*>(e->h_pub)->rcond;
   const bool failed = e->h_scal->chol_fail != 0;
-  CUDA_OK(cudaStreamSynchronize(st));  // (the restore behind the published block)
+  CUDA_OK(stream_sync(st));  // (the restore behind the published block)
   if (rc) return rc;
   if (rcond) *rcond = rc_value;
   // Ceres' default min_reciprocal_condition_number; the estimate is the pivot ratio, see include/ctvio.h
@@ -616,7 +616,7 @@ int point_covariance(ctvio_engine* e, PointCovLaunch& a, double* cov9) {
   e->launches += launch_point_cov(a, st);
   CUDA_OK(cudaMemcpyAsync(cov9, w.pose.p, 9 * size_t(a.n) * sizeof(double), cudaMemcpyDeviceToHost, st));
   e->d2h_bytes += 9 * size_t(a.n) * sizeof(double);
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   return CTVIO_OK;
 }
 
@@ -639,7 +639,7 @@ extern "C" int ctvio_covariance(ctvio_handle e, double* cov_cc, double* var_rho,
     CUDA_OK(cudaMemcpyAsync(var_rho, w.var.p, nL * sizeof(double), cudaMemcpyDeviceToHost, st));
     e->d2h_bytes += nL * sizeof(double);
   }
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   return CTVIO_OK;
 }
 
@@ -679,7 +679,7 @@ extern "C" int ctvio_pose_covariance(ctvio_handle e, int32_t n, const int64_t* t
   e->launches += launch_pose_cov(a, st);
   CUDA_OK(cudaMemcpyAsync(cov12, w.pose.p, 144 * size_t(n) * sizeof(double), cudaMemcpyDeviceToHost, st));
   e->d2h_bytes += 144 * size_t(n) * sizeof(double);
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   return CTVIO_OK;
 }
 
@@ -728,7 +728,7 @@ extern "C" int ctvio_relative_pose_covariance(ctvio_handle e, int32_t n, const i
   CUDA_OK(cudaMemcpyAsync(cov6, a.out, 36 * nn * sizeof(double), cudaMemcpyDeviceToHost, st));
   if (cross6) CUDA_OK(cudaMemcpyAsync(cross6, a.cross, 36 * nn * sizeof(double), cudaMemcpyDeviceToHost, st));
   e->d2h_bytes += n_out * nn * sizeof(double);
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   return CTVIO_OK;
 }
 

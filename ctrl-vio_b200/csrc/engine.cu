@@ -272,7 +272,18 @@ int prepare(ctvio_engine* e) {
       for (int c = 0; c < 6; ++c) bs[6 * k + c] = o.s[c];
     }
     CUDA_OK(e->d_bf_ij.upload(bij, st));
-    CUDA_OK(e->d_bf_s.upload(bs, st));
+    if (e->n_bf_dev == 0) {
+      CUDA_OK(e->d_bf_s.upload(bs, st));
+    } else {
+      // rows on the device are copied there; only the host-recorded rows after them go up
+      const size_t nd = 6 * size_t(e->n_bf_dev), nh = bs.size() - nd;
+      CUDA_OK(e->d_bf_s.reserve(bs.size()));
+      CUDA_OK(cudaMemcpyAsync(e->d_bf_s.p, e->bf_s_dev, nd * sizeof(double), cudaMemcpyDeviceToDevice, st));
+      if (nh) {
+        CUDA_OK(staged_h2d(e->d_bf_s.p + nd, bs.data() + nd, nh * sizeof(double), st));
+        g_upload_bytes += nh * sizeof(double);
+      }
+    }
 
     // ---- buffers ----
     const size_t np = size_t(d.np);
@@ -466,7 +477,7 @@ int fetch_new_prior(ctvio_engine* e) {
   CUDA_OK(cudaMemcpyAsync(np_.J.data(), e->mws.J.p, np_.J.size() * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
   CUDA_OK(cudaMemcpyAsync(np_.r.data(), e->mws.r.p, np_.r.size() * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
   CUDA_OK(cudaMemcpyAsync(np_.x0.data(), e->d_newprior_x0.p, np_.x0.size() * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
-  CUDA_OK(cudaStreamSynchronize(e->stream));
+  CUDA_OK(stream_sync(e->stream));
   e->d2h_bytes += (np_.J.size() + np_.r.size() + np_.x0.size()) * sizeof(double);
   e->new_prior_on_host = true;
   return CTVIO_OK;
@@ -612,13 +623,14 @@ void reset_tickets(ctvio_engine* e) {
 // mapped host memory with sequence number e->pub_seq: spin on it instead of copy + stream synchronise
 int read_scalars(ctvio_engine* e, bool published) {
   if (published) {
+    ++g_host_waits;
     volatile unsigned long long* seq = &e->h_pub->seq;
     unsigned spins = 0;
     while (*seq != e->pub_seq) {
       if ((++spins & 0xfffu) == 0 && cudaStreamQuery(e->stream) != cudaErrorNotReady) {
         if (*seq == e->pub_seq) break;
-        CUDA_OK(cudaStreamSynchronize(e->stream));
-        CUDA_OK(cudaStreamSynchronize(e->stream2));  // (the factor kernels forked onto stream2 are settled too)
+        CUDA_OK(stream_sync(e->stream));
+        CUDA_OK(stream_sync(e->stream2));  // (the factor kernels forked onto stream2 are settled too)
         if (*seq != e->pub_seq) return fail(CTVIO_ERR_CUDA, "LM step finished without publishing its scalars");
       }
     }
@@ -626,12 +638,47 @@ int read_scalars(ctvio_engine* e, bool published) {
     *e->h_scal = const_cast<const LmPublished*>(e->h_pub)->s;
   } else {
     CUDA_OK(cudaMemcpyAsync(e->h_scal, e->d_scal.p, sizeof(LmScalars), cudaMemcpyDeviceToHost, e->stream));
-    CUDA_OK(cudaStreamSynchronize(e->stream));
+    CUDA_OK(stream_sync(e->stream));
   }
   if ((e->h_scal->error_flags & 1) || (e->world > 1 && e->h_scal->err_sum > 0.0)) {
     cudaMemsetAsync(&e->d_scal.p->error_flags, 0, sizeof(int32_t), e->stream);
     return fail(CTVIO_ERR_TIME_RANGE, "a factor time left its knot window / the spline (line delay too large?)");
   }
+  return CTVIO_OK;
+}
+
+int add_bias_factors_device(ctvio_engine* e, int n, const int32_t* ni, const int32_t* nj, const double* d_s6,
+                            const int32_t* marg) {
+  if (int(e->biasf.size()) != e->n_bf_dev) return fail(CTVIO_ERR_STATE, "bias factors with host weights are already present");
+  for (int k = 0; k < n; ++k)
+    e->biasf.push_back(HostBias{ni[k], nj[k], {0, 0, 0, 0, 0, 0}, marg ? marg[k] : 0});  // weights: d_s6 row k
+  e->bf_s_dev = d_s6;
+  e->n_bf_dev += n;
+  e->structure_dirty = true;
+  return CTVIO_OK;
+}
+
+// ctvio_adopt_prior.  keep_new_prior: the marginalization's buffers are copied device-to-device instead of handed over,
+// so that ctvio_get_prior still returns the prior just produced (the odometry cycle)
+int adopt_prior_body(ctvio_engine* e, bool keep_new_prior) {
+  // only the block bookkeeping (a few dozen ints) lives on the host
+  e->prior.n = e->new_prior.n;
+  e->prior.type = e->new_prior.type; e->prior.index = e->new_prior.index; e->prior.col = e->new_prior.col;
+  e->prior.J.clear(); e->prior.r.clear(); e->prior.x0.clear();
+  if (keep_new_prior) {
+    const size_t n = size_t(e->new_prior.n), nb = e->new_prior.type.size();
+    CUDA_OK(e->d_prior_J.reserve(n * n)); CUDA_OK(e->d_prior_r.reserve(n)); CUDA_OK(e->d_prior_x0.reserve(4 * nb));
+    CUDA_OK(cudaMemcpyAsync(e->d_prior_J.p, e->mws.J.p, n * n * sizeof(double), cudaMemcpyDeviceToDevice, e->stream));
+    CUDA_OK(cudaMemcpyAsync(e->d_prior_r.p, e->mws.r.p, n * sizeof(double), cudaMemcpyDeviceToDevice, e->stream));
+    CUDA_OK(cudaMemcpyAsync(e->d_prior_x0.p, e->d_newprior_x0.p, 4 * nb * sizeof(double), cudaMemcpyDeviceToDevice, e->stream));
+  } else {
+    // the buffers of the marginalization workspace BECOME the active prior (pointer swap)
+    swap(e->d_prior_J, e->mws.J); swap(e->d_prior_r, e->mws.r); swap(e->d_prior_x0, e->d_newprior_x0);
+    e->new_prior = ctvio::PriorHost();  // its device buffers are gone
+  }
+  e->prior_on_device = true;
+  e->prior_dirty = true;
+  e->masks_dirty = true;
   return CTVIO_OK;
 }
 
@@ -705,7 +752,7 @@ int ctvio_create(const ctvio_config* cfg, ctvio_handle* out) {
 int ctvio_destroy(ctvio_handle e) {
   if (!e) return CTVIO_OK;
   cudaSetDevice(e->cfg.device);
-  cudaStreamSynchronize(e->stream);
+  stream_sync(e->stream);
   ctvio::comm_destroy(e->nccl_comm);
   if (e->h_scal) cudaFreeHost(e->h_scal);
   if (e->h_pub) cudaFreeHost(e->h_pub);
@@ -816,7 +863,7 @@ int ctvio_get_knots(ctvio_handle e, double* q, double* p) {
     p4.resize(kPStride * size_t(e->nK));
     CUDA_OK(cudaMemcpyAsync(p4.data(), e->x[e->cur].p.p, p4.size() * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
   }
-  CUDA_OK(cudaStreamSynchronize(e->stream));
+  CUDA_OK(stream_sync(e->stream));
   if (p) for (int k = 0; k < e->nK; ++k) for (int c = 0; c < 3; ++c) p[3 * k + c] = p4[kPStride * k + c];
   return CTVIO_OK;
 }
@@ -829,7 +876,7 @@ int ctvio_get_biases(ctvio_handle e, double* b) {
     return CTVIO_OK;
   }
   if (e->nB > 0) CUDA_OK(cudaMemcpyAsync(b, e->x[e->cur].bias.p, 6 * size_t(e->nB) * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
-  CUDA_OK(cudaStreamSynchronize(e->stream));
+  CUDA_OK(stream_sync(e->stream));
   return CTVIO_OK;
 }
 int ctvio_get_inv_depths(ctvio_handle e, double* r) {
@@ -841,7 +888,7 @@ int ctvio_get_inv_depths(ctvio_handle e, double* r) {
     return CTVIO_OK;
   }
   if (e->nL > 0) CUDA_OK(cudaMemcpyAsync(r, e->x[e->cur].rho.p, size_t(e->nL) * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
-  CUDA_OK(cudaStreamSynchronize(e->stream));
+  CUDA_OK(stream_sync(e->stream));
   return CTVIO_OK;
 }
 int ctvio_get_line_delay(ctvio_handle e, double* ld) {
@@ -852,7 +899,7 @@ int ctvio_get_line_delay(ctvio_handle e, double* ld) {
     return CTVIO_OK;
   }
   CUDA_OK(cudaMemcpyAsync(ld, e->x[e->cur].ld.p, sizeof(double), cudaMemcpyDeviceToHost, e->stream));
-  CUDA_OK(cudaStreamSynchronize(e->stream));
+  CUDA_OK(stream_sync(e->stream));
   return CTVIO_OK;
 }
 
@@ -861,6 +908,7 @@ int ctvio_clear_factors(ctvio_handle e) {
   e->img.clear(); e->imu.clear(); e->biasf.clear();
   e->img_desc.clear(); e->imu_src.clear();
   e->n_img_dev = 0;
+  e->n_bf_dev = 0;
   e->structure_dirty = true;
   return CTVIO_OK;
 }
@@ -952,7 +1000,7 @@ int ctvio_gauge_realign(ctvio_handle e, int32_t min_idx, const double* R0, const
     const int rcm = refresh_mirror(e);
     if (rcm) return rcm;
   }
-  CUDA_OK(cudaStreamSynchronize(e->stream));
+  CUDA_OK(stream_sync(e->stream));
   e->table_valid = true;
   return CTVIO_OK;
 }
@@ -1173,7 +1221,7 @@ int ctvio_profile_kernels(ctvio_handle e, int32_t reps, int32_t flush_l2, double
     }
     out[0] = total / reps;
     cudaMemsetAsync(&e->d_scal.p->error_flags, 0, sizeof(int32_t), st);
-    CUDA_OK(cudaStreamSynchronize(st));
+    CUDA_OK(stream_sync(st));
     return CTVIO_OK;
   }
   // a valid linearisation + step so that every stage has meaningful inputs
@@ -1241,7 +1289,7 @@ int ctvio_profile_kernels(ctvio_handle e, int32_t reps, int32_t flush_l2, double
   rc = time_stage(6, &out[6]);
   if (rc) return rc;
   cudaMemsetAsync(&e->d_scal.p->error_flags, 0, sizeof(int32_t), st);
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   return CTVIO_OK;
 }
 
@@ -1269,7 +1317,7 @@ int ctvio_selfcheck_solver(ctvio_handle e, int32_t reps, int32_t* mismatches, do
     if (r > 0) CUDA_OK(cudaMemcpyAsync(lin.M, backup.p, len * sizeof(double), cudaMemcpyDeviceToDevice, st));
     launch_factor_solve(lin, st);
     CUDA_OK(cudaMemcpyAsync((r == 0 ? x0 : x).data(), lin.y, n * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CUDA_OK(cudaStreamSynchronize(st));
+    CUDA_OK(stream_sync(st));
     if (r > 0 && std::memcmp(x.data(), x0.data(), n * sizeof(double)) != 0) ++*mismatches;
   }
   // residual of the first solve against the host copy (only the lower triangle of M is maintained by K4)
@@ -1285,7 +1333,7 @@ int ctvio_selfcheck_solver(ctvio_handle e, int32_t reps, int32_t* mismatches, do
   }
   *rel_residual = bmax > 0 ? rmax / bmax : rmax;
   cudaMemsetAsync(&e->d_scal.p->error_flags, 0, sizeof(int32_t), st);
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   return CTVIO_OK;
 }
 
@@ -1341,10 +1389,10 @@ int ctvio_debug_lm_step_poison(ctvio_handle e, double radius, double* out, int64
   // (pageable destinations: each copy has completed when it returns, so M and rhs are taken before K5 runs)
   CUDA_OK(cudaMemcpyAsync(M, lin.M, npad * npad * sizeof(double), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaMemcpyAsync(rhs, lin.rhs, npad * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   launch_factor_solve(lin, st);
   CUDA_OK(cudaMemcpyAsync(y, lin.y, npad * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   launch_step_vectors(lin, st);
   const NormalEqPtrs ne = e->ne(cur);
   std::vector<double> Wc(size_t(e->w_len)), wld(nL);
@@ -1370,7 +1418,7 @@ int ctvio_debug_lm_step_poison(ctvio_handle e, double radius, double* out, int64
   }
   CUDA_OK(cudaMemcpyAsync(e->h_scal, e->d_scal.p, sizeof(LmScalars), cudaMemcpyDeviceToHost, st));
   cudaMemsetAsync(&e->d_scal.p->error_flags, 0, sizeof(int32_t), st);
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   std::memset(W, 0, nL * np * sizeof(double));
   for (size_t l = 0; l < nL; ++l) {
     for (int g = lo[l]; g < hi[l]; ++g) W[l * np + g] = Wc[size_t(woff[l]) + (g - lo[l])];
@@ -1501,8 +1549,11 @@ int ctvio_marginalize(ctvio_handle e, int32_t* n_out, int32_t* nb_out) {
   }
   std::vector<int2> bij;
   std::vector<double> bs;
-  for (const HostBias& o : e->biasf) {  // [4] bias factors (:280-285), drop {bg_i, ba_i}
+  std::vector<int2> bs_dev;  // (row of bs, device row) of the marginalized factors whose weights live on the device
+  for (size_t k = 0; k < e->biasf.size(); ++k) {  // [4] bias factors (:280-285), drop {bg_i, ba_i}
+    const HostBias& o = e->biasf[k];
     if (!o.marg) continue;
+    if (int(k) < e->n_bf_dev) bs_dev.push_back(make_int2(int(bij.size()), int(k)));
     bij.push_back(make_int2(o.i, o.j));
     for (int c = 0; c < 6; ++c) bs.push_back(o.s[c]);
     touch(CTVIO_BLK_BG, o.i, true); touch(CTVIO_BLK_BG, o.j, false);
@@ -1550,6 +1601,9 @@ int ctvio_marginalize(ctvio_handle e, int32_t* n_out, int32_t* nb_out) {
   CUDA_OK(d_marg_imu.upload(marg_imu, st));
   CUDA_OK(d_bij.upload(bij, st));
   CUDA_OK(d_bs.upload(bs, st));
+  for (const int2 r : bs_dev)
+    CUDA_OK(cudaMemcpyAsync(d_bs.p + 6 * size_t(r.x), e->bf_s_dev + 6 * size_t(r.y), 6 * sizeof(double),
+                            cudaMemcpyDeviceToDevice, st));
   CUDA_OK(d_A.reserve(size_t(P) * P));
   CUDA_OK(d_b.reserve(P));
   {
@@ -1645,7 +1699,7 @@ int ctvio_marginalize(ctvio_handle e, int32_t* n_out, int32_t* nb_out) {
     CUDA_OK(d_i.upload(np_.index, st));
     CUDA_OK(e->d_newprior_x0.reserve(4 * np_.type.size()));
     e->launches += ctvio::launch_prior_x0(e->x[e->cur].ptrs(), d_t.p, d_i.p, int(np_.type.size()), e->d_newprior_x0.p, st);
-    CUDA_OK(cudaStreamSynchronize(st));  // the uploads above come from host vectors that are reused by the next call
+    CUDA_OK(stream_sync(st));  // the uploads above come from host vectors that are reused by the next call
   }
   *n_out = n;
   *nb_out = int32_t(np_.type.size());
@@ -1672,17 +1726,7 @@ int ctvio_adopt_prior(ctvio_handle e) {
   if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
   if (e->new_prior.n <= 0) return fail(CTVIO_ERR_STATE, "no prior has been produced");
   cudaSetDevice(e->cfg.device);
-  // device-to-device: the buffers of the marginalization workspace BECOME the active prior (pointer swap), only the
-  // block bookkeeping (a few dozen ints) lives on the host
-  e->prior.n = e->new_prior.n;
-  e->prior.type = e->new_prior.type; e->prior.index = e->new_prior.index; e->prior.col = e->new_prior.col;
-  e->prior.J.clear(); e->prior.r.clear(); e->prior.x0.clear();
-  swap(e->d_prior_J, e->mws.J); swap(e->d_prior_r, e->mws.r); swap(e->d_prior_x0, e->d_newprior_x0);
-  e->prior_on_device = true;
-  e->new_prior = ctvio::PriorHost();  // its device buffers are gone
-  e->prior_dirty = true;
-  e->masks_dirty = true;
-  return CTVIO_OK;
+  return adopt_prior_body(e, false);
 }
 
 int ctvio_set_deterministic(ctvio_handle e, int32_t on) {
@@ -1697,6 +1741,13 @@ int ctvio_enable_prior(ctvio_handle e, int32_t on) {
   if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
   if (e->prior_enabled != (on != 0)) e->masks_dirty = true;
   e->prior_enabled = on != 0;
+  return CTVIO_OK;
+}
+
+int ctvio_sync_stats(ctvio_handle e, int64_t* host_waits, int32_t reset) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (host_waits) *host_waits = g_host_waits;
+  if (reset) g_host_waits = 0;
   return CTVIO_OK;
 }
 

@@ -26,6 +26,14 @@ inline int fail(int code, const std::string& msg) {
       return fail(CTVIO_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_));                  \
   } while (0)
 
+// host waits on the device by this thread's C-ABI calls (stream synchronisations and spins on the LM step's published
+// scalars), see ctvio_sync_stats
+inline thread_local int64_t g_host_waits = 0;
+inline cudaError_t stream_sync(cudaStream_t s) {
+  ++g_host_waits;
+  return cudaStreamSynchronize(s);
+}
+
 inline thread_local size_t g_upload_bytes = 0;  // bytes moved by DevBuf::upload (index tables etc.), see ctvio_transfer_stats
 
 // Pinned staging arena of one engine: every host -> device copy of a C-ABI call is staged here and issued as a truly
@@ -87,7 +95,7 @@ struct DevBuf {
     DevBuf<T> nb;
     cudaError_t e = nb.reserve(n);
     if (e == cudaSuccess && count) e = cudaMemcpyAsync(nb.p, p + from, count * sizeof(T), cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) e = stream_sync(s);
     if (e == cudaSuccess) swap(*this, nb);
     return e;
   }
@@ -172,6 +180,10 @@ struct ctvio_engine {
   int n_imu_items = 0;
   DevBuf<int2> d_bf_ij;
   DevBuf<double> d_bf_s;
+  // the first n_bf_dev bias factors of the set take their sqrt_info6 rows from bf_s_dev (device memory, row k for factor
+  // k) instead of their host record: the odometry cycle's weights never leave the device
+  const double* bf_s_dev = nullptr;
+  int n_bf_dev = 0;
 
   // landmark layout / schur batches
   std::vector<int32_t> h_lo, h_hi;
@@ -281,6 +293,19 @@ struct ctvio_engine {
     DevBuf<int64_t> t;
     DevBuf<int32_t> lm;
   } cws;
+  // the per-image odometry cycle (odometry.cu): the window's frames and the bookkeeping a caller of the separate entry
+  // points keeps itself
+  struct Cycle {
+    bool started = false;
+    ctvio_cycle_options opt{};
+    int32_t slot[16] = {0};        // window position -> frame slot, oldest to newest
+    int64_t t[16] = {0};           // window position -> frame time
+    int n_frames = 0;
+    int64_t next_frame = 0;        // number of frames the cycle has taken in (the allocator's f)
+    DevBuf<double> bias_w;         // [n_frames - 1][6] bias random-walk weights of the current window
+    DevBuf<double> imu_carry;      // {prefix of dt^2 at the last sample ingested, its time (int64 bits), valid}
+    DevBuf<double> snap;           // local knot 0 before the main solve: q (4), p (3), then R0 / t0 (12)
+  } cyc;
   int n_marg_img = -1;  // marginalized image factors of the last ctvio_marginalize (-1: pos_cam / pos_lm / marg_img not built)
 
   // multi-GPU
@@ -344,5 +369,13 @@ int read_scalars(ctvio_engine* e, bool published = false);
 LinearLaunch linear_launch(ctvio_engine* e, int nb);
 int refresh_mirror(ctvio_engine* e);
 int alloc_state(ctvio_engine* e, DevState& s);
+// bodies of entry points the odometry cycle (odometry.cu) runs without their trailing stream synchronisation
+int add_bias_factors_device(ctvio_engine* e, int n, const int32_t* ni, const int32_t* nj, const double* d_sqrt_info6,
+                            const int32_t* marg);
+int adopt_prior_body(ctvio_engine* e, bool keep_new_prior);
+int ingest_feature_cloud_body(ctvio_engine* e, int32_t slot, int64_t t_ns, int32_t n, const float* points, const float* ch_id,
+                              const float* ch_v, bool sync);
+int ingest_imu_body(ctvio_engine* e, int32_t n, const void* records, int32_t stride, int32_t off_gyro, int32_t off_accel,
+                    int64_t drop_before_ns, bool sync, int* first_new);
 
 }  // namespace ctvio::host

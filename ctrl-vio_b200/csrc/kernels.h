@@ -460,6 +460,10 @@ int launch_apply_step(const ApplyLaunch& a, cudaStream_t s, bool reset = true);
 // step vectors + full step (alpha = 1) applied in one launch; the per-step accumulators must already be zero
 int launch_step_and_apply(const LinearLaunch& a, const ApplyLaunch& ap, cudaStream_t s);
 int launch_gauge_realign(const StatePtrs& st, int nK, int min_idx, const double* R0_t0_dev, cudaStream_t s);
+// ctvio_gauge_realign with R0 / t0 formed on the device from snap_dev = the knot's q (4), p (3) before the solve (the
+// odometry cycle); the R0 / t0 it used go to R0_t0_out (12)
+int launch_gauge_realign_snapshot(const StatePtrs& st, int nK, int min_idx, const double* snap_dev, double* R0_t0_out,
+                                  cudaStream_t s);
 
 struct QueryLaunch {
   StatePtrs st;

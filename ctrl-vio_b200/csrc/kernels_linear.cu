@@ -691,7 +691,7 @@ __device__ void r2ypr_deg(const M3& R, double ypr[3]) {
   ypr[0] = y * k; ypr[1] = p * k; ypr[2] = r * k;
 }
 
-__global__ void gauge_realign_kernel(StatePtrs st, int nK, int min_idx, const double* R0t0) {
+__device__ __forceinline__ void gauge_realign_apply(StatePtrs st, int nK, int min_idx, const double* R0t0) {
   __shared__ double T[16];  // qd (4), tran_diff (3)
   if (threadIdx.x == 0) {
     M3 R0;
@@ -721,8 +721,44 @@ __global__ void gauge_realign_kernel(StatePtrs st, int nK, int min_idx, const do
   }
 }
 
+__global__ void gauge_realign_kernel(StatePtrs st, int nK, int min_idx, const double* R0t0) {
+  gauge_realign_apply(st, nK, min_idx, R0t0);
+}
+
+// numpy's cross(a, b) component c: each product rounded, then the difference (no contraction)
+__device__ __forceinline__ double np_cross(const double* a, const double* b, int c) {
+  const int i = (c + 1) % 3, j = (c + 2) % 3;
+  return __dsub_rn(__dmul_rn(a[i], b[j]), __dmul_rn(a[j], b[i]));
+}
+
+// The realignment of the odometry cycle: R0 / t0 formed on the device from the snapshot q (4), p (3) of the knot taken
+// before the solve, with the operations of the host's R0 = qrot(q, I).T (synthetic.py, numpy): column j of R is
+// v + w uv + qv x uv, uv = 2 (qv x v), v = e_j.  R0t0_out receives R0 (row-major) and t0 (12 doubles).
+__global__ void gauge_realign_snapshot_kernel(StatePtrs st, int nK, int min_idx, const double* snap, double* R0t0_out) {
+  __shared__ double R0t0[12];
+  if (threadIdx.x == 0) {
+    const double qv[3] = {snap[0], snap[1], snap[2]}, w = snap[3];
+    for (int j = 0; j < 3; ++j) {
+      const double v[3] = {j == 0 ? 1.0 : 0.0, j == 1 ? 1.0 : 0.0, j == 2 ? 1.0 : 0.0};
+      double uv[3];
+      for (int c = 0; c < 3; ++c) uv[c] = __dmul_rn(2.0, np_cross(qv, v, c));
+      for (int c = 0; c < 3; ++c) R0t0[3 * c + j] = __dadd_rn(__dadd_rn(v[c], __dmul_rn(w, uv[c])), np_cross(qv, uv, c));
+    }
+    for (int c = 0; c < 3; ++c) R0t0[9 + c] = snap[4 + c];
+    for (int k = 0; k < 12; ++k) R0t0_out[k] = R0t0[k];
+  }
+  __syncthreads();
+  gauge_realign_apply(st, nK, min_idx, R0t0);
+}
+
 int launch_gauge_realign(const StatePtrs& st, int nK, int min_idx, const double* R0_t0_dev, cudaStream_t s) {
   gauge_realign_kernel<<<1, 256, 0, s>>>(st, nK, min_idx, R0_t0_dev);
+  return 1 + launch_knot_table(st, nK, s);
+}
+
+int launch_gauge_realign_snapshot(const StatePtrs& st, int nK, int min_idx, const double* snap_dev, double* R0_t0_out,
+                                  cudaStream_t s) {
+  gauge_realign_snapshot_kernel<<<1, 256, 0, s>>>(st, nK, min_idx, snap_dev, R0_t0_out);
   return 1 + launch_knot_table(st, nK, s);
 }
 

@@ -43,7 +43,7 @@ int shard_consensus(ctvio_engine* e, int local_rc) {
   std::string err;
   if (!ctvio::comm_allreduce_sum(e->nccl_comm, e->d_tmp.p, 1, st, &err)) return fail(CTVIO_ERR_NCCL, err);
   CUDA_OK(cudaMemcpyAsync(&total, e->d_tmp.p, sizeof(double), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   if (local_rc) return fail(local_rc, local_msg);
   if (total != 0.0) return fail(CTVIO_ERR_STATE, "another rank of the sharded solve failed before the first collective");
   return CTVIO_OK;
@@ -63,7 +63,7 @@ int shard_check_ownership(ctvio_engine* e) {
   std::string err;
   if (!ctvio::comm_allreduce_sum(e->nccl_comm, e->d_rho_sync.p, owned.size(), st, &err)) return fail(CTVIO_ERR_NCCL, err);
   CUDA_OK(cudaMemcpyAsync(owned.data(), e->d_rho_sync.p, owned.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   for (int l = 0; l < e->nL; ++l)
     if (owned[l] > 1.0)
       return fail(CTVIO_ERR_INVALID, "sharded solve: landmark " + std::to_string(l) + " has observations on " +
@@ -244,7 +244,7 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
   if (is_constrained) {  // IterationZero: x = Plus(x, 0) projects the line delay into its bounds
     double ld;
     CUDA_OK(cudaMemcpyAsync(&ld, e->x[e->cur].ld.p, sizeof(double), cudaMemcpyDeviceToHost, st));
-    CUDA_OK(cudaStreamSynchronize(st));
+    CUDA_OK(stream_sync(st));
     const double c = std::min(std::max(ld, e->opt.ld_lower), e->opt.ld_upper);
     if (c != ld) CUDA_OK(cudaMemcpyAsync(e->x[e->cur].ld.p, &c, sizeof(double), cudaMemcpyHostToDevice, st));
   }
@@ -441,7 +441,7 @@ int ctvio_solve(ctvio_handle e, int32_t max_iterations, ctvio_summary* out) {
   cudaEventRecord(e->ev1, st);
   rc = refresh_mirror(e);  // state -> pinned host mirror, rides on the synchronisation below
   if (rc) return rc;
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   float ms = 0;
   cudaEventElapsedTime(&ms, e->ev0, e->ev1);
   sum.iterations = iter;

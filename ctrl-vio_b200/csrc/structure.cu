@@ -473,7 +473,7 @@ int structure_build_device(ctvio_engine* e, int T) {
   std::vector<uint32_t>& c = e->h_struct_counts;
   c.assign(kHdrWords + words, 0);
   CUDA_OK(cudaMemcpyAsync(c.data(), a.counts, c.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   e->d2h_bytes += c.size() * sizeof(uint32_t);
   if (c[kErr]) {
     const uint32_t code = c[kErr] - 1u;
@@ -527,7 +527,7 @@ int marg_discover_device(ctvio_engine* e, std::vector<uint32_t>& knots, int& n_m
   e->launches += 1;
   std::vector<uint32_t> c(2 + words);
   CUDA_OK(cudaMemcpyAsync(c.data(), a.counts, c.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   e->d2h_bytes += c.size() * sizeof(uint32_t);
   n_marg = int(c[0]);
   n_rho = int(c[1]);
@@ -584,7 +584,7 @@ extern "C" int ctvio_debug_structure(ctvio_handle e, int64_t* out, int64_t* len)
   CUDA_OK(get(sitems, e->d_schur_items.p)); CUDA_OK(get(entries, e->d_schur_list.p)); CUDA_OK(get(active, e->d_active.p));
   CUDA_OK(get(pos_cam, e->mws.pos_cam.p)); CUDA_OK(get(pos_lm, e->mws.pos_lm.p)); CUDA_OK(get(marg, e->mws.marg_img.p));
   CUDA_OK(get(imu_items, e->d_imu_items.p));
-  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(stream_sync(st));
   std::memset(out, 0, 16 * sizeof(int64_t));
   out[0] = int64_t(n); out[1] = int64_t(n_desc); out[2] = int64_t(ni); out[3] = int64_t(nL); out[4] = int64_t(nsi);
   out[5] = int64_t(ne); out[6] = int64_t(np); out[7] = e->n_marg_img; out[8] = int64_t(nii);

@@ -1019,4 +1019,137 @@ class ResidentRunner(StreamingRunner):
         return b
 
 
+class CycleRunner:
+    """ResidentRunner(triangulate=True, device_features=True) through the library's per-image cycle: window 0 is one
+    ctvio_odometry_start, every later window one ctvio_process_image, fed with the sequence's clouds and IMU records.
+    The frame slots, the window's frames, the knot range of each frame and the bias nodes are the library's; the runner
+    only keeps what a caller publishes: the trajectory (q, p, ld), the records and the last map.
+
+    Options as ResidentRunner's: second_new_every (through marg_flag_override), min_parallax (the device's keyframe
+    decision), publish_map, reanchor, iters / init_iters.  want_knots / want_map=False leave the knot / map outputs
+    unrequested (the trajectory is then not carried into q / p, and last_map stays None).  Not supported: the host
+    association (device_features=False), the rho0 mode (triangulate=False), predictor=False, the covariance
+    publications and a perm_seed."""
+
+    def __init__(self, lib, seq, iters=15, init_iters=8, device=0, second_new_every=0, min_parallax=None,
+                 publish_map=False, reanchor=False, want_knots=True, want_map=True, triangulate=True,
+                 device_features=True, predictor=True, perm_seed=None, publish_covariance=False,
+                 publish_map_covariance=False, publish_odometry_covariance=False):
+        from . import binding, make_config
+        if not triangulate or not device_features:
+            raise ValueError("CycleRunner runs the device feature table with triangulation only "
+                             "(triangulate=True, device_features=True)")
+        if not predictor:
+            raise ValueError("CycleRunner always runs the IMU predictor (predictor=True)")
+        if perm_seed is not None:
+            raise ValueError("CycleRunner takes the factors from the resident tables: no perm_seed")
+        if publish_covariance or publish_map_covariance or publish_odometry_covariance:
+            raise ValueError("CycleRunner does not publish covariances: use ResidentRunner or the separate calls")
+        if min_parallax is not None and second_new_every:
+            raise ValueError("min_parallax and second_new_every both choose the branch: pick one")
+        if min_parallax is not None and not min_parallax > 0:
+            raise ValueError("min_parallax must be > 0 (None: every image is a keyframe)")
+        self.lib, self.seq = lib, seq
+        self.second_new_every = second_new_every
+        self.want_knots, self.want_map = want_knots, want_map and publish_map
+        s = seq
+        self.clouds = FrameClouds(seq)
+        self.frames = list(range(WIN_KF))
+        self.next_frame = WIN_KF
+        self.q = s.q0.copy(); self.p = s.p0.copy(); self.ld = s.ld0
+        self.bias = s.bias0.copy()
+        self.ncp = StreamingRunner._cp_needed(self, int(s.kf_times[WIN_KF - 1]) + EXTEND_NS)
+        self.est = Estimator(lib, make_config(device=device, **s.config_kwargs()))
+        self.opt = binding.CycleOptions()
+        lib.call("cycle_default_options", C_byref(self.opt))
+        self.opt.window_size = WINDOW_SIZE
+        self.opt.solve_iterations = iters
+        self.opt.predictor_iterations = init_iters
+        self.opt.min_parallax = 0.0 if min_parallax is None else float(min_parallax)
+        self.opt.extend_ns = EXTEND_NS
+        self.opt.ld_lower, self.opt.ld_upper = 0.0, syn.LD_UPPER
+        self.opt.sigma_wb_discrete, self.opt.sigma_ab_discrete = syn.SIGMA_BG, syn.SIGMA_BA
+        self.opt.reanchor = int(reanchor)
+        self.opt.publish_map = int(publish_map)
+        self.reanchor, self.publish_map = reanchor, publish_map
+        self.last_map = None
+        self.records = []
+        self.step_index = 0
+        self.imu_sent = 0
+
+    def _override(self):
+        """the second_new_every rule of StreamingRunner, or -1 (the device decides)"""
+        n = self.second_new_every
+        if not n:
+            return -1
+        return MARGIN_SECOND_NEW if (self.frames[-2] % n) == n - 1 else MARGIN_OLD
+
+    def _imu_records(self, t_newest):
+        s = self.seq
+        hi = int(np.searchsorted(s.imu_t, t_newest, side="right"))
+        lo, self.imu_sent = self.imu_sent, max(hi, self.imu_sent)
+        return ResidentRunner._imu_records(self, lo, hi) if hi > lo else None
+
+    def step(self, k=None):
+        s, e = self.seq, self.est
+        first = self.step_index == 0
+        if not first:
+            self.frames.append(self.next_frame)
+            self.next_frame += 1
+        t_newest = int(s.kf_times[self.frames[-1]])
+        imu = self._imu_records(t_newest)
+        e.TransferStats(reset=True)
+        t0 = time.perf_counter()
+        if first:
+            f = self.frames
+            res, arr = e.OdometryStart(self.opt, s.t0_ns, self.q[:self.ncp], self.p[:self.ncp],
+                                       [self.clouds.message(i) for i in f], s.kf_times[f], self.bias[f], self.ld, imu,
+                                       marg_flag_override=self._override(), want_knots=self.want_knots,
+                                       want_map=self.want_map)
+        else:
+            res, arr = e.ProcessImage(t_newest, self.clouds.message(self.frames[-1]), imu,
+                                      marg_flag_override=self._override(), want_knots=self.want_knots,
+                                      want_map=self.want_map)
+        t_wall = time.perf_counter() - t0
+        h2d, d2h = e.TransferStats(reset=True)
+        marg_flag = res["marg_flag"]
+        ks = int((res["knot_t0_ns"] - s.t0_ns) // s.dt_ns)
+        self.ncp = ks + res["n_knots"]
+        if "q" in arr:
+            self.q[ks:self.ncp] = arr["q"]; self.p[ks:self.ncp] = arr["p"]; self.ld = arr["line_delay"]
+        if "map" in arr:
+            self.last_map = arr["map"]
+        self.frames.pop(0 if marg_flag == MARGIN_OLD else -2)
+        sv, pr = res["solve"], res["predictor"]
+        rec = dict(window=self.step_index, ms=1e3 * t_wall, host_ms=res["host_ms"], prior_const=0.0,
+                   iterations=sv["iterations"], final_cost=sv["final_cost"], initial_cost=sv["initial_cost"],
+                   termination=sv["termination"], n_obs=res["n_image_factors"], n_imu=res["n_imu_factors"],
+                   n_knots=res["n_knots"], n_lm=res["n_landmarks"], device_ms=sv["device_ms"], marg_flag=marg_flag,
+                   init_iterations=None if res["n_predictor_imu"] == 0 or first else pr["iterations"],
+                   init_device_ms=pr["device_ms"], prior_dim=res["prior_dim"], h2d_bytes=h2d, d2h_bytes=d2h,
+                   n_triangulated=res["n_triangulated"], n_fallback=res["n_fallback"], n_removed=res["n_removed"],
+                   frame_slot=res["frame_slot"])
+        if self.opt.min_parallax > 0:
+            rec.update(StreamingRunner._decision_record(res["n_tracked"], res["parallax_num"], res["parallax_sum"]))
+        if self.reanchor:
+            rec.update(n_reanchored=res["n_reanchored"])
+        if self.publish_map:
+            rec.update(n_map_points=res["n_map_points"], n_margin_points=res["n_margin_points"])
+        self.records.append(rec)
+        self.step_index += 1
+        return rec
+
+    def run(self, n_windows, first=0):
+        for _ in range(n_windows):
+            self.step()
+        return self.records
+
+    def state_error(self):
+        """RMS translation error of the optimised part of the spline against the generator's truth (sanity metric)."""
+        s = self.seq
+        ks = int((s.kf_times[self.frames[0]] - s.t0_ns) // s.dt_ns)
+        return float(np.sqrt(np.mean(np.sum((self.p[ks:self.ncp - 2] - s.p_gt[ks:self.ncp - 2]) ** 2, axis=1))))
+
+
 from ctypes import byref, c_int32 as C_int32  # noqa: E402  (used by ResidentRunner.step)
+from ctypes import byref as C_byref  # noqa: E402  (used by CycleRunner)

@@ -596,6 +596,162 @@ int ctvio_feature_table_point_covariance(ctvio_handle h, int32_t n_landmarks, in
 
 /* bytes moved host<->device by the C-ABI calls since the last reset (state, factors, priors, index tables) */
 int ctvio_transfer_stats(ctvio_handle h, int64_t* h2d_bytes, int64_t* d2h_bytes, int32_t reset);
+/* host waits on the device (stream synchronisations, and spins on the scalars an LM step publishes to mapped memory) by
+ * the C-ABI calls made on the calling thread since the last reset: a debug counter for measuring how often the host
+ * stops for the device. */
+int ctvio_sync_stats(ctvio_handle h, int64_t* host_waits, int32_t reset);
+
+/* ---- the per-image odometry cycle: OdometryManager::ProcessVIOData (odometry_manager.cpp:178-299) behind two calls ----
+ * The resident window (SURVEY §8f-1) driven as the reference drives it after every image, with every stage of the
+ * section above in the reference's order and the bookkeeping a caller of those calls keeps itself (frame slots, the
+ * window's frames and frame times, the knot range of each frame, bias nodes) held by the library.  The caller passes
+ * only messages: the tracker's PointClouds and the IMUData records.  Not covered: the covariance publications, the
+ * host-association and rho0 modes of the separate calls, sharded engines and the initialisers.
+ * Every image takes a frame slot: frame f (counting the frames since ctvio_odometry_start, the first one 0) takes slot
+ * f % 16 when the feature table does not hold it, else the lowest free slot. */
+
+/* One tracker message: sensor_msgs::PointCloud as ctvio_ingest_feature_cloud takes it. */
+typedef struct ctvio_image_msg {
+  int64_t t_ns;          /* image time                                                   */
+  int32_t n_points;
+  int32_t reserved;
+  const float* points_xyz;  /* geometry_msgs::Point32[] (x, y, z = 1)                     */
+  const float* ch_id;       /* channels[0..4]: id, u, v, velocity_x, velocity_y           */
+  const float* ch_u;
+  const float* ch_v;
+  const float* ch_vx;
+  const float* ch_vy;
+} ctvio_image_msg;
+
+/* IMUData records as ctvio_ingest_imu takes them: int64 timestamp at offset 0, Vector3d gyro at off_gyro, Vector3d
+ * accel at off_accel, record size stride_bytes. */
+typedef struct ctvio_imu_msgs {
+  int32_t n;
+  int32_t stride_bytes;
+  int32_t off_gyro;
+  int32_t off_accel;
+  const void* data;
+} ctvio_imu_msgs;
+
+/* Options of the cycle, fixed by ctvio_odometry_start for the whole run.  ctvio_cycle_default_options fills the values
+ * in brackets. */
+typedef struct ctvio_cycle_options {
+  int32_t window_size;          /* WINDOW_SIZE (parameters.h:8): the window holds window_size + 1 frames, 2..15 [10] */
+  int32_t solve_iterations;     /* UpdateTrajectory's Solve (odometry_manager.cpp:264)                        [15]  */
+  int32_t predictor_iterations; /* InitTrajectory's Solve (trajectory_manager.cpp:288-315)                    [8]   */
+  int32_t fix_ld;               /* line delay constant in the main solve                                      [0]   */
+  double min_parallax;          /* MIN_PARALLAX, focal-length normalised; <= 0: every image is a keyframe       [0]   */
+  double init_depth;            /* INIT_DEPTH (parameters.cpp:44): triangulation fallback and depth shift      [5]   */
+  int64_t extend_ns;            /* the spline is extended to image time + extend_ns (odometry_manager.cpp:246) [40 ms] */
+  double ld_lower, ld_upper;    /* line-delay bounds of the main solve                                   [0, 35e-6] */
+  double sigma_wb_discrete;     /* bias random walk (trajectory_manager.cpp:420-450)                          [2e-5] */
+  double sigma_ab_discrete;     /*                                                                            [4e-4] */
+  int32_t reanchor;             /* the feature list slides as the reference's does (ctvio_feature_table_slide_reanchor)
+                                   instead of dropping a landmark with its anchor frame (ctvio_feature_table_slide) [0] */
+  int32_t publish_map;          /* ctvio_feature_table_map of the post-slide window after every image         [1]   */
+  int32_t reserved[4];
+} ctvio_cycle_options;
+
+/* Optional outputs; a NULL pointer means the output is not wanted. */
+typedef struct ctvio_cycle_outputs {
+  /* the window's knots and line delay after ctvio_gauge_realign, before the slide (what the reference publishes) */
+  int32_t knot_capacity;   /* rows of q_xyzw / p_xyz; CTVIO_ERR_INVALID (after the cycle ran) when below the knot count */
+  int32_t map_capacity;    /* rows of the map point arrays, as ctvio_feature_table_map's capacity                    */
+  double* q_xyzw;          /* [knot_capacity][4]                                                                     */
+  double* p_xyz;           /* [knot_capacity][3]                                                                     */
+  double* line_delay;      /* [1]                                                                                    */
+  /* ctvio_feature_table_map of the post-slide window (publish_map only) */
+  double* map_xyz;         /* [map_capacity][3]                                                                      */
+  int32_t* map_feature_id; /* [map_capacity]                                                                         */
+  uint8_t* map_in_margin_cloud;
+  double* cam_q_xyzw;      /* [16][4]: the post-slide window's camera poses, oldest to newest                       */
+  double* cam_p_xyz;       /* [16][3]                                                                                */
+} ctvio_cycle_outputs;
+
+/* What one cycle did. */
+typedef struct ctvio_cycle_result {
+  int32_t marg_flag;        /* 0 MARGIN_OLD, 1 MARGIN_SECOND_NEW                                                    */
+  int32_t n_tracked;        /* ctvio_check_keyframe's counts; -1 / 0 when no check ran                              */
+  int32_t parallax_num;
+  int32_t frame_slot;       /* the slot the image took (ctvio_odometry_start: the newest frame's)                   */
+  double parallax_sum;
+  int32_t n_frames;         /* frames of the window that was solved                                                 */
+  int32_t n_knots;          /* its knots; knot 0 sits at knot_t0_ns                                                 */
+  int64_t knot_t0_ns;
+  int32_t n_landmarks, n_image_factors, n_imu_factors, n_predictor_imu, n_triangulated, n_fallback;
+  ctvio_summary predictor;  /* all zero when the predictor did not run (window 0, or no IMU sample in its range)    */
+  ctvio_summary solve;
+  int32_t prior_dim;        /* dimension of the active prior after the cycle                                        */
+  int32_t n_removed;        /* entries that left the feature table                                                  */
+  int32_t n_reanchored;     /* reanchor only, else 0                                                                */
+  int32_t n_map_points;     /* publish_map only, else 0                                                             */
+  int32_t n_margin_points;
+  int32_t n_knots_after;    /* knots of the engine's window after the slide                                         */
+  double host_ms;           /* the call's own host wall clock                                                       */
+} ctvio_cycle_result;
+
+/* the defaults in brackets above */
+int ctvio_cycle_default_options(ctvio_cycle_options* opt);
+/* ctvio_odometry_start - SetInitialState + InitWindow + the first UpdateTrajectory (odometry_manager.cpp:230-264), which
+ *   runs no predictor (first_opt_flag): the initializer's window of n_frames = window_size + 1 images goes up once.
+ *   Knots q_xyzw / p_xyz [n_knots] start at t0_ns (knot 0, on the configured knot grid), bg_ba6 [n_frames] holds one
+ *   bias node per frame, line_delay the initial line delay; imu: every IMUData record up to the newest image (may be
+ *   NULL when there is none).  The engine's earlier run, if any, is forgotten: feature table, frame slots, IMU table and
+ *   prior start empty.  Then the window is solved as ctvio_process_image solves it, without the predictor.
+ *   marg_flag_override: -1 lets the keyframe decision choose, 0 / 1 force MARGIN_OLD / MARGIN_SECOND_NEW.
+ *   Errors: see ctvio_process_image; CTVIO_ERR_INVALID also for n_frames != window_size + 1, n_knots < 4 or a NULL
+ *   array, all checked before anything changes. */
+int ctvio_odometry_start(ctvio_handle h, const ctvio_cycle_options* opt, int64_t t0_ns, int32_t n_knots, const double* q_xyzw,
+                         const double* p_xyz, int32_t n_frames, const ctvio_image_msg* frames, const double* bg_ba6,
+                         double line_delay, const ctvio_imu_msgs* imu, int32_t marg_flag_override, ctvio_cycle_outputs* out,
+                         ctvio_cycle_result* result);
+/* ctvio_process_image - one image of OdometryManager::ProcessVIOData (odometry_manager.cpp:178-299) on the resident
+ *   window.  imu: the IMUData records since the last call (may be NULL).  In order:
+ *    1. the cloud goes into the image's frame slot and joins the feature table (ctvio_ingest_feature_cloud,
+ *       ctvio_feature_table_add; AddImageToWindow, visual_odometry.cpp:180-183);
+ *    2. the keyframe decision: ctvio_check_keyframe over the window's slots when min_parallax > 0, else MARGIN_OLD,
+ *       unless marg_flag_override says otherwise;
+ *    3. ExtendTrajectory to the image time + extend_ns (trajectory_manager.cpp:108-120), then the IMU records go in,
+ *       samples before the window's first knot retired (AddIMUData / RemoveIMUData, :472-475);
+ *    4. ctvio_feature_table_window (setDepth + getDepthVector);
+ *    5. InitTrajectory (:288-315): IMU factors over [end of the spline before the extension, end after it) with the
+ *       newest bias node, prior off, knots up to the last one before the extension fixed, biases locked, line delay
+ *       fixed, predictor_iterations LM steps (skipped without a sample in that range);
+ *    6. ctvio_triangulate_window_from_table (FeatureManager::triangulate, visual_odometry.cpp:185-191);
+ *    7. UpdateTrajectory's factors (:317-453): the prior, the table's image factors, IMU factors over [first knot,
+ *       min(end of spline, image time + 1 ns)) with bias nodes from the keyframe intervals, and the bias random-walk
+ *       factors between consecutive frames; MARGIN_OLD flags for marginalization the oldest frame's image factors, the
+ *       IMU samples before the second frame and the first bias factor (:206-263);
+ *    8. Solve(solve_iterations);
+ *    9. double2vector (:485-516): ctvio_gauge_realign to knot 0 as it was before the solve;
+ *   10. MARGIN_OLD: UpdateVIOPrior (:122-286): ctvio_marginalize, and the new prior becomes the active one
+ *       (ctvio_get_prior still returns it afterwards, until the next marginalization);
+ *   11. reanchor: ctvio_feature_table_slide_reanchor;
+ *   12. SlideWindow: ctvio_slide_window(knots of the oldest frame, 1, 1) or ctvio_slide_window_second_new;
+ *   13. without reanchor: ctvio_feature_table_slide of the leaving frame's slot;
+ *   14. publish_map: ctvio_feature_table_map of the post-slide window.
+ *   Computed on the device from what it already holds, where a caller of the separate calls computes them on the host:
+ *   - the bias random-walk weights (trajectory_manager.cpp:420-450): for frames i, i+1, with s2 the sum of dt^2 over the
+ *     IMU intervals that start at or after frame i's time and end before frame i+1's, sqrt_info = 1 / sqrt(s2 sigma^2)
+ *     per axis (0 when s2 == 0).  s2 is the difference of two entries of a sequential prefix sum of dt^2 that runs over
+ *     every sample ingested since ctvio_odometry_start, in sample order, with dt = (t_k - t_{k-1}) * 1e-9;
+ *   - the pre-solve pose of knot 0 for the re-alignment, a device-to-device snapshot taken before the main solve
+ *     (trajectory_manager.cpp:325-327).
+ *   The host still reads back what it decides on or sizes launches with: the keyframe flag, the feature table's counts,
+ *   the LM step scalars, the marginalization's block bookkeeping.
+ *   Errors (through ctvio_last_error): CTVIO_ERR_INVALID for a NULL handle, options (start) or result, options out of
+ *   range (window_size outside 2..15, iterations < 1 or predictor_iterations < 0, init_depth not finite and > 0,
+ *   extend_ns <= 0, a min_parallax that is not finite), a bad message (NULL arrays, n_points outside 0..1024) or IMU
+ *   layout (as ctvio_ingest_imu), marg_flag_override outside -1..1; CTVIO_ERR_STATE before ctvio_odometry_start, on a
+ *   sharded engine (world > 1), or when the feature table holds all 16 frame slots so the image has none.  These are
+ *   checked before any device work and leave the engine unchanged.  An error of a stage (CTVIO_ERR_TIME_RANGE, ...)
+ *   stops the cycle there; the engine must then be restarted with ctvio_odometry_start. */
+int ctvio_process_image(ctvio_handle h, const ctvio_image_msg* img, const ctvio_imu_msgs* imu, int32_t marg_flag_override,
+                        ctvio_cycle_outputs* out, ctvio_cycle_result* result);
+/* test support: the bias random-walk weights ctvio_process_image computes, for the keyframe times kf_t_ns[0 .. n_kf-1]
+ *   (2..16, ascending) over the resident IMU table as the last cycle left it; sqrt_info6 [n_kf - 1][6]. */
+int ctvio_debug_bias_weights(ctvio_handle h, int32_t n_kf, const int64_t* kf_t_ns, double sigma_wb_discrete,
+                             double sigma_ab_discrete, double* sqrt_info6);
 
 /* ---- measurement support (bench.py roofline) ----
  * Average CUDA-event duration (ms, on the engine stream) of one launch of each stage of an LM step at the
