@@ -112,7 +112,8 @@ class CycleOptions(C.Structure):
         ("fix_ld", C.c_int32), ("min_parallax", C.c_double), ("init_depth", C.c_double), ("extend_ns", C.c_int64),
         ("ld_lower", C.c_double), ("ld_upper", C.c_double), ("sigma_wb_discrete", C.c_double),
         ("sigma_ab_discrete", C.c_double), ("reanchor", C.c_int32), ("publish_map", C.c_int32),
-        ("reserved", C.c_int32 * 4),
+        ("publish_pose_covariance", C.c_int32), ("publish_odometry_covariance", C.c_int32),
+        ("publish_map_covariance", C.c_int32), ("covariance_gauge_knot", C.c_int32),
     ]
 
 
@@ -144,6 +145,19 @@ class CycleResult(C.Structure):
         return d
 
 
+class CycleCovarianceInfo(C.Structure):
+    """ctvio_cycle_covariance_info (include/ctvio.h)."""
+
+    _fields_ = [
+        ("requested", C.c_int32), ("available", C.c_int32), ("status", C.c_int32), ("gauge_knot", C.c_int32),
+        ("rcond", C.c_double), ("pose_t_ns", C.c_int64), ("n_pairs", C.c_int32), ("n_map_points", C.c_int32),
+        ("n_map_points_without_cov", C.c_int32), ("reserved", C.c_int32),
+    ]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_ if k != "reserved"}
+
+
 # every symbol include/ctvio.h declares (without prefix); used by the
 # export-completeness test and by the binder.
 ABI_SYMBOLS = [
@@ -161,7 +175,7 @@ ABI_SYMBOLS = [
     "feature_table_add", "feature_table_window", "triangulate_window_from_table", "add_image_features_from_table",
     "feature_table_slide", "feature_table_landmarks", "feature_table_map", "feature_table_slide_reanchor",
     "debug_structure", "feature_table_point_covariance", "sync_stats", "cycle_default_options", "odometry_start",
-    "process_image", "debug_bias_weights",
+    "process_image", "debug_bias_weights", "cycle_covariances",
 ]
 
 
@@ -175,7 +189,8 @@ DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enab
                        "add_image_features_from_table", "feature_table_slide", "feature_table_landmarks",
                        "feature_table_map", "feature_table_slide_reanchor", "debug_structure", "covariance",
                        "pose_covariance", "relative_pose_covariance", "point_covariance", "feature_table_point_covariance",
-                       "sync_stats", "cycle_default_options", "odometry_start", "process_image", "debug_bias_weights")
+                       "sync_stats", "cycle_default_options", "odometry_start", "process_image", "debug_bias_weights",
+                       "cycle_covariances")
 
 
 def _addr(a):
@@ -762,6 +777,32 @@ class Estimator:
         self.n_knots = res.n_knots_after
         self.n_bias = res.n_frames   # (the newest node stands for the next image)
         self.n_lm = res.n_landmarks
+
+    CTVIO_ERR_STATE = -4
+
+    def CycleCovariances(self):
+        """ctvio_cycle_covariances: what the last cycle published with its publish_*_covariance options, as
+        (cov12 [12, 12] or None, cov6 [n_frames - 1, 6, 6] or None, map_cov9 [n_map_points, 3, 3] or None, info dict).
+        The info dict (ctvio_cycle_covariance_info) also carries pose_t_ns, pair_t_ns [n_pairs, 2] and, when nothing is
+        available, the reason as "error".  Raises CtvioError when no cycle asked for covariances."""
+        info = CycleCovarianceInfo()
+        cov12 = np.zeros((12, 12)); cov6 = np.zeros((15, 6, 6)); pair_t = np.zeros((15, 2), np.int64)
+        cap = self.MAP_CAPACITY
+        cov9 = np.empty((cap, 3, 3))
+        t = C.c_int64()
+        fn = self.lib._fn["cycle_covariances"]
+        rc = fn(self.h, _dp(cov12), C.byref(t), _dp(cov6), _lp(pair_t), C.c_int32(cap), _dp(cov9), C.byref(info))
+        d = info.as_dict()
+        if rc != 0:
+            msg = self.lib._fn["last_error"]().decode()
+            if rc != self.CTVIO_ERR_STATE or not info.requested:
+                raise CtvioError(f"{self.lib.prefix}cycle_covariances failed ({rc}): {msg}")
+            d["error"] = msg
+            return None, None, None, d
+        a = info.available
+        d["pair_t_ns"] = pair_t[:info.n_pairs].copy()
+        return (cov12 if a & 1 else None, cov6[:info.n_pairs].copy() if a & 2 else None,
+                cov9[:info.n_map_points].copy() if a & 4 else None, d)
 
     def DebugBiasWeights(self, kf_times, sigma_wb, sigma_ab):
         """(test support) the bias random-walk weights of ctvio_process_image for these keyframe times over the resident

@@ -523,10 +523,11 @@ int launch_relative_pose_cov(const RelativePoseCovLaunch& a, cudaStream_t s) {
 namespace {
 
 // Sigma of the window at the current state into cws.cov and the inverse-depth variances into cws.var, with the knots
-// <= gauge_knot held constant on top of what the options hold constant (-1: the options alone).  Returns CTVIO_OK, an
-// error of the evaluation, or CTVIO_ERR_STATE "<who>: rank deficient"; *rcond (may be null) is written in these last two
-// cases only.  Ends with the stream synchronised.
-int form_covariance(ctvio_engine* e, int gauge_knot, const char* who, double* rcond) {
+// <= gauge_knot held constant on top of what the options hold constant (-1: the options alone), enqueued on the engine
+// stream up to the publication of the rank test's inputs (the scalar block and rcond) to pub with sequence number seq
+// and the restore of the LM driver's scalar block: no host wait.  Right after a solve of the same factor set (the
+// odometry cycle) prepare() finds structure, masks and prior built and does nothing.
+int enqueue_covariance(ctvio_engine* e, int gauge_knot, LmPublished* pub, unsigned long long seq) {
   int rc = prepare(e);
   if (rc) return rc;
   cudaStream_t st = e->stream;
@@ -577,22 +578,72 @@ int form_covariance(ctvio_engine* e, int gauge_knot, const char* who, double* rc
   v.var = w.var.p;
   v.scal = e->d_scal.p;
   e->launches += launch_landmark_variance(v, st);
-  e->launches += launch_cov_publish(w.piv.p, int(nb), e->d_scal.p, e->h_pub, ++e->pub_seq, st);
+  e->launches += launch_cov_publish(w.piv.p, int(nb), e->d_scal.p, pub, seq, st);
   CUDA_OK(cudaMemcpyAsync(e->d_scal.p, w.scal.p, sizeof(LmScalars), cudaMemcpyDeviceToDevice, st));
-  rc = read_scalars(e, true);
-  const double rc_value = const_cast<const LmPublished*>(e->h_pub)->rcond;
-  const bool failed = e->h_scal->chol_fail != 0;
-  CUDA_OK(stream_sync(st));  // (the restore behind the published block)
-  if (rc) return rc;
-  if (rcond) *rcond = rc_value;
+  return CTVIO_OK;
+}
+
+// form_covariance's rank test on the published block, for a caller that has already synchronised: the error of the
+// evaluation, or CTVIO_ERR_STATE "<who>: rank deficient" (message in *why), else CTVIO_OK
+int rank_test(const LmPublished& pub, const char* who, std::string* why) {
+  if (pub.s.error_flags & 1) {
+    *why = "a factor time left its knot window / the spline (line delay too large?)";
+    return CTVIO_ERR_TIME_RANGE;
+  }
+  const double rc_value = pub.rcond;
+  const bool failed = pub.s.chol_fail != 0;
   // Ceres' default min_reciprocal_condition_number; the estimate is the pivot ratio, see include/ctvio.h
   if (failed || !(rc_value >= 1e-14)) {
     char msg[128];
-    std::snprintf(msg, sizeof(msg), "%s: rank deficient (rcond %.3e%s)", who, rc_value,
-                  failed ? ", non-positive pivot" : "");
-    return fail(CTVIO_ERR_STATE, msg);
+    std::snprintf(msg, sizeof(msg), "%s: rank deficient (rcond %.3e%s)", who, rc_value, failed ? ", non-positive pivot" : "");
+    *why = msg;
+    return CTVIO_ERR_STATE;
   }
   return CTVIO_OK;
+}
+
+// Sigma as enqueue_covariance forms it, then the rank test.  Returns CTVIO_OK, an error of the evaluation, or
+// CTVIO_ERR_STATE "<who>: rank deficient"; *rcond (may be null) is written in these last two cases only.  Ends with the
+// stream synchronised.
+int form_covariance(ctvio_engine* e, int gauge_knot, const char* who, double* rcond) {
+  int rc = enqueue_covariance(e, gauge_knot, e->h_pub, ++e->pub_seq);
+  if (rc) return rc;
+  rc = read_scalars(e, true);
+  const double rc_value = const_cast<const LmPublished*>(e->h_pub)->rcond;
+  CUDA_OK(stream_sync(e->stream));  // (the restore behind the published block)
+  if (rc) return rc;
+  if (rcond) *rcond = rc_value;
+  LmPublished pub;
+  pub.s = *e->h_scal;
+  pub.rcond = rc_value;
+  std::string why;
+  if ((rc = rank_test(pub, who, &why))) return fail(rc, why);
+  return CTVIO_OK;
+}
+
+// point_cov_kernel over the a.n points whose inputs a names into out (device memory), right after Sigma on the same
+// stream
+void launch_point_covariance(ctvio_engine* e, PointCovLaunch& a, double* out) {
+  const ProblemDims d = e->dims();
+  a.st = e->x[e->cur].ptrs();
+  a.sp = e->sp;
+  a.R_CI = e->rig.R_CI;
+  a.p_CI = e->rig.p_CI;
+  a.np = d.np; a.idx_ld = d.idx_ld;
+  a.cov = e->cws.cov.p;
+  a.var = e->cws.var.p;
+  a.ne = e->ne(e->cur ^ 1);  // the buffer enqueue_covariance evaluated into
+  a.lm = e->lml();
+  a.active = e->d_active.p;
+  a.out = out;
+  e->launches += launch_point_cov(a, e->stream);
+}
+
+// the anchors of the feature table's window landmarks: the first entry of each observation CSR row
+void table_anchors(ctvio_engine* e, PointCovLaunch& a) {
+  auto& ft = e->ft;
+  a.obs_offset = ft.obs_offset.p; a.obs_slot = ft.obs_slot.p; a.obs_idx = ft.obs_idx.p;
+  a.table = e->d_frames.p; a.frame_t = e->d_frame_t.p; a.frame_cap = ctvio_engine::kFrameCap;
 }
 
 // point_cov_kernel over the a.n points whose inputs a names, right after form_covariance on the same stream; the n x 9
@@ -600,20 +651,8 @@ int form_covariance(ctvio_engine* e, int gauge_knot, const char* who, double* rc
 int point_covariance(ctvio_engine* e, PointCovLaunch& a, double* cov9) {
   cudaStream_t st = e->stream;
   auto& w = e->cws;
-  const ProblemDims d = e->dims();
   CUDA_OK(w.pose.reserve(9 * size_t(a.n)));
-  a.st = e->x[e->cur].ptrs();
-  a.sp = e->sp;
-  a.R_CI = e->rig.R_CI;
-  a.p_CI = e->rig.p_CI;
-  a.np = d.np; a.idx_ld = d.idx_ld;
-  a.cov = w.cov.p;
-  a.var = w.var.p;
-  a.ne = e->ne(e->cur ^ 1);  // the buffer form_covariance evaluated into
-  a.lm = e->lml();
-  a.active = e->d_active.p;
-  a.out = w.pose.p;
-  e->launches += launch_point_cov(a, st);
+  launch_point_covariance(e, a, w.pose.p);
   CUDA_OK(cudaMemcpyAsync(cov9, w.pose.p, 9 * size_t(a.n) * sizeof(double), cudaMemcpyDeviceToHost, st));
   e->d2h_bytes += 9 * size_t(a.n) * sizeof(double);
   CUDA_OK(stream_sync(st));
@@ -796,7 +835,83 @@ extern "C" int ctvio_feature_table_point_covariance(ctvio_handle e, int32_t n_la
   // the anchors come from the window's observation CSR and the frame table: nothing goes up
   PointCovLaunch a = {};
   a.n = n_landmarks;
-  a.obs_offset = ft.obs_offset.p; a.obs_slot = ft.obs_slot.p; a.obs_idx = ft.obs_idx.p;
-  a.table = e->d_frames.p; a.frame_t = e->d_frame_t.p; a.frame_cap = ctvio_engine::kFrameCap;
+  table_anchors(e, a);
   return point_covariance(e, a, cov9);
 }
+
+namespace ctvio::host {
+
+// the cycle's device workspace cov_out: cov12 (144) | cov6 [15][36] | cov9 [n_landmarks][9]
+constexpr size_t kCycleCov6 = 144, kCycleCov9 = kCycleCov6 + 36 * (kKeyframeMaxSlots - 1);
+
+int covariance_rank_test(const LmPublished& pub, const char* who, std::string* why) { return rank_test(pub, who, why); }
+
+int cycle_covariance_enqueue(ctvio_engine* e, int gauge_knot, bool pose, bool rel, bool points) {
+  auto& c = e->cyc;
+  auto& cv = c.cov;
+  if (!c.cov_host) {
+    void* p = nullptr;
+    if (cudaHostAlloc(&p, sizeof(CycleCovHost), cudaHostAllocMapped) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(CTVIO_ERR_CUDA, "could not allocate the mapped covariance buffer");
+    }
+    c.cov_host = static_cast<CycleCovHost*>(p);
+  }
+  // sized for any window once: a growing reserve() would free, and cudaFree waits for the device
+  CUDA_OK(c.cov_t.reserve(1 + kKeyframeMaxSlots));
+  CUDA_OK(c.cov_out.reserve(kCycleCov9 + 9 * size_t(kFeatureTableMaxEntries)));
+  CycleCovHost* h = c.cov_host;
+  cudaStream_t st = e->stream;
+  const int nf = cv.n_frames, n_pairs = rel ? nf - 1 : 0;
+  // the times go up from the mapped block (the last cycle's copy out of it completed before that cycle ended)
+  const int n_t = (pose || n_pairs > 0) ? 1 + (n_pairs > 0 ? nf : 0) : 0;
+  h->t[0] = cv.pose_t;
+  for (int k = 0; k < nf; ++k) h->t[1 + k] = cv.frame_t[k];
+  if (n_t) {
+    CUDA_OK(cudaMemcpyAsync(c.cov_t.p, h->t, size_t(n_t) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    e->h2d_bytes += size_t(n_t) * sizeof(int64_t);
+  }
+  if (const int rc = enqueue_covariance(e, gauge_knot, &h->pub, ++cv.seq)) return rc;
+  if (pose) {  // the camera pose and velocity at the TF time: ctvio_pose_covariance(camera_frame = 1)
+    PoseCovLaunch a = {};
+    a.st = e->x[e->cur].ptrs();
+    a.sp = e->sp;
+    a.R_CI = e->rig.R_CI;
+    a.p_CI = e->rig.p_CI;
+    a.n = 1; a.np = e->dims().np; a.camera_frame = 1;
+    a.t = c.cov_t.p;
+    a.cov = e->cws.cov.p;
+    a.out = c.cov_out.p;
+    e->launches += launch_pose_cov(a, st);
+    CUDA_OK(cudaMemcpyAsync(h->cov12, a.out, 144 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    e->d2h_bytes += 144 * sizeof(double);
+  }
+  if (n_pairs > 0) {  // the odometry edges (t[i], t[i + 1]): ctvio_relative_pose_covariance(camera_frame = 1)
+    RelativePoseCovLaunch a = {};
+    a.st = e->x[e->cur].ptrs();
+    a.sp = e->sp;
+    a.R_CI = e->rig.R_CI;
+    a.p_CI = e->rig.p_CI;
+    a.n = n_pairs; a.np = e->dims().np; a.camera_frame = 1;
+    a.t_a = c.cov_t.p + 1;
+    a.t_b = c.cov_t.p + 2;
+    a.cov = e->cws.cov.p;
+    a.out = c.cov_out.p + kCycleCov6;
+    a.cross = nullptr;
+    e->launches += launch_relative_pose_cov(a, st);
+    CUDA_OK(cudaMemcpyAsync(h->cov6, a.out, 36 * size_t(n_pairs) * sizeof(double), cudaMemcpyDeviceToHost, st));
+    e->d2h_bytes += 36 * size_t(n_pairs) * sizeof(double);
+  }
+  if (points && cv.n_lm > 0) {  // the window landmarks' world points, anchored as the table holds them: stay on the
+                                // device until the map kernel gathers them
+    PointCovLaunch a = {};
+    a.n = cv.n_lm;
+    table_anchors(e, a);
+    launch_point_covariance(e, a, c.cov_out.p + kCycleCov9);
+  }
+  return CTVIO_OK;
+}
+
+const double* cycle_point_covariances(ctvio_engine* e) { return e->cyc.cov_out.p + kCycleCov9; }
+
+}  // namespace ctvio::host

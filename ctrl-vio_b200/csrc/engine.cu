@@ -758,6 +758,7 @@ int ctvio_destroy(ctvio_handle e) {
   if (e->h_pub) cudaFreeHost(e->h_pub);
   if (e->h_mirror) cudaFreeHost(e->h_mirror);
   if (e->ft.h_map_head) cudaFreeHost(e->ft.h_map_head);
+  if (e->cyc.cov_host) cudaFreeHost(e->cyc.cov_host);
   if (e->ev_zero) cudaEventDestroy(e->ev_zero);
   cudaEventDestroy(e->ev0);
   cudaEventDestroy(e->ev1);

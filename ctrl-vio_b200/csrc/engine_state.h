@@ -3,6 +3,7 @@
 // what ctvio_last_error reports, and every upload is counted.
 #pragma once
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -118,6 +119,33 @@ struct DevState {
 struct HostImage { int64_t ti, tj; int32_t rowi, rowj; double pi[2], pj[2]; int32_t lm, marg; };
 struct HostImu { int64_t t; double gyro[3], accel[3]; int32_t node, marg; };
 struct HostBias { int32_t i, j; double s[6]; int32_t marg; };
+
+// The odometry cycle's covariance publications (ctvio_cycle_covariances).  Host side: pinned + mapped, allocated on
+// first use; the kernels and copies of one cycle write it, the host reads it after a synchronisation the cycle makes
+// anyway.
+struct CycleCovHost {
+  LmPublished pub;                                         // the rank test's inputs, written by cov_publish_kernel
+  int64_t t[kKeyframeMaxSlots + 1];                        // staging of Cycle::cov_t
+  double cov12[144];
+  double cov6[(kKeyframeMaxSlots - 1) * 36];
+  double map_cov9[size_t(kFeatureTableMaxEntries) * 9];    // written by feature_table_map_kernel<true>
+};
+// what the last cycle published
+struct CycleCovState {
+  bool ran = false;         // the last cycle completed (cleared when one starts)
+  int32_t requested = 0;    // its options' publications: 1 pose, 2 odometry, 4 map
+  int32_t available = 0;    // the same bits for what it published
+  int32_t status = CTVIO_OK;
+  double rcond = NAN;
+  int64_t pose_t = 0;
+  int32_t n_frames = 0;     // frames of the solved window: n_frames - 1 pairs
+  int64_t frame_t[kKeyframeMaxSlots] = {0};
+  int32_t n_lm = 0;         // landmarks of the solved window: rows of the per-landmark covariances
+  int32_t n_map = 0, n_map_nan = 0;
+  bool pending = false;     // Sigma was enqueued; the rank test has not been read yet
+  unsigned long long seq = 0;
+  std::string why = "no odometry cycle has run";  // why nothing is available (the getter's error message)
+};
 
 }  // namespace ctvio::host
 
@@ -305,6 +333,12 @@ struct ctvio_engine {
     DevBuf<double> bias_w;         // [n_frames - 1][6] bias random-walk weights of the current window
     DevBuf<double> imu_carry;      // {prefix of dt^2 at the last sample ingested, its time (int64 bits), valid}
     DevBuf<double> snap;           // local knot 0 before the main solve: q (4), p (3), then R0 / t0 (12)
+    // the covariance publications: workspace that lives from the re-alignment to the map (not cws, which every
+    // covariance call reuses), and what the last cycle published
+    DevBuf<int64_t> cov_t;         // the TF time, then the solved window's frame times
+    DevBuf<double> cov_out;        // cov12 (144) | cov6 [n_frames - 1][36] | cov9 [n_landmarks][9]
+    CycleCovHost* cov_host = nullptr;
+    CycleCovState cov;
   } cyc;
   int n_marg_img = -1;  // marginalized image factors of the last ctvio_marginalize (-1: pos_cam / pos_lm / marg_img not built)
 
@@ -377,5 +411,19 @@ int ingest_feature_cloud_body(ctvio_engine* e, int32_t slot, int64_t t_ns, int32
                               const float* ch_v, bool sync);
 int ingest_imu_body(ctvio_engine* e, int32_t n, const void* records, int32_t stride, int32_t off_gyro, int32_t off_accel,
                     int64_t drop_before_ns, bool sync, int* first_new);
+// ctvio_feature_table_map; with point_cov9 (mapped host memory) the kernel also writes each point's covariance there,
+// gathered from lm_cov9 [n_cov][9] by the entry's number (feature_table_map_kernel<true>)
+int feature_table_map_body(ctvio_engine* e, int32_t n_frames, const int32_t* frame_slots, int32_t window_size,
+                           int32_t capacity, double* xyz_world, int32_t* feature_id, uint8_t* in_margin_cloud,
+                           int32_t* n_points, double* cam_q_xyzw, double* cam_p_xyz, const double* lm_cov9, int32_t n_cov,
+                           double* point_cov9);
+// covariance.cu, for the odometry cycle: Sigma with the knots <= gauge_knot held constant and its projections enqueued
+// on the engine stream without a host wait, the rank test's inputs published to e->cyc.cov_host->pub (the cycle reads
+// them after its next synchronisation, cycle_covariance_rank_test).  pose / rel / points: the TF pose at
+// e->cyc.cov.pose_t, the consecutive frame pairs of e->cyc.cov.frame_t, the window's landmarks.
+int cycle_covariance_enqueue(ctvio_engine* e, int gauge_knot, bool pose, bool rel, bool points);
+const double* cycle_point_covariances(ctvio_engine* e);  // [n_lm][9] in the solved window's numbering, on the device
+// CTVIO_OK, or the error the separate covariance calls return for the same inputs (message in *why)
+int covariance_rank_test(const LmPublished& pub, const char* who, std::string* why);
 
 }  // namespace ctvio::host

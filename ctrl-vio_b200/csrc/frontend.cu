@@ -548,6 +548,10 @@ __global__ void feature_table_factors_kernel(FeatureTableFactorArgs a) {
 // over the listed window.  The listed frames' camera poses (GetCameraPose at the frame time, :197-202) are evaluated
 // first into shared memory; then the entries, in chunks of kFtThreads: IsLandMarkStable (visual_odometry.h:82-93), a
 // block scan, and the stable ones are written compacted, in table order, to mapped host memory.  No atomics.
+// kCov: each written point also gets its 3 x 3 covariance at the same row of point_cov9, gathered from the window's
+// per-landmark covariances lm_cov9 at the entry's number; NaN for an entry without one (never numbered, or re-anchored
+// by the slide, which clears the number).
+template <bool kCov>
 __global__ void __launch_bounds__(kFtThreads) feature_table_map_kernel(FeatureTableMapArgs a) {
   __shared__ double s_cam[kKeyframeMaxSlots][12];  // by window position: camera R (9) | camera t (3)
   __shared__ int s_scan[32];
@@ -573,6 +577,7 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_map_kernel(FeatureTa
     const int e = c + tid;
     bool stable = false, margin = false;
     MapPoint p;
+    [[maybe_unused]] int lm_cov = -1;
     if (e < a.n_entries) {
       const int anchor = t.anchor[e], lm = t.lm[e];
       const uint32_t mask = t.mask[e];
@@ -593,11 +598,19 @@ __global__ void __launch_bounds__(kFtThreads) feature_table_map_kernel(FeatureTa
         for (int r = 0; r < 3; ++r) p.xyz[r] = w[3 * r] * pc.x + w[3 * r + 1] * pc.y + w[3 * r + 2] * pc.z + w[9 + r];
         p.id = t.id[e];
         p.in_margin_cloud = margin ? 1 : 0;
+        if constexpr (kCov) lm_cov = lm >= 0 && lm < a.n_cov ? lm : -1;
       }
     }
     int total;
     const int r = block_exclusive_scan(stable, s_scan, total);
-    if (stable) a.points[n_points + r] = p;
+    if (stable) {
+      a.points[n_points + r] = p;
+      if constexpr (kCov) {
+        double* dst = a.point_cov9 + 9 * size_t(n_points + r);
+#pragma unroll
+        for (int k = 0; k < 9; ++k) dst[k] = lm_cov >= 0 ? a.lm_cov9[9 * size_t(lm_cov) + k] : NAN;
+      }
+    }
     n_points += total;
   }
   if (tid == 0) { a.head->n_points = n_points; a.head->pad = 0; }
@@ -767,7 +780,11 @@ int launch_feature_table_factors(const FeatureTableFactorArgs& a, cudaStream_t s
   return 1;
 }
 int launch_feature_table_map(const FeatureTableMapArgs& a, cudaStream_t s) {
-  feature_table_map_kernel<<<1, kFtThreads, 0, s>>>(a);
+  feature_table_map_kernel<false><<<1, kFtThreads, 0, s>>>(a);
+  return 1;
+}
+int launch_feature_table_map_cov(const FeatureTableMapArgs& a, cudaStream_t s) {
+  feature_table_map_kernel<true><<<1, kFtThreads, 0, s>>>(a);
   return 1;
 }
 int launch_unpack_cloud(const UnpackCloudArgs& a, cudaStream_t s) {

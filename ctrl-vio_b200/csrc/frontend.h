@@ -228,6 +228,10 @@ struct FeatureTableMapArgs {
   int32_t n_rho;               // their count (0: no numbering)
   MapHeader* head;             // mapped host memory
   MapPoint* points;            // mapped host memory, [kFeatureTableMaxEntries]
+  // feature_table_map_kernel<true> (launch_feature_table_map_cov) only
+  const double* lm_cov9;       // [n_cov][9] point covariances in the last window's numbering (entry lm)
+  int32_t n_cov;               // their count
+  double* point_cov9;          // mapped host memory, [kFeatureTableMaxEntries][9], row k for points[k]
 };
 int launch_feature_table_add(const FeatureTableAddArgs& a, cudaStream_t s);
 int launch_feature_table_slide(const FeatureTableSlideArgs& a, cudaStream_t s);
@@ -235,6 +239,7 @@ int launch_feature_table_slide_reanchor(const FeatureTableSlideArgs& a, cudaStre
 int launch_feature_table_window(const FeatureTableWindowArgs& a, cudaStream_t s);
 int launch_feature_table_factors(const FeatureTableFactorArgs& a, cudaStream_t s);
 int launch_feature_table_map(const FeatureTableMapArgs& a, cudaStream_t s);
+int launch_feature_table_map_cov(const FeatureTableMapArgs& a, cudaStream_t s);
 
 // device-resident window bookkeeping (all on the device)
 int launch_extend_knots(const StatePtrs& st, int old_n, int new_n, cudaStream_t s);

@@ -2,6 +2,7 @@
 // window's entry points in OdometryManager::ProcessVIOData's order, with the window's frame bookkeeping held here and the
 // last two host computations of a caller of those entry points (the bias random-walk weights and the pre-solve pose of
 // knot 0) done on the device.
+#include <atomic>
 #include <chrono>
 #include <cmath>
 
@@ -116,6 +117,73 @@ int check_options(const ctvio_cycle_options* o) {
   if (!std::isfinite(o->min_parallax)) return fail(CTVIO_ERR_INVALID, "min_parallax must be finite");
   if (!std::isfinite(o->sigma_wb_discrete) || !std::isfinite(o->sigma_ab_discrete))
     return fail(CTVIO_ERR_INVALID, "bias sigmas must be finite");
+  for (const int32_t f : {o->publish_pose_covariance, o->publish_odometry_covariance, o->publish_map_covariance})
+    if (f != 0 && f != 1) return fail(CTVIO_ERR_INVALID, "the publish_*_covariance options must be 0 or 1");
+  if (o->covariance_gauge_knot < -1 || o->covariance_gauge_knot > 3)
+    return fail(CTVIO_ERR_INVALID, "covariance_gauge_knot must be -1..3");
+  if (o->publish_map_covariance && !o->publish_map)
+    return fail(CTVIO_ERR_INVALID, "publish_map_covariance requires publish_map");
+  return CTVIO_OK;
+}
+
+// ---- the covariance publications (ctvio_cycle_covariances) ----
+constexpr int64_t kTfLagNs = 50'000'000;  // the TF time: maxTimeNs() - 50 ms (odometry_manager.cpp:287-288)
+
+// a cycle starts: nothing it or an earlier one published is available until it completes
+void clear_covariances(ctvio_engine* e) {
+  auto& cv = e->cyc.cov;
+  const ctvio_cycle_options& o = e->cyc.opt;
+  cv.ran = false;
+  cv.requested = (o.publish_pose_covariance ? 1 : 0) | (o.publish_odometry_covariance ? 2 : 0) |
+                 (o.publish_map_covariance ? 4 : 0);
+  cv.available = 0;
+  cv.status = CTVIO_ERR_STATE;
+  cv.rcond = NAN;
+  cv.n_frames = cv.n_lm = cv.n_map = cv.n_map_nan = 0;
+  cv.pending = false;
+  cv.why = "the last cycle stopped on an error";
+}
+
+// step 9 done: Sigma of the solved window and its projections go on the stream, unless a time they need lies outside
+// the spline (then the status says so and the cycle goes on)
+int start_covariances(ctvio_engine* e, int64_t max_t, int n_lm) {
+  auto& c = e->cyc;
+  auto& cv = c.cov;
+  const bool pose = cv.requested & 1, rel = cv.requested & 2, points = cv.requested & 4;
+  cv.pose_t = max_t - kTfLagNs;
+  cv.n_frames = c.n_frames;
+  for (int k = 0; k < c.n_frames; ++k) cv.frame_t[k] = c.t[k];
+  cv.n_lm = n_lm;
+  // the ranges the separate calls check: the query times, and every held slot's frame time (the anchors)
+  bool inside = true;
+  int32_t s;
+  double u;
+  if (pose) inside = spline_index(e->sp, cv.pose_t, s, u);
+  for (int k = 0; rel && k < c.n_frames; ++k) inside = inside && spline_index(e->sp, c.t[k], s, u);
+  for (int slot = 0; points && slot < ctvio_engine::kFrameSlots; ++slot)
+    if (e->ft.held >> slot & 1u) inside = inside && spline_index(e->sp, e->h_frame_t[slot], s, u);
+  if (!inside) {
+    cv.status = CTVIO_ERR_TIME_RANGE;
+    cv.why = "a covariance time falls outside the spline";
+    return CTVIO_OK;
+  }
+  if (const int rc = cycle_covariance_enqueue(e, c.opt.covariance_gauge_knot, pose, rel, points)) return rc;
+  cv.pending = true;
+  return CTVIO_OK;
+}
+
+// after a stream synchronisation that follows start_covariances: the rank test on the published block
+int finish_covariances(ctvio_engine* e) {
+  auto& cv = e->cyc.cov;
+  if (!cv.pending) return CTVIO_OK;
+  cv.pending = false;
+  const LmPublished& pub = *const_cast<const LmPublished*>(&e->cyc.cov_host->pub);
+  if (*reinterpret_cast<const volatile unsigned long long*>(&pub.seq) != cv.seq)
+    return fail(CTVIO_ERR_CUDA, "the window covariance was not published before the cycle's synchronisation");
+  std::atomic_thread_fence(std::memory_order_acquire);
+  cv.rcond = pub.rcond;
+  cv.status = covariance_rank_test(pub, "window covariance", &cv.why);
+  if (cv.status == CTVIO_OK) cv.available = cv.requested & 3;  // the map's bit comes with the map
   return CTVIO_OK;
 }
 
@@ -261,6 +329,9 @@ int run_cycle(ctvio_engine* e, bool first, int32_t marg_flag_override, int64_t n
   e->launches += ctvio::launch_gauge_realign_snapshot(e->x[e->cur].ptrs(), e->nK, 0, c.snap.p, c.snap.p + 7, e->stream);
   e->table_valid = true;
   e->mirror_valid = false;
+  // the covariance publications, on the solved window's H: Sigma once, then its projections, all enqueued; the rank
+  // test is read after the slide's synchronisation below
+  if (c.cov.requested && (rc = start_covariances(e, max_t, n_lm))) return rc;
   r->n_frames = nf;
   r->n_knots = e->nK;
   r->knot_t0_ns = e->cfg.t0_ns;
@@ -305,21 +376,35 @@ int run_cycle(ctvio_engine* e, bool first, int32_t marg_flag_override, int64_t n
   r->n_knots_after = e->nK;
   for (int k = leave; k + 1 < nf; ++k) { c.slot[k] = c.slot[k + 1]; c.t[k] = c.t[k + 1]; }
   --c.n_frames;
-  // 14. the map of the post-slide window
+  // both branches have synchronised since step 9 (the feature table's slide reads its counts back)
+  if ((rc = finish_covariances(e))) return rc;
+  // 14. the map of the post-slide window, with each point's covariance when Sigma passed the rank test
   r->n_map_points = r->n_margin_points = 0;
   if (o.publish_map) {
     const bool pts = out && out->map_xyz && out->map_feature_id && out->map_in_margin_cloud;
+    const bool cov = (c.cov.requested & 4) && c.cov.status == CTVIO_OK;
     auto& t = e->ft;
-    if ((rc = ctvio_feature_table_map(e, c.n_frames, c.slot, o.window_size, pts ? out->map_capacity : 0, pts ? out->map_xyz : nullptr,
-                                      pts ? out->map_feature_id : nullptr, pts ? out->map_in_margin_cloud : nullptr,
-                                      &r->n_map_points, out ? out->cam_q_xyzw : nullptr, out ? out->cam_p_xyz : nullptr))) {
+    if ((rc = feature_table_map_body(e, c.n_frames, c.slot, o.window_size, pts ? out->map_capacity : 0, pts ? out->map_xyz : nullptr,
+                                     pts ? out->map_feature_id : nullptr, pts ? out->map_in_margin_cloud : nullptr,
+                                     &r->n_map_points, out ? out->cam_q_xyzw : nullptr, out ? out->cam_p_xyz : nullptr,
+                                     cov ? cycle_point_covariances(e) : nullptr, cov ? c.cov.n_lm : 0,
+                                     cov ? &c.cov_host->map_cov9[0] : nullptr))) {
       if (!(rc == CTVIO_ERR_INVALID && !pts)) return rc;  // a map without point buffers: only the count is wanted
     }
     int nm = 0;
     for (int k = 0; k < r->n_map_points; ++k) nm += t.h_map_points[k].in_margin_cloud ? 1 : 0;
     r->n_margin_points = nm;
     if (!pts) e->d2h_bytes -= sizeof(ctvio::MapPoint) * size_t(r->n_map_points);  // the points stayed in the mapped buffer
+    if (cov) {
+      int nan_rows = 0;
+      for (int k = 0; k < r->n_map_points; ++k) nan_rows += std::isnan(c.cov_host->map_cov9[9 * size_t(k)]) ? 1 : 0;
+      c.cov.n_map = r->n_map_points;
+      c.cov.n_map_nan = nan_rows;
+      c.cov.available |= 4;
+    }
   }
+  c.cov.ran = true;
+  if (!c.cov.requested) c.cov.why = "the cycle's options publish no covariances";
   return CTVIO_OK;
 }
 
@@ -343,6 +428,7 @@ int ctvio_cycle_default_options(ctvio_cycle_options* o) {
   o->sigma_ab_discrete = 4.0e-4;
   o->reanchor = 0;
   o->publish_map = 1;
+  o->covariance_gauge_knot = 3;
   return CTVIO_OK;
 }
 
@@ -365,6 +451,7 @@ int ctvio_odometry_start(ctvio_handle e, const ctvio_cycle_options* opt, int64_t
   // a fresh run: feature table, frame slots, IMU table and prior start empty
   c.started = false;
   c.opt = *opt;
+  clear_covariances(e);
   c.n_frames = 0;
   c.next_frame = 0;
   e->ft.held = 0;
@@ -409,6 +496,7 @@ int ctvio_process_image(ctvio_handle e, const ctvio_image_msg* img, const ctvio_
   cudaSetDevice(e->cfg.device);
   std::memset(r, 0, sizeof(*r));
   c.started = false;  // until the cycle completes
+  clear_covariances(e);
   // 1. the cloud joins the window and the feature table
   if ((rc = take_image(e, slot, img))) return rc;
   r->frame_slot = slot;
@@ -420,6 +508,43 @@ int ctvio_process_image(ctvio_handle e, const ctvio_image_msg* img, const ctvio_
   if (!rc) c.started = true;
   r->host_ms = std::chrono::duration<double, std::milli>(Clock::now() - t_start).count();
   return rc;
+}
+
+int ctvio_cycle_covariances(ctvio_handle e, double* cov12, int64_t* pose_t_ns, double* cov6, int64_t* pair_t_ns,
+                            int32_t map_capacity, double* map_cov9, ctvio_cycle_covariance_info* info) {
+  if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
+  if (map_capacity < 0) return fail(CTVIO_ERR_INVALID, "map_capacity must be >= 0");
+  const auto& cv = e->cyc.cov;
+  const bool ok = cv.ran && cv.available;
+  const int n_pairs = (ok && (cv.available & 2)) ? cv.n_frames - 1 : 0;
+  const int n_map = (ok && (cv.available & 4)) ? cv.n_map : 0;
+  if (info) {
+    std::memset(info, 0, sizeof(*info));
+    info->requested = cv.requested;
+    info->available = ok ? cv.available : 0;
+    info->status = cv.ran ? cv.status : CTVIO_ERR_STATE;
+    info->gauge_knot = e->cyc.opt.covariance_gauge_knot;
+    info->rcond = cv.ran ? cv.rcond : NAN;
+    info->pose_t_ns = cv.pose_t;
+    info->n_pairs = n_pairs;
+    info->n_map_points = n_map;
+    info->n_map_points_without_cov = (ok && (cv.available & 4)) ? cv.n_map_nan : 0;
+  }
+  if (!ok) return fail(CTVIO_ERR_STATE, "ctvio_cycle_covariances: not available: " + cv.why);
+  if (map_cov9 && map_capacity < n_map)
+    return fail(CTVIO_ERR_INVALID, "ctvio_cycle_covariances: map_capacity is smaller than the map's point count");
+  const CycleCovHost* h = e->cyc.cov_host;
+  if (cv.available & 1) {
+    if (cov12) std::memcpy(cov12, h->cov12, 144 * sizeof(double));
+    if (pose_t_ns) *pose_t_ns = cv.pose_t;
+  }
+  if (cov6) std::memcpy(cov6, h->cov6, 36 * size_t(n_pairs) * sizeof(double));
+  for (int k = 0; pair_t_ns && k < n_pairs; ++k) {
+    pair_t_ns[2 * k] = cv.frame_t[k];
+    pair_t_ns[2 * k + 1] = cv.frame_t[k + 1];
+  }
+  if (map_cov9) std::memcpy(map_cov9, h->map_cov9, 9 * size_t(n_map) * sizeof(double));
+  return CTVIO_OK;
 }
 
 int ctvio_debug_bias_weights(ctvio_handle e, int32_t n_kf, const int64_t* kf_t, double sigma_wb, double sigma_ab,

@@ -548,6 +548,18 @@ int ctvio_feature_table_landmarks(ctvio_handle e, int32_t n_landmarks, int32_t* 
 int ctvio_feature_table_map(ctvio_handle e, int32_t n_frames, const int32_t* frame_slots, int32_t window_size,
                             int32_t capacity, double* xyz_world, int32_t* feature_id, uint8_t* in_margin_cloud,
                             int32_t* n_points, double* cam_q_xyzw, double* cam_p_xyz) {
+  return feature_table_map_body(e, n_frames, frame_slots, window_size, capacity, xyz_world, feature_id, in_margin_cloud,
+                                n_points, cam_q_xyzw, cam_p_xyz, nullptr, 0, nullptr);
+}
+
+}  // extern "C"
+
+namespace ctvio::host {
+
+int feature_table_map_body(ctvio_engine* e, int32_t n_frames, const int32_t* frame_slots, int32_t window_size,
+                           int32_t capacity, double* xyz_world, int32_t* feature_id, uint8_t* in_margin_cloud,
+                           int32_t* n_points, double* cam_q_xyzw, double* cam_p_xyz, const double* lm_cov9, int32_t n_cov,
+                           double* point_cov9) {
   if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
   if (!frame_slots || !n_points) return fail(CTVIO_ERR_INVALID, "null argument");
   if (n_frames < 1 || n_frames > ctvio_engine::kFrameSlots) return fail(CTVIO_ERR_INVALID, "n_frames must be 1..16");
@@ -584,12 +596,14 @@ int ctvio_feature_table_map(ctvio_handle e, int32_t n_frames, const int32_t* fra
   a.st = e->x[e->cur].ptrs(); a.sp = e->sp; a.R_CI = e->rig.R_CI; a.p_CI = e->rig.p_CI;
   a.rho = e->x[e->cur].rho.p; a.n_rho = std::max(t.n_lm, 0);
   a.head = t.h_map_head; a.points = t.h_map_points;
+  a.lm_cov9 = lm_cov9; a.n_cov = n_cov; a.point_cov9 = point_cov9;
   // the slot list goes with the launch parameters; the kernel writes the result straight into mapped host memory
-  e->launches += ctvio::launch_feature_table_map(a, st);
+  e->launches += point_cov9 ? ctvio::launch_feature_table_map_cov(a, st) : ctvio::launch_feature_table_map(a, st);
   CUDA_OK(stream_sync(st));
   const ctvio::MapHeader& h = *t.h_map_head;
   const int n = h.n_points;
   e->d2h_bytes += 8 + 56 * size_t(n_frames) + sizeof(ctvio::MapPoint) * size_t(n);
+  if (point_cov9) e->d2h_bytes += 9 * sizeof(double) * size_t(n);
   *n_points = n;
   if (n > capacity) return fail(CTVIO_ERR_INVALID, "capacity is smaller than the number of map points");
   for (int k = 0; k < n; ++k) {
@@ -604,6 +618,10 @@ int ctvio_feature_table_map(ctvio_handle e, int32_t n_frames, const int32_t* fra
   }
   return CTVIO_OK;
 }
+
+}  // namespace ctvio::host
+
+extern "C" {
 
 int ctvio_check_keyframe(ctvio_handle e, int32_t n_frames, const int32_t* frame_slots, double min_parallax,
                          int32_t* is_keyframe, int32_t* n_tracked, int32_t* parallax_num, double* parallax_sum) {

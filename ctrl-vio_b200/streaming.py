@@ -1028,13 +1028,22 @@ class CycleRunner:
     Options as ResidentRunner's: second_new_every (through marg_flag_override), min_parallax (the device's keyframe
     decision), publish_map, reanchor, iters / init_iters.  want_knots / want_map=False leave the knot / map outputs
     unrequested (the trajectory is then not carried into q / p, and last_map stays None).  Not supported: the host
-    association (device_features=False), the rho0 mode (triangulate=False), predictor=False, the covariance
-    publications and a perm_seed."""
+    association (device_features=False), the rho0 mode (triangulate=False), predictor=False and a perm_seed.
+
+    covariances: any subset of ("pose", "odometry", "map") ("map" requires publish_map=True), the library's covariance
+    publications (ctvio_cycle_covariances): the window covariance is formed once per image, with the gauge of
+    ResidentRunner (knots 0..3, opt.covariance_gauge_knot), and projected to ResidentRunner's three publications.
+    They are kept on last_pose_cov [1, 12, 12], last_rel_cov [n_frames - 1, 6, 6] and last_map_cov [n_points, 3, 3]
+    (None when the cycle could not form them), and the record gains pose_cov_rcond / rel_cov_rcond / point_cov_rcond
+    (nan with *_error when the window is rank deficient) and n_map_points_without_cov.  ResidentRunner's
+    publish_*covariance keywords are not taken: name the publications in covariances instead."""
+
+    COVARIANCES = ("pose", "odometry", "map")
 
     def __init__(self, lib, seq, iters=15, init_iters=8, device=0, second_new_every=0, min_parallax=None,
                  publish_map=False, reanchor=False, want_knots=True, want_map=True, triangulate=True,
                  device_features=True, predictor=True, perm_seed=None, publish_covariance=False,
-                 publish_map_covariance=False, publish_odometry_covariance=False):
+                 publish_map_covariance=False, publish_odometry_covariance=False, covariances=()):
         from . import binding, make_config
         if not triangulate or not device_features:
             raise ValueError("CycleRunner runs the device feature table with triangulation only "
@@ -1044,7 +1053,16 @@ class CycleRunner:
         if perm_seed is not None:
             raise ValueError("CycleRunner takes the factors from the resident tables: no perm_seed")
         if publish_covariance or publish_map_covariance or publish_odometry_covariance:
-            raise ValueError("CycleRunner does not publish covariances: use ResidentRunner or the separate calls")
+            raise ValueError("CycleRunner takes the covariance publications as covariances=('pose', 'odometry', 'map'), "
+                             "not as ResidentRunner's publish_*covariance keywords")
+        if isinstance(covariances, str):
+            raise ValueError("covariances is a collection of names, e.g. covariances=('pose',)")
+        covariances = tuple(covariances)
+        unknown = [c for c in covariances if c not in self.COVARIANCES]
+        if unknown:
+            raise ValueError(f"unknown covariances {unknown}: pick from {self.COVARIANCES}")
+        if "map" in covariances and not publish_map:
+            raise ValueError("covariances=('map', ...) requires publish_map=True: the covariances belong to the map's points")
         if min_parallax is not None and second_new_every:
             raise ValueError("min_parallax and second_new_every both choose the branch: pick one")
         if min_parallax is not None and not min_parallax > 0:
@@ -1071,8 +1089,14 @@ class CycleRunner:
         self.opt.sigma_wb_discrete, self.opt.sigma_ab_discrete = syn.SIGMA_BG, syn.SIGMA_BA
         self.opt.reanchor = int(reanchor)
         self.opt.publish_map = int(publish_map)
+        self.covariances = covariances
+        self.opt.publish_pose_covariance = int("pose" in covariances)
+        self.opt.publish_odometry_covariance = int("odometry" in covariances)
+        self.opt.publish_map_covariance = int("map" in covariances)
         self.reanchor, self.publish_map = reanchor, publish_map
         self.last_map = None
+        self.last_pose_cov = self.last_rel_cov = self.last_map_cov = None
+        self.last_cov_info = None
         self.records = []
         self.step_index = 0
         self.imu_sent = 0
@@ -1110,6 +1134,7 @@ class CycleRunner:
             res, arr = e.ProcessImage(t_newest, self.clouds.message(self.frames[-1]), imu,
                                       marg_flag_override=self._override(), want_knots=self.want_knots,
                                       want_map=self.want_map)
+        cov_rec = self._covariances(res["n_map_points"]) if self.covariances else None
         t_wall = time.perf_counter() - t0
         h2d, d2h = e.TransferStats(reset=True)
         marg_flag = res["marg_flag"]
@@ -1135,8 +1160,26 @@ class CycleRunner:
             rec.update(n_reanchored=res["n_reanchored"])
         if self.publish_map:
             rec.update(n_map_points=res["n_map_points"], n_margin_points=res["n_margin_points"])
+        if cov_rec is not None:
+            rec.update(cov_rec)
         self.records.append(rec)
         self.step_index += 1
+        return rec
+
+    def _covariances(self, n_map_points):
+        """the last cycle's covariance publications onto last_*_cov, and their record entries"""
+        cov12, cov6, cov9, info = self.est.CycleCovariances()
+        self.last_cov_info = info
+        self.last_pose_cov = None if cov12 is None else cov12[None]
+        self.last_rel_cov, self.last_map_cov = cov6, cov9
+        rec = {}
+        for name, key, got in (("pose", "pose_cov", cov12), ("odometry", "rel_cov", cov6), ("map", "point_cov", cov9)):
+            if name in self.covariances:
+                rec[key + "_rcond"] = info["rcond"] if got is not None else float("nan")
+                if got is None:
+                    rec[key + "_error"] = info.get("error", "")
+        if "map" in self.covariances:
+            rec["n_map_points_without_cov"] = info["n_map_points_without_cov"] if cov9 is not None else n_map_points
         return rec
 
     def run(self, n_windows, first=0):

@@ -605,8 +605,9 @@ int ctvio_sync_stats(ctvio_handle h, int64_t* host_waits, int32_t reset);
  * The resident window (SURVEY §8f-1) driven as the reference drives it after every image, with every stage of the
  * section above in the reference's order and the bookkeeping a caller of those calls keeps itself (frame slots, the
  * window's frames and frame times, the knot range of each frame, bias nodes) held by the library.  The caller passes
- * only messages: the tracker's PointClouds and the IMUData records.  Not covered: the covariance publications, the
- * host-association and rho0 modes of the separate calls, sharded engines and the initialisers.
+ * only messages: the tracker's PointClouds and the IMUData records.  The cycle can also publish the uncertainty of what
+ * it publishes (ctvio_cycle_covariances).  Not covered: the host-association and rho0 modes of the separate calls,
+ * sharded engines and the initialisers.
  * Every image takes a frame slot: frame f (counting the frames since ctvio_odometry_start, the first one 0) takes slot
  * f % 16 when the feature table does not hold it, else the lowest free slot. */
 
@@ -649,7 +650,12 @@ typedef struct ctvio_cycle_options {
   int32_t reanchor;             /* the feature list slides as the reference's does (ctvio_feature_table_slide_reanchor)
                                    instead of dropping a landmark with its anchor frame (ctvio_feature_table_slide) [0] */
   int32_t publish_map;          /* ctvio_feature_table_map of the post-slide window after every image         [1]   */
-  int32_t reserved[4];
+  /* the covariance publications (ctvio_cycle_covariances), each 0 or 1: */
+  int32_t publish_pose_covariance;     /* the camera pose and velocity at the TF time, 12 x 12                  [0]   */
+  int32_t publish_odometry_covariance; /* the relative camera pose of each consecutive frame pair, 6 x 6         [0]   */
+  int32_t publish_map_covariance;      /* each map point's world point, 3 x 3; requires publish_map             [0]   */
+  int32_t covariance_gauge_knot;       /* -1..3: knots <= it are held constant for the covariances only (the
+                                          gauge_knot_index of the separate calls)                               [3]   */
 } ctvio_cycle_options;
 
 /* Optional outputs; a NULL pointer means the output is not wanted. */
@@ -692,6 +698,21 @@ typedef struct ctvio_cycle_result {
 
 /* the defaults in brackets above */
 int ctvio_cycle_default_options(ctvio_cycle_options* opt);
+/* What ctvio_cycle_covariances returns besides the matrices. */
+typedef struct ctvio_cycle_covariance_info {
+  int32_t requested;        /* the last cycle's publications (bits): 1 pose, 2 odometry edges, 4 map points     */
+  int32_t available;        /* the same bits for what it published; 0 when ctvio_cycle_covariances fails        */
+  int32_t status;           /* CTVIO_OK when available; CTVIO_ERR_STATE: rank deficient, nothing requested or no
+                               completed cycle; CTVIO_ERR_TIME_RANGE: a time outside the spline or the evaluation */
+  int32_t gauge_knot;       /* covariance_gauge_knot of the run                                                  */
+  double rcond;             /* of the window covariance, as ctvio_covariance reports it; NaN when not formed     */
+  int64_t pose_t_ns;        /* the TF time of cov12                                                              */
+  int32_t n_pairs;          /* rows of cov6 / pair_t_ns (0 unless the odometry edges are available)              */
+  int32_t n_map_points;     /* rows of map_cov9: the cycle's map points (0 unless the map's are available)      */
+  int32_t n_map_points_without_cov; /* of those, the rows of NaN                                                  */
+  int32_t reserved;
+} ctvio_cycle_covariance_info;
+
 /* ctvio_odometry_start - SetInitialState + InitWindow + the first UpdateTrajectory (odometry_manager.cpp:230-264), which
  *   runs no predictor (first_opt_flag): the initializer's window of n_frames = window_size + 1 images goes up once.
  *   Knots q_xyzw / p_xyz [n_knots] start at t0_ns (knot 0, on the configured knot grid), bg_ba6 [n_frames] holds one
@@ -730,6 +751,7 @@ int ctvio_odometry_start(ctvio_handle h, const ctvio_cycle_options* opt, int64_t
  *   12. SlideWindow: ctvio_slide_window(knots of the oldest frame, 1, 1) or ctvio_slide_window_second_new;
  *   13. without reanchor: ctvio_feature_table_slide of the leaving frame's slot;
  *   14. publish_map: ctvio_feature_table_map of the post-slide window.
+ *   With a publish_*_covariance flag set, the covariances of ctvio_cycle_covariances are formed right after step 9.
  *   Computed on the device from what it already holds, where a caller of the separate calls computes them on the host:
  *   - the bias random-walk weights (trajectory_manager.cpp:420-450): for frames i, i+1, with s2 the sum of dt^2 over the
  *     IMU intervals that start at or after frame i's time and end before frame i+1's, sqrt_info = 1 / sqrt(s2 sigma^2)
@@ -741,13 +763,37 @@ int ctvio_odometry_start(ctvio_handle h, const ctvio_cycle_options* opt, int64_t
  *   the LM step scalars, the marginalization's block bookkeeping.
  *   Errors (through ctvio_last_error): CTVIO_ERR_INVALID for a NULL handle, options (start) or result, options out of
  *   range (window_size outside 2..15, iterations < 1 or predictor_iterations < 0, init_depth not finite and > 0,
- *   extend_ns <= 0, a min_parallax that is not finite), a bad message (NULL arrays, n_points outside 0..1024) or IMU
+ *   extend_ns <= 0, a min_parallax that is not finite, a publish_*_covariance flag other than 0 / 1,
+ *   covariance_gauge_knot outside -1..3, publish_map_covariance without publish_map), a bad message (NULL arrays, n_points outside 0..1024) or IMU
  *   layout (as ctvio_ingest_imu), marg_flag_override outside -1..1; CTVIO_ERR_STATE before ctvio_odometry_start, on a
  *   sharded engine (world > 1), or when the feature table holds all 16 frame slots so the image has none.  These are
  *   checked before any device work and leave the engine unchanged.  An error of a stage (CTVIO_ERR_TIME_RANGE, ...)
  *   stops the cycle there; the engine must then be restarted with ctvio_odometry_start. */
 int ctvio_process_image(ctvio_handle h, const ctvio_image_msg* img, const ctvio_imu_msgs* imu, int32_t marg_flag_override,
                         ctvio_cycle_outputs* out, ctvio_cycle_result* result);
+/* ctvio_cycle_covariances - the covariances the last ctvio_odometry_start / ctvio_process_image published, with the
+ *   options' publish_*_covariance flags.  The cycle forms them right after step 9, on the solved window's H, before
+ *   the marginalization and the slide change it: the window covariance Sigma once (as ctvio_covariance forms it, with
+ *   the knots <= covariance_gauge_knot held constant), then its projections on the device, all in the camera frame:
+ *   - cov12 [12][12]: ctvio_pose_covariance at pose_t_ns = the solved window's maxTimeNs() - 50 ms, the time of the
+ *     reference's TF (odometry_manager.cpp:287-288);
+ *   - cov6 [n_pairs][6][6]: ctvio_relative_pose_covariance of the solved window's consecutive frames, pair_t_ns
+ *     [n_pairs][2] their times (the odometry edges a pose graph fuses);
+ *   - map_cov9 [n_map_points][3][3]: the covariance of each point of that cycle's map output, in its order: the
+ *     point's matrix from ctvio_feature_table_point_covariance by the entry's number in the solved window, attached by
+ *     the map kernel.  A point without a number there, or re-anchored by the slide (reanchor), gets NaNs.
+ *   Sigma never leaves the device, and the cycle waits for nothing more: the rank test (as ctvio_covariance's) reads
+ *   its inputs after the synchronisation the slide makes anyway.  A rank-deficient window does not stop the cycle:
+ *   info->status is CTVIO_ERR_STATE with info->rcond, and nothing is available.
+ *   Every pointer but the handle may be NULL.  The call copies from host memory the cycle filled: no device work, no
+ *   synchronisation.  Each cycle clears what the last one published before it starts.
+ *   Errors (info, when given, is filled first): CTVIO_ERR_INVALID for a NULL handle, a negative map_capacity, or a
+ *   map_capacity below n_map_points with map_cov9; CTVIO_ERR_STATE "not available" before any cycle, after a cycle
+ *   that stopped on an error or published nothing (flags off, rank deficient, ...).
+ *   ctvio_transfer_stats counts, in the cycle: 8 bytes up for the TF time and 8 n_frames for the frame times, 1152
+ *   bytes down for cov12, 288 n_pairs for cov6 and 72 n_map_points for map_cov9. */
+int ctvio_cycle_covariances(ctvio_handle h, double* cov12, int64_t* pose_t_ns, double* cov6, int64_t* pair_t_ns,
+                            int32_t map_capacity, double* map_cov9, ctvio_cycle_covariance_info* info);
 /* test support: the bias random-walk weights ctvio_process_image computes, for the keyframe times kf_t_ns[0 .. n_kf-1]
  *   (2..16, ascending) over the resident IMU table as the last cycle left it; sqrt_info6 [n_kf - 1][6]. */
 int ctvio_debug_bias_weights(ctvio_handle h, int32_t n_kf, const int64_t* kf_t_ns, double sigma_wb_discrete,
