@@ -175,7 +175,7 @@ ABI_SYMBOLS = [
     "feature_table_add", "feature_table_window", "triangulate_window_from_table", "add_image_features_from_table",
     "feature_table_slide", "feature_table_landmarks", "feature_table_map", "feature_table_slide_reanchor",
     "debug_structure", "feature_table_point_covariance", "sync_stats", "cycle_default_options", "odometry_start",
-    "process_image", "debug_bias_weights", "cycle_covariances",
+    "process_image", "debug_bias_weights", "cycle_covariances", "odometry_checkpoint", "odometry_restore",
 ]
 
 
@@ -190,7 +190,13 @@ DEVICE_ONLY_SYMBOLS = ("nccl_unique_id", "comm_init", "set_deterministic", "enab
                        "feature_table_map", "feature_table_slide_reanchor", "debug_structure", "covariance",
                        "pose_covariance", "relative_pose_covariance", "point_covariance", "feature_table_point_covariance",
                        "sync_stats", "cycle_default_options", "odometry_start", "process_image", "debug_bias_weights",
-                       "cycle_covariances")
+                       "cycle_covariances", "odometry_checkpoint", "odometry_restore")
+
+# ctypes prototypes of the entry points whose arguments ctypes must convert on its own (include/ctvio.h)
+PROTOTYPES = {
+    "odometry_checkpoint": [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)],
+    "odometry_restore": [C.c_void_p, C.c_void_p, C.c_int64],
+}
 
 
 def _addr(a):
@@ -238,6 +244,8 @@ class CtvioLib:
         for name, f in self._fn.items():
             if name != "last_error":
                 f.restype = C.c_int
+            if name in PROTOTYPES:
+                f.argtypes = PROTOTYPES[name]
 
     def has(self, name):
         return name in self._fn
@@ -803,6 +811,24 @@ class Estimator:
         d["pair_t_ns"] = pair_t[:info.n_pairs].copy()
         return (cov12 if a & 1 else None, cov6[:info.n_pairs].copy() if a & 2 else None,
                 cov9[:info.n_map_points].copy() if a & 4 else None, d)
+
+    # the blob's header size: the counts section follows it and starts with nK, nB, nL (int32)
+    CHECKPOINT_HEADER_BYTES = 40 + 16 * 21
+
+    def Checkpoint(self) -> bytes:
+        """ctvio_odometry_checkpoint: the odometry cycle's run as one blob (ctvio_odometry_restore continues it)."""
+        n = C.c_int64()
+        self.lib.call("odometry_checkpoint", self.h, None, 0, C.byref(n))
+        buf = C.create_string_buffer(n.value)
+        self.lib.call("odometry_checkpoint", self.h, buf, n.value, C.byref(n))
+        return buf.raw[:n.value]
+
+    def Restore(self, blob: bytes):
+        """ctvio_odometry_restore: replace this engine's run with the blob's; the next call is ProcessImage."""
+        blob = bytes(blob)
+        self.lib.call("odometry_restore", self.h, blob, len(blob))
+        nK, nB, nL = np.frombuffer(blob, np.int32, 3, self.CHECKPOINT_HEADER_BYTES).tolist()
+        self.n_knots, self.n_bias, self.n_lm = nK, nB, nL
 
     def DebugBiasWeights(self, kf_times, sigma_wb, sigma_ab):
         """(test support) the bias random-walk weights of ctvio_process_image for these keyframe times over the resident

@@ -759,6 +759,8 @@ int ctvio_destroy(ctvio_handle e) {
   if (e->h_mirror) cudaFreeHost(e->h_mirror);
   if (e->ft.h_map_head) cudaFreeHost(e->ft.h_map_head);
   if (e->cyc.cov_host) cudaFreeHost(e->cyc.cov_host);
+  if (e->ckpt.h_stage) cudaFreeHost(e->ckpt.h_stage);
+  if (e->ckpt.h_verdict) cudaFreeHost(e->ckpt.h_verdict);
   if (e->ev_zero) cudaEventDestroy(e->ev_zero);
   cudaEventDestroy(e->ev0);
   cudaEventDestroy(e->ev1);

@@ -340,6 +340,17 @@ struct ctvio_engine {
     CycleCovHost* cov_host = nullptr;
     CycleCovState cov;
   } cyc;
+  // ctvio_odometry_checkpoint / ctvio_odometry_restore (checkpoint.cu): the blob's device and pinned staging, the
+  // checksum's per-CTA partial sums and ticket, and the restore's verdict (pinned + mapped).  Scratch only: a restore
+  // writes the engine's run only after the verdict passed.
+  struct CkptWs {
+    DevBuf<unsigned char> stage;
+    DevBuf<unsigned long long> partial;
+    DevBuf<int32_t> ticket;        // zeroed once; the last CTA of every launch resets it
+    unsigned char* h_stage = nullptr;
+    size_t h_cap = 0;
+    int32_t* h_verdict = nullptr;
+  } ckpt;
   int n_marg_img = -1;  // marginalized image factors of the last ctvio_marginalize (-1: pos_cam / pos_lm / marg_img not built)
 
   // multi-GPU
@@ -387,6 +398,11 @@ inline int ensure_table(ctvio_engine* e) {
 
 // structure.cu: the structure build of a factor set with device-resident descriptors (T: tiles per side of the reduced
 // system).  structure_build_device reads back the one count block; schur_lists_device fills the K4 lists it sized.
+// resident.cu: the resident feature table's arrays, at full size, on first use
+int ensure_feature_table(ctvio_engine* e);
+// odometry.cu: ctvio_odometry_start's option checks (also applied to a checkpoint's options by ctvio_odometry_restore)
+int check_cycle_options(const ctvio_cycle_options* o);
+
 int structure_build_device(ctvio_engine* e, int T);
 int schur_lists_device(ctvio_engine* e, int T);
 // ctvio_marginalize's image part: marg_img, pos_lm relative to the first inverse-depth position (offset_pos_lm_device

@@ -410,6 +410,8 @@ int run_cycle(ctvio_engine* e, bool first, int32_t marg_flag_override, int64_t n
 
 }  // namespace
 
+int ctvio::host::check_cycle_options(const ctvio_cycle_options* o) { return check_options(o); }
+
 extern "C" {
 
 int ctvio_cycle_default_options(ctvio_cycle_options* o) {

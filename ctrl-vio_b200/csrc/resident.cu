@@ -77,8 +77,10 @@ int triangulate_window_device(ctvio_engine* e, int nl, const int32_t* d_off, con
   return CTVIO_OK;
 }
 
+}  // namespace
+
 // the resident feature table's arrays, at full size (kFeatureTableMaxEntries entries), on first use
-int ensure_feature_table(ctvio_engine* e) {
+int ctvio::host::ensure_feature_table(ctvio_engine* e) {
   auto& t = e->ft;
   if (t.id.p) return CTVIO_OK;
   const size_t cap = ctvio::kFeatureTableMaxEntries, slots = ctvio_engine::kFrameSlots;
@@ -92,6 +94,8 @@ int ensure_feature_table(ctvio_engine* e) {
   CUDA_OK(t.desc.reserve((slots - 1) * cap));
   return CTVIO_OK;
 }
+
+namespace {
 
 // room for n descriptors in the factor set's device-side list, keeping the ones it holds
 int reserve_device_descriptors(ctvio_engine* e, size_t n) {

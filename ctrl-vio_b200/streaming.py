@@ -1182,6 +1182,33 @@ class CycleRunner:
             rec["n_map_points_without_cov"] = info["n_map_points_without_cov"] if cov9 is not None else n_map_points
         return rec
 
+    def checkpoint(self):
+        """The run after the last step(): the library's blob (ctvio_odometry_checkpoint) with the runner's own host-side
+        counters and carried trajectory, as a dict for restore() / resume()."""
+        return dict(blob=self.est.Checkpoint(), frames=list(self.frames), next_frame=self.next_frame,
+                    imu_sent=self.imu_sent, step_index=self.step_index, ncp=self.ncp, q=self.q.copy(), p=self.p.copy(),
+                    ld=self.ld)
+
+    def restore(self, state):
+        """Continue from a checkpoint() on this runner's engine: the next step() is the image after it.  The records
+        and the last publications of the steps since are dropped."""
+        if state["step_index"] < 1:
+            raise ValueError("a checkpoint is taken after a step")
+        self.est.Restore(state["blob"])
+        self.frames = list(state["frames"])
+        self.next_frame, self.imu_sent = state["next_frame"], state["imu_sent"]
+        self.step_index, self.ncp = state["step_index"], state["ncp"]
+        self.q, self.p, self.ld = state["q"].copy(), state["p"].copy(), state["ld"]
+        self.records = []
+        self.last_map = self.last_pose_cov = self.last_rel_cov = self.last_map_cov = self.last_cov_info = None
+        return self
+
+    @classmethod
+    def resume(cls, lib, seq, state, **kw):
+        """A runner on a fresh engine that continues a checkpoint() of a run over `seq`; kw: the options of that run
+        (the engine's deterministic mode is not part of the checkpoint)."""
+        return cls(lib, seq, **kw).restore(state)
+
     def run(self, n_windows, first=0):
         for _ in range(n_windows):
             self.step()

@@ -794,6 +794,42 @@ int ctvio_process_image(ctvio_handle h, const ctvio_image_msg* img, const ctvio_
  *   bytes down for cov12, 288 n_pairs for cov6 and 72 n_map_points for map_cov9. */
 int ctvio_cycle_covariances(ctvio_handle h, double* cov12, int64_t* pose_t_ns, double* cov6, int64_t* pair_t_ns,
                             int32_t map_capacity, double* map_cov9, ctvio_cycle_covariance_info* info);
+/* ctvio_odometry_checkpoint - the run of the odometry cycle as one self-describing blob, from which
+ *   ctvio_odometry_restore continues it on this or another engine: a later ctvio_process_image computes, bit for bit,
+ *   what it computes on the engine that took the checkpoint.  Valid after any ctvio_odometry_start /
+ *   ctvio_process_image that returned CTVIO_OK.
+ *   The blob holds what the next cycle reads: the knots, bias nodes, inverse depths and line delay with their counts,
+ *   the time origin as the slides moved it, the active prior (J, r, x0, block lists, whether it is enabled), the clouds
+ *   of the frame slots the feature table holds (up to each point count) with their times, the live rows of the
+ *   resident IMU table with their dt^2 prefix values and the prefix carry, the feature table's live entries (id, anchor,
+ *   number, per-slot feature indices, masks, inverse depths, sorted keys) and counts, and the cycle's options, window
+ *   frames and frame counter.  Not held: what the next call rebuilds (factor structures, knot-pair table, scales,
+ *   workspaces), the last cycle's covariance publications, and the engine's deterministic mode.
+ *   Format: little-endian; a magic number, the format version (1), CTVIO_ABI_VERSION, the length, a 64-bit checksum
+ *   of everything after the header, a section table, then the counts and the configuration (ctvio_config without
+ *   device), the prior's block lists and the device sections.  The device sections are gathered by one kernel
+ *   launch into a staging buffer that also sums their checksum terms, then come back in one copy.
+ *   buf NULL: only *len is written (the size the checkpoint needs; no device work).  Otherwise the blob's *len bytes are
+ *   written to buf.
+ *   Transfers: *len bytes down, nothing up.  Synchronises the engine stream once.
+ *   Errors (nothing is written but *len): CTVIO_ERR_INVALID for a NULL len, capacity < 0, a NULL handle, or (buf
+ *   given) capacity below the size needed; CTVIO_ERR_STATE before ctvio_odometry_start, after a cycle that stopped on
+ *   an error, on a sharded engine, or when the active prior came from ctvio_set_prior after the cycle. */
+int ctvio_odometry_checkpoint(ctvio_handle h, void* buf, int64_t capacity, int64_t* len);
+/* ctvio_odometry_restore - replaces the engine's run, if any, with the one of a blob of ctvio_odometry_checkpoint; the
+ *   next call is ctvio_process_image.  The engine must have been created with an equal configuration (every
+ *   ctvio_config field but device and t0_ns; the blob's time origin must lie on the engine's knot grid); the device
+ *   ordinal may differ.  The engine keeps its deterministic mode.  Until the next cycle, ctvio_cycle_covariances
+ *   reports "not available" and ctvio_get_prior "no prior has been produced".
+ *   The host checks the header, counts and section table; the blob then goes up in one copy, and a kernel recomputes
+ *   the checksum and checks the section table on the device, into scratch buffers.  Only a blob that passes is
+ *   written into the engine's buffers (a second launch), so a refused blob leaves the engine's run bitwise unchanged.
+ *   Transfers: len bytes up, the device check's 4-byte verdict down.  Synchronises the engine stream once.
+ *   Errors: CTVIO_ERR_INVALID for len < 0, a NULL buf with len > 0, a NULL handle, a malformed blob (bad magic number,
+ *   a format version other than 1, another CTVIO_ABI_VERSION, a length other than the blob's, counts or a section
+ *   table that do not agree, a checksum mismatch) or a configuration that differs from the engine's; CTVIO_ERR_STATE
+ *   on a sharded engine.  All of them leave the engine unchanged. */
+int ctvio_odometry_restore(ctvio_handle h, const void* buf, int64_t len);
 /* test support: the bias random-walk weights ctvio_process_image computes, for the keyframe times kf_t_ns[0 .. n_kf-1]
  *   (2..16, ascending) over the resident IMU table as the last cycle left it; sqrt_info6 [n_kf - 1][6]. */
 int ctvio_debug_bias_weights(ctvio_handle h, int32_t n_kf, const int64_t* kf_t_ns, double sigma_wb_discrete,
