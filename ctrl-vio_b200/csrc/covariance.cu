@@ -56,22 +56,6 @@ __device__ __forceinline__ void frag_store_global(double* dst, int ld, const Fra
       *reinterpret_cast<double2*>(dst + size_t(L.row(mt)) * ld + L.col(nt)) = make_double2(f.c[mt][nt][0], f.c[mt][nt][1]);
 }
 
-__device__ __forceinline__ double warp_min_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-__device__ __forceinline__ double warp_max_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // lane's part of sum_b row[col_b] w_b over a landmark's coupling row: its n knot dims lo .. lo + n - 1, then the line
 // delay (b = n).  Lane b takes b, b + 32, ... in order; the caller finishes with one fixed shuffle tree.
 __device__ __forceinline__ double coupling_dot_part(const double* row, int lo, int n, int ld, const double* Wl, double wld,
@@ -79,6 +63,61 @@ __device__ __forceinline__ double coupling_dot_part(const double* row, int lo, i
   double s = 0.0;
   for (int b = lane; b <= n; b += 32) s = fma(row[b < n ? lo + b : ld], b < n ? Wl[b] : wld, s);
   return s;
+}
+
+// The projections C = G Sigma_blk G' of the window covariance (pose_cov_kernel, point_cov_kernel,
+// relative_pose_cov_kernel), one warp each: the block of Sigma, then T = G Sigma_blk (warp_mul), then C = T G'
+// (warp_mul_t), every entry one fixed-order fma chain (from 0, k ascending), no atomics.
+
+// S[i * ld + j] = Sigma at dims i, j < m of the union of segments sa and sb (relative_union_knot), m = 6 (4 + off); M: m
+// when it is known at compile time.  sa == sb is the 24 x 24 block at the contiguous dims 6 sa .. 6 sa + 23.  Dim i of
+// the union is 6 lo + i below the 6 off dims of lo's knots that hi does not share, 6 (hi - off) + i from there on: the
+// same dims as relative_union_knot's, without its division by 6 (which costs pose_cov_kernel a spill).
+template <int M>
+__device__ __forceinline__ void gather_union_block(double* S, int ld, const double* cov, int np, int32_t sa, int32_t sb,
+                                                   int lane) {
+  const int off = relative_union_offset(sa, sb), m = M ? M : 6 * (4 + off);
+  const int d0 = 6 * (sa < sb ? sa : sb), d1 = 6 * ((sa < sb ? sb : sa) - off);
+  for (int e = lane; e < m * m; e += 32) {  // row by row
+    const int i = e / m, j = e - i * m;
+    const int gi = (i < 6 * off ? d0 : d1) + i, gj = (j < 6 * off ? d0 : d1) + j;
+    S[i * ld + j] = cov[size_t(gi) * np + gj];
+  }
+}
+
+// T = A S: T [rows][cols] and A [rows][kn] dense, S [kn][cols] with row stride lds; fma(A[i][k], S[k][b], acc)
+template <int UNROLL>
+__device__ __forceinline__ void warp_mul(double* T, const double* A, const double* S, int lds, int rows, int cols, int kn,
+                                         int lane) {
+  for (int e = lane; e < rows * cols; e += 32) {
+    const int i = e / cols, b = e - i * cols;
+    double acc = 0.0;
+#pragma unroll UNROLL
+    for (int k = 0; k < kn; ++k) acc = fma(A[i * kn + k], S[k * lds + b], acc);
+    T[e] = acc;
+  }
+}
+
+// out = T B': out [rows][cols], T [rows][kn] and B [cols][kn] dense; fma(T[i][k], B[j][k], acc).  SYM (T B' symmetric,
+// rows == cols): the lower triangle is formed and mirrored, so that out is exactly symmetric.
+template <int UNROLL, bool SYM>
+__device__ __forceinline__ void warp_mul_t(double* out, const double* T, const double* B, int rows, int cols, int kn,
+                                           int lane) {
+  for (int e = lane; e < (SYM ? rows * (rows + 1) / 2 : rows * cols); e += 32) {
+    int i = 0, j;
+    if (SYM) {
+      while ((i + 1) * (i + 2) / 2 <= e) ++i;
+      j = e - i * (i + 1) / 2;
+    } else {
+      i = e / cols;
+      j = e - i * cols;
+    }
+    double acc = 0.0;
+#pragma unroll UNROLL
+    for (int k = 0; k < kn; ++k) acc = fma(T[i * kn + k], B[j * kn + k], acc);
+    out[i * cols + j] = acc;
+    if (SYM) out[j * cols + i] = acc;
+  }
 }
 
 }  // namespace
@@ -284,8 +323,7 @@ int launch_cov_publish(const double* piv, int nb, const LmScalars* scal, LmPubli
 
 // One warp per query time: C = (J Sigma_sub) J' with J = J(t) (12 x 24, PoseJacobian) and Sigma_sub the 24 x 24 block of
 // the window covariance at the dims of knots s..s+3, which are contiguous (6s .. 6s + 23).  Every lane evaluates the
-// spline (the same values in all lanes) and lanes 0..23 write one column of J each; the products are fixed-order fma
-// chains, one output entry per lane, no atomics.  The lower triangle is formed and mirrored: exactly symmetric.
+// spline (the same values in all lanes) and lanes 0..23 write one column of J each.
 constexpr int kPoseCovWarps = 4;
 __global__ void __launch_bounds__(32 * kPoseCovWarps) pose_cov_kernel(PoseCovLaunch a) {
   __shared__ double sJ[kPoseCovWarps][12 * 24], sS[kPoseCovWarps][24 * 24], sT[kPoseCovWarps][12 * 24];
@@ -298,8 +336,7 @@ __global__ void __launch_bounds__(32 * kPoseCovWarps) pose_cov_kernel(PoseCovLau
   int32_t s;
   double u;
   spline_index(a.sp, a.t[n], s, u);
-  const double* src = a.cov + size_t(6 * s) * a.np + 6 * s;
-  for (int e = lane; e < 24 * 24; e += 32) S[e] = src[size_t(e / 24) * a.np + e % 24];
+  gather_union_block<24>(S, 24, a.cov, a.np, s, s, lane);
   PoseJacobian pj;
   pose_jacobian<kPStride>(a.sp, a.st.q, a.st.p, a.st.tab, s, u, pj);
   if (lane < 24) {
@@ -309,25 +346,9 @@ __global__ void __launch_bounds__(32 * kPoseCovWarps) pose_cov_kernel(PoseCovLau
     for (int i = 0; i < 12; ++i) J[i * 24 + lane] = col[i];
   }
   __syncwarp();
-  for (int e = lane; e < 12 * 24; e += 32) {  // T = J Sigma_sub
-    const int i = e / 24, b = e % 24;
-    double acc = 0.0;
-#pragma unroll 8
-    for (int k = 0; k < 24; ++k) acc = fma(J[i * 24 + k], S[k * 24 + b], acc);
-    T[e] = acc;
-  }
+  warp_mul<8>(T, J, S, 24, 12, 24, 24, lane);  // T = J Sigma_sub
   __syncwarp();
-  double* out = a.out + size_t(n) * 144;
-  for (int e = lane; e < 78; e += 32) {  // C[i][j] = T[i] . J[j], i >= j
-    int i = 0;
-    while ((i + 1) * (i + 2) / 2 <= e) ++i;
-    const int j = e - i * (i + 1) / 2;
-    double acc = 0.0;
-#pragma unroll 8
-    for (int k = 0; k < 24; ++k) acc = fma(T[i * 24 + k], J[j * 24 + k], acc);
-    out[i * 12 + j] = acc;
-    out[j * 12 + i] = acc;
-  }
+  warp_mul_t<8, true>(a.out + size_t(n) * 144, T, J, 12, 12, 24, lane);
 }
 
 int launch_pose_cov(const PoseCovLaunch& a, cudaStream_t s) {
@@ -340,7 +361,7 @@ int launch_pose_cov(const PoseCovLaunch& a, cudaStream_t s) {
 // Sigma_25 the joint covariance of the segment's 24 knot dims (6s .. 6s + 23) and rho_l:
 //   [[Sigma_sub, c], [c', var_l]],  c = -(Sigma_{6s.., row} W_l') / h_l over the coupling row landmark_variance_kernel walks.
 // A landmark without factors has rho constant: c = 0 and var_l = 0.  An inverse depth that is not > 0 and finite leaves
-// the point undefined: NaN.  Fixed-order fma chains and shuffle trees, no atomics; the lower triangle is mirrored.
+// the point undefined: NaN.  The coupling column is reduced by fixed shuffle trees.
 constexpr int kPointCovWarps = 4;
 __global__ void __launch_bounds__(32 * kPointCovWarps) point_cov_kernel(PointCovLaunch a) {
   __shared__ double sG[kPointCovWarps][3 * 25], sS[kPointCovWarps][25 * 25], sT[kPointCovWarps][3 * 25];
@@ -375,8 +396,7 @@ __global__ void __launch_bounds__(32 * kPointCovWarps) point_cov_kernel(PointCov
   int32_t s;
   double u;
   spline_index(a.sp, t, s, u);
-  const double* src = a.cov + size_t(6 * s) * a.np + 6 * s;
-  for (int e = lane; e < 24 * 24; e += 32) S[(e / 24) * 25 + e % 24] = src[size_t(e / 24) * a.np + e % 24];
+  gather_union_block<24>(S, 25, a.cov, a.np, s, s, lane);
   const double hl = a.ne.hl[l];
   if (a.active[a.np + l] && hl > 0.0) {  // (h_l <= 0 with factors fails the covariance before this kernel runs)
     const int lo = a.lm.lo[l], nw = a.lm.hi[l] - lo;
@@ -400,22 +420,9 @@ __global__ void __launch_bounds__(32 * kPointCovWarps) point_cov_kernel(PointCov
     for (int i = 0; i < 3; ++i) G[i * 25 + lane] = col[i];
   }
   __syncwarp();
-  for (int e = lane; e < 3 * 25; e += 32) {  // T = G Sigma_25
-    const int i = e / 25, b = e % 25;
-    double acc = 0.0;
-#pragma unroll 5
-    for (int k = 0; k < 25; ++k) acc = fma(G[i * 25 + k], S[k * 25 + b], acc);
-    T[e] = acc;
-  }
+  warp_mul<5>(T, G, S, 25, 3, 25, 25, lane);  // T = G Sigma_25
   __syncwarp();
-  if (lane < 6) {  // C[i][j] = T[i] . G[j], i >= j
-    const int i = lane < 1 ? 0 : lane < 3 ? 1 : 2, j = lane - i * (i + 1) / 2;
-    double acc = 0.0;
-#pragma unroll 5
-    for (int k = 0; k < 25; ++k) acc = fma(T[i * 25 + k], G[j * 25 + k], acc);
-    out[i * 3 + j] = acc;
-    out[j * 3 + i] = acc;
-  }
+  warp_mul_t<5, true>(out, T, G, 3, 3, 25, lane);
 }
 
 int launch_point_cov(const PointCovLaunch& a, cudaStream_t s) {
@@ -429,8 +436,7 @@ int launch_point_cov(const PointCovLaunch& a, cudaStream_t s) {
 // relative-pose Jacobian (relative_pose_jacobian_column over the two poses' dtheta / dp rows J_a, J_b, 6 x 24 each).
 // Shared knots get one column, so their terms cancel inside G rather than between two stacked 24-dim blocks.  The cross
 // block X = (J_a Sigma_ab) J_b' reads the same Sigma_U at the two segments' slots.  Every lane evaluates both splines (the
-// same values in all lanes); the products are fixed-order fma chains, one output entry per lane, no atomics; the lower
-// triangle of C is formed and mirrored: exactly symmetric.  26.5 KB of static shared memory per CTA.
+// same values in all lanes).  26.5 KB of static shared memory per CTA.
 constexpr int kRelUnion = 48;
 __global__ void __launch_bounds__(32) relative_pose_cov_kernel(RelativePoseCovLaunch a) {
   __shared__ double S[kRelUnion * kRelUnion], Ja[6 * 24], Jb[6 * 24], G[6 * kRelUnion], T[6 * kRelUnion], X[6 * 24];
@@ -442,11 +448,7 @@ __global__ void __launch_bounds__(32) relative_pose_cov_kernel(RelativePoseCovLa
   spline_index(a.sp, a.t_b[n], sb, ub);
   const int off = relative_union_offset(sa, sb), m = 6 * (4 + off);
   const int fa = relative_union_first(sa, sb), fb = relative_union_first(sb, sa);
-  for (int e = lane; e < m * m; e += 32) {  // Sigma_U, row by row
-    const int i = e / m, j = e - i * m;
-    const int gi = 6 * relative_union_knot(sa, sb, i / 6) + i % 6, gj = 6 * relative_union_knot(sa, sb, j / 6) + j % 6;
-    S[e] = a.cov[size_t(gi) * a.np + gj];
-  }
+  gather_union_block<0>(S, m, a.cov, a.np, sa, sb, lane);
   M3 R[2];
   V3 pos[2];
 #pragma unroll 1
@@ -471,45 +473,11 @@ __global__ void __launch_bounds__(32) relative_pose_cov_kernel(RelativePoseCovLa
     for (int i = 0; i < 6; ++i) G[i * m + c] = g[i];
   }
   __syncwarp();
-  for (int e = lane; e < 6 * m; e += 32) {  // T = G Sigma_U
-    const int i = e / m, b = e - i * m;
-    double acc = 0.0;
-#pragma unroll 6
-    for (int k = 0; k < m; ++k) acc = fma(G[i * m + k], S[k * m + b], acc);
-    T[e] = acc;
-  }
-  if (a.cross) {
-    for (int e = lane; e < 6 * 24; e += 32) {  // X = J_a Sigma_ab: rows at a's slots, columns at b's
-      const int i = e / 24, b = e % 24;
-      const double* Sab = S + size_t(6 * fa) * m + 6 * fb;
-      double acc = 0.0;
-#pragma unroll 8
-      for (int k = 0; k < 24; ++k) acc = fma(Ja[i * 24 + k], Sab[k * m + b], acc);
-      X[e] = acc;
-    }
-  }
+  warp_mul<6>(T, G, S, m, 6, m, m, lane);  // T = G Sigma_U
+  if (a.cross) warp_mul<8>(X, Ja, S + 6 * fa * m + 6 * fb, m, 6, 24, 24, lane);  // X = J_a Sigma_ab: a's rows, b's columns
   __syncwarp();
-  double* out = a.out + size_t(n) * 36;
-  if (lane < 21) {  // C[i][j] = T[i] . G[j], i >= j
-    int i = 0;
-    while ((i + 1) * (i + 2) / 2 <= lane) ++i;
-    const int j = lane - i * (i + 1) / 2;
-    double acc = 0.0;
-#pragma unroll 6
-    for (int k = 0; k < m; ++k) acc = fma(T[i * m + k], G[j * m + k], acc);
-    out[i * 6 + j] = acc;
-    out[j * 6 + i] = acc;
-  }
-  if (a.cross) {
-    double* cx = a.cross + size_t(n) * 36;
-    for (int e = lane; e < 36; e += 32) {  // cross[i][j] = X[i] . J_b[j]
-      const int i = e / 6, j = e % 6;
-      double acc = 0.0;
-#pragma unroll 8
-      for (int k = 0; k < 24; ++k) acc = fma(X[i * 24 + k], Jb[j * 24 + k], acc);
-      cx[e] = acc;
-    }
-  }
+  warp_mul_t<6, true>(a.out + size_t(n) * 36, T, G, 6, 6, m, lane);
+  if (a.cross) warp_mul_t<8, false>(a.cross + size_t(n) * 36, X, Jb, 6, 6, 24, lane);
 }
 
 int launch_relative_pose_cov(const RelativePoseCovLaunch& a, cudaStream_t s) {
@@ -583,29 +551,20 @@ int enqueue_covariance(ctvio_engine* e, int gauge_knot, LmPublished* pub, unsign
   return CTVIO_OK;
 }
 
-// form_covariance's rank test on the published block, for a caller that has already synchronised: the error of the
-// evaluation, or CTVIO_ERR_STATE "<who>: rank deficient" (message in *why), else CTVIO_OK
-int rank_test(const LmPublished& pub, const char* who, std::string* why) {
-  if (pub.s.error_flags & 1) {
-    *why = "a factor time left its knot window / the spline (line delay too large?)";
-    return CTVIO_ERR_TIME_RANGE;
-  }
-  const double rc_value = pub.rcond;
-  const bool failed = pub.s.chol_fail != 0;
-  // Ceres' default min_reciprocal_condition_number; the estimate is the pivot ratio, see include/ctvio.h
-  if (failed || !(rc_value >= 1e-14)) {
-    char msg[128];
-    std::snprintf(msg, sizeof(msg), "%s: rank deficient (rcond %.3e%s)", who, rc_value, failed ? ", non-positive pivot" : "");
-    *why = msg;
-    return CTVIO_ERR_STATE;
-  }
+// the checks of a covariance call that follow its own argument checks: the gauge knot (-1: none of its own), then
+// sharded mode
+int check_covariance_call(ctvio_engine* e, int32_t gauge_knot_index, const char* who) {
+  if (gauge_knot_index < -1 || gauge_knot_index >= e->nK)
+    return fail(CTVIO_ERR_INVALID, std::string(who) + ": gauge_knot_index outside -1 .. n_knots - 1");
+  if (e->world > 1) return fail(CTVIO_ERR_STATE, std::string(who) + ": not available in sharded mode");
   return CTVIO_OK;
 }
 
-// Sigma as enqueue_covariance forms it, then the rank test.  Returns CTVIO_OK, an error of the evaluation, or
-// CTVIO_ERR_STATE "<who>: rank deficient"; *rcond (may be null) is written in these last two cases only.  Ends with the
-// stream synchronised.
+// Sigma as enqueue_covariance forms it on the engine's device, then the rank test.  Returns CTVIO_OK, an error of the
+// evaluation, or CTVIO_ERR_STATE "<who>: rank deficient"; *rcond (may be null) is written in these last two cases only.
+// Ends with the stream synchronised.
 int form_covariance(ctvio_engine* e, int gauge_knot, const char* who, double* rcond) {
+  cudaSetDevice(e->cfg.device);
   int rc = enqueue_covariance(e, gauge_knot, e->h_pub, ++e->pub_seq);
   if (rc) return rc;
   rc = read_scalars(e, true);
@@ -621,8 +580,30 @@ int form_covariance(ctvio_engine* e, int gauge_knot, const char* who, double* rc
   return CTVIO_OK;
 }
 
-// point_cov_kernel over the a.n points whose inputs a names into out (device memory), right after Sigma on the same
-// stream
+// The projection kernels over the a.n items whose inputs a names into out (device memory), right after Sigma on the
+// same stream: each builder fills in the state, the spline, the rig and Sigma.
+void launch_pose_covariance(ctvio_engine* e, PoseCovLaunch& a, double* out) {
+  a.st = e->x[e->cur].ptrs();
+  a.sp = e->sp;
+  a.R_CI = e->rig.R_CI;
+  a.p_CI = e->rig.p_CI;
+  a.np = e->dims().np;
+  a.cov = e->cws.cov.p;
+  a.out = out;
+  e->launches += launch_pose_cov(a, e->stream);
+}
+
+void launch_relative_pose_covariance(ctvio_engine* e, RelativePoseCovLaunch& a, double* out) {
+  a.st = e->x[e->cur].ptrs();
+  a.sp = e->sp;
+  a.R_CI = e->rig.R_CI;
+  a.p_CI = e->rig.p_CI;
+  a.np = e->dims().np;
+  a.cov = e->cws.cov.p;
+  a.out = out;
+  e->launches += launch_relative_pose_cov(a, e->stream);
+}
+
 void launch_point_covariance(ctvio_engine* e, PointCovLaunch& a, double* out) {
   const ProblemDims d = e->dims();
   a.st = e->x[e->cur].ptrs();
@@ -649,36 +630,24 @@ void table_anchors(ctvio_engine* e, PointCovLaunch& a) {
 // point_cov_kernel over the a.n points whose inputs a names, right after form_covariance on the same stream; the n x 9
 // result to cov9.  Ends with the stream synchronised.
 int point_covariance(ctvio_engine* e, PointCovLaunch& a, double* cov9) {
-  cudaStream_t st = e->stream;
   auto& w = e->cws;
   CUDA_OK(w.pose.reserve(9 * size_t(a.n)));
   launch_point_covariance(e, a, w.pose.p);
-  CUDA_OK(cudaMemcpyAsync(cov9, w.pose.p, 9 * size_t(a.n) * sizeof(double), cudaMemcpyDeviceToHost, st));
-  e->d2h_bytes += 9 * size_t(a.n) * sizeof(double);
-  CUDA_OK(stream_sync(st));
-  return CTVIO_OK;
+  return read_result(e, cov9, w.pose.p, 9 * size_t(a.n));
 }
 
 }  // namespace
 
 extern "C" int ctvio_covariance(ctvio_handle e, double* cov_cc, double* var_rho, double* rcond) {
   if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
-  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_covariance: not available in sharded mode");
-  cudaSetDevice(e->cfg.device);
+  if (int rc = check_covariance_call(e, -1, "ctvio_covariance")) return rc;
   int rc = form_covariance(e, -1, "ctvio_covariance", rcond);
   if (rc) return rc;
-  cudaStream_t st = e->stream;
   const size_t np = size_t(e->dims().np), nL = size_t(e->nL);
   auto& w = e->cws;
-  if (cov_cc) {
-    CUDA_OK(cudaMemcpyAsync(cov_cc, w.cov.p, np * np * sizeof(double), cudaMemcpyDeviceToHost, st));
-    e->d2h_bytes += np * np * sizeof(double);
-  }
-  if (var_rho && nL) {
-    CUDA_OK(cudaMemcpyAsync(var_rho, w.var.p, nL * sizeof(double), cudaMemcpyDeviceToHost, st));
-    e->d2h_bytes += nL * sizeof(double);
-  }
-  CUDA_OK(stream_sync(st));
+  if (cov_cc && (rc = copy_to_host(e, cov_cc, w.cov.p, np * np))) return rc;
+  if (var_rho && nL && (rc = copy_to_host(e, var_rho, w.var.p, nL))) return rc;
+  CUDA_OK(stream_sync(e->stream));
   return CTVIO_OK;
 }
 
@@ -687,39 +656,22 @@ extern "C" int ctvio_pose_covariance(ctvio_handle e, int32_t n, const int64_t* t
   if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
   if (n < 0 || (n > 0 && (!t_ns || !cov12))) return fail(CTVIO_ERR_INVALID, "ctvio_pose_covariance: bad argument");
   if (camera_frame != 0 && camera_frame != 1) return fail(CTVIO_ERR_INVALID, "ctvio_pose_covariance: camera_frame must be 0 or 1");
-  if (gauge_knot_index < -1 || gauge_knot_index >= e->nK)
-    return fail(CTVIO_ERR_INVALID, "ctvio_pose_covariance: gauge_knot_index outside -1 .. n_knots - 1");
-  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_pose_covariance: not available in sharded mode");
+  if (int rc = check_covariance_call(e, gauge_knot_index, "ctvio_pose_covariance")) return rc;
   if (n == 0) return CTVIO_OK;
   if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
-  for (int32_t i = 0; i < n; ++i) {  // the range ctvio_query_trajectory accepts
-    int32_t s;
-    double u;
-    if (!spline_index(e->sp, t_ns[i], s, u)) return fail(CTVIO_ERR_TIME_RANGE, "ctvio_pose_covariance: a time outside the spline");
-  }
-  cudaSetDevice(e->cfg.device);
+  if (!times_inside(e->sp, n, t_ns)) return fail(CTVIO_ERR_TIME_RANGE, "ctvio_pose_covariance: a time outside the spline");
   int rc = form_covariance(e, gauge_knot_index, "ctvio_pose_covariance", rcond);
   if (rc) return rc;
-  cudaStream_t st = e->stream;
   auto& w = e->cws;
   CUDA_OK(w.t.reserve(size_t(n)));
   CUDA_OK(w.pose.reserve(144 * size_t(n)));
-  CUDA_OK(cudaMemcpyAsync(w.t.p, t_ns, size_t(n) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(w.t.p, t_ns, size_t(n) * sizeof(int64_t), cudaMemcpyHostToDevice, e->stream));
   e->h2d_bytes += size_t(n) * sizeof(int64_t);
-  PoseCovLaunch a;
-  a.st = e->x[e->cur].ptrs();
-  a.sp = e->sp;
-  a.R_CI = e->rig.R_CI;
-  a.p_CI = e->rig.p_CI;
-  a.n = n; a.np = e->dims().np; a.camera_frame = camera_frame;
+  PoseCovLaunch a = {};
+  a.n = n; a.camera_frame = camera_frame;
   a.t = w.t.p;
-  a.cov = w.cov.p;
-  a.out = w.pose.p;
-  e->launches += launch_pose_cov(a, st);
-  CUDA_OK(cudaMemcpyAsync(cov12, w.pose.p, 144 * size_t(n) * sizeof(double), cudaMemcpyDeviceToHost, st));
-  e->d2h_bytes += 144 * size_t(n) * sizeof(double);
-  CUDA_OK(stream_sync(st));
-  return CTVIO_OK;
+  launch_pose_covariance(e, a, w.pose.p);
+  return read_result(e, cov12, w.pose.p, 144 * size_t(n));
 }
 
 extern "C" int ctvio_relative_pose_covariance(ctvio_handle e, int32_t n, const int64_t* t_a_ns, const int64_t* t_b_ns,
@@ -730,43 +682,29 @@ extern "C" int ctvio_relative_pose_covariance(ctvio_handle e, int32_t n, const i
     return fail(CTVIO_ERR_INVALID, "ctvio_relative_pose_covariance: bad argument");
   if (camera_frame != 0 && camera_frame != 1)
     return fail(CTVIO_ERR_INVALID, "ctvio_relative_pose_covariance: camera_frame must be 0 or 1");
-  if (gauge_knot_index < -1 || gauge_knot_index >= e->nK)
-    return fail(CTVIO_ERR_INVALID, "ctvio_relative_pose_covariance: gauge_knot_index outside -1 .. n_knots - 1");
-  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_relative_pose_covariance: not available in sharded mode");
+  if (int rc = check_covariance_call(e, gauge_knot_index, "ctvio_relative_pose_covariance")) return rc;
   if (n == 0) return CTVIO_OK;
   if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
-  for (int32_t i = 0; i < n; ++i) {  // the range ctvio_query_trajectory accepts
-    int32_t s;
-    double u;
-    if (!spline_index(e->sp, t_a_ns[i], s, u) || !spline_index(e->sp, t_b_ns[i], s, u))
-      return fail(CTVIO_ERR_TIME_RANGE, "ctvio_relative_pose_covariance: a time outside the spline");
-  }
-  cudaSetDevice(e->cfg.device);
+  if (!times_inside(e->sp, n, t_a_ns) || !times_inside(e->sp, n, t_b_ns))
+    return fail(CTVIO_ERR_TIME_RANGE, "ctvio_relative_pose_covariance: a time outside the spline");
   int rc = form_covariance(e, gauge_knot_index, "ctvio_relative_pose_covariance", rcond);
   if (rc) return rc;
   cudaStream_t st = e->stream;
   auto& w = e->cws;
-  const size_t nn = size_t(n), n_out = cross6 ? 72 : 36;
+  const size_t nn = size_t(n);
   CUDA_OK(w.t.reserve(2 * nn));
-  CUDA_OK(w.pose.reserve(n_out * nn));  // cov6, then cross6
+  CUDA_OK(w.pose.reserve((cross6 ? 72 : 36) * nn));  // cov6, then cross6
   CUDA_OK(cudaMemcpyAsync(w.t.p, t_a_ns, nn * sizeof(int64_t), cudaMemcpyHostToDevice, st));
   CUDA_OK(cudaMemcpyAsync(w.t.p + nn, t_b_ns, nn * sizeof(int64_t), cudaMemcpyHostToDevice, st));
   e->h2d_bytes += 2 * nn * sizeof(int64_t);
-  RelativePoseCovLaunch a;
-  a.st = e->x[e->cur].ptrs();
-  a.sp = e->sp;
-  a.R_CI = e->rig.R_CI;
-  a.p_CI = e->rig.p_CI;
-  a.n = n; a.np = e->dims().np; a.camera_frame = camera_frame;
+  RelativePoseCovLaunch a = {};
+  a.n = n; a.camera_frame = camera_frame;
   a.t_a = w.t.p;
   a.t_b = w.t.p + nn;
-  a.cov = w.cov.p;
-  a.out = w.pose.p;
   a.cross = cross6 ? w.pose.p + 36 * nn : nullptr;
-  e->launches += launch_relative_pose_cov(a, st);
-  CUDA_OK(cudaMemcpyAsync(cov6, a.out, 36 * nn * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (cross6) CUDA_OK(cudaMemcpyAsync(cross6, a.cross, 36 * nn * sizeof(double), cudaMemcpyDeviceToHost, st));
-  e->d2h_bytes += n_out * nn * sizeof(double);
+  launch_relative_pose_covariance(e, a, w.pose.p);
+  if ((rc = copy_to_host(e, cov6, a.out, 36 * nn))) return rc;
+  if (cross6 && (rc = copy_to_host(e, cross6, a.cross, 36 * nn))) return rc;
   CUDA_OK(stream_sync(st));
   return CTVIO_OK;
 }
@@ -778,18 +716,11 @@ extern "C" int ctvio_point_covariance(ctvio_handle e, int32_t n, const int32_t* 
     return fail(CTVIO_ERR_INVALID, "ctvio_point_covariance: bad argument");
   for (int32_t i = 0; i < n; ++i)
     if (landmark[i] < 0 || landmark[i] >= e->nL) return fail(CTVIO_ERR_INVALID, "ctvio_point_covariance: landmark out of range");
-  if (gauge_knot_index < -1 || gauge_knot_index >= e->nK)
-    return fail(CTVIO_ERR_INVALID, "ctvio_point_covariance: gauge_knot_index outside -1 .. n_knots - 1");
-  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_point_covariance: not available in sharded mode");
+  if (int rc = check_covariance_call(e, gauge_knot_index, "ctvio_point_covariance")) return rc;
   if (n == 0) return CTVIO_OK;
   if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
-  for (int32_t i = 0; i < n; ++i) {  // the range ctvio_query_trajectory accepts
-    int32_t s;
-    double u;
-    if (!spline_index(e->sp, t_anchor_ns[i], s, u))
-      return fail(CTVIO_ERR_TIME_RANGE, "ctvio_point_covariance: an anchor time outside the spline");
-  }
-  cudaSetDevice(e->cfg.device);
+  if (!times_inside(e->sp, n, t_anchor_ns))
+    return fail(CTVIO_ERR_TIME_RANGE, "ctvio_point_covariance: an anchor time outside the spline");
   int rc = form_covariance(e, gauge_knot_index, "ctvio_point_covariance", rcond);
   if (rc) return rc;
   cudaStream_t st = e->stream;
@@ -812,9 +743,7 @@ extern "C" int ctvio_point_covariance(ctvio_handle e, int32_t n, const int32_t* 
 extern "C" int ctvio_feature_table_point_covariance(ctvio_handle e, int32_t n_landmarks, int32_t gauge_knot_index,
                                                     double* cov9, double* rcond) {
   if (!e) return fail(CTVIO_ERR_INVALID, "null handle");
-  if (gauge_knot_index < -1 || gauge_knot_index >= e->nK)
-    return fail(CTVIO_ERR_INVALID, "ctvio_feature_table_point_covariance: gauge_knot_index outside -1 .. n_knots - 1");
-  if (e->world > 1) return fail(CTVIO_ERR_STATE, "ctvio_feature_table_point_covariance: not available in sharded mode");
+  if (int rc = check_covariance_call(e, gauge_knot_index, "ctvio_feature_table_point_covariance")) return rc;
   auto& ft = e->ft;
   if (!ft.window_current) return fail(CTVIO_ERR_STATE, "no feature-table window since the last add / slide");
   if (e->nL != ft.n_lm) return fail(CTVIO_ERR_STATE, "the resident inverse depths no longer follow the table's numbering");
@@ -823,13 +752,8 @@ extern "C" int ctvio_feature_table_point_covariance(ctvio_handle e, int32_t n_la
   if (n_landmarks > 0 && !cov9) return fail(CTVIO_ERR_INVALID, "ctvio_feature_table_point_covariance: null argument");
   if (n_landmarks == 0) return CTVIO_OK;
   if (!e->have_knots) return fail(CTVIO_ERR_STATE, "knots have not been set");
-  for (int slot = 0; slot < ctvio_engine::kFrameSlots; ++slot) {  // every anchor is a held slot
-    int32_t s;
-    double u;
-    if ((ft.held >> slot & 1u) && !spline_index(e->sp, e->h_frame_t[slot], s, u))
-      return fail(CTVIO_ERR_TIME_RANGE, "ctvio_feature_table_point_covariance: a held frame time falls outside the spline");
-  }
-  cudaSetDevice(e->cfg.device);
+  if (!held_frames_inside(e))  // every anchor is a held slot
+    return fail(CTVIO_ERR_TIME_RANGE, "ctvio_feature_table_point_covariance: a held frame time falls outside the spline");
   int rc = form_covariance(e, gauge_knot_index, "ctvio_feature_table_point_covariance", rcond);
   if (rc) return rc;
   // the anchors come from the window's observation CSR and the frame table: nothing goes up
@@ -841,10 +765,39 @@ extern "C" int ctvio_feature_table_point_covariance(ctvio_handle e, int32_t n_la
 
 namespace ctvio::host {
 
+int rank_test(const LmPublished& pub, const char* who, std::string* why) {
+  if (pub.s.error_flags & 1) {
+    *why = "a factor time left its knot window / the spline (line delay too large?)";
+    return CTVIO_ERR_TIME_RANGE;
+  }
+  const double rc_value = pub.rcond;
+  const bool failed = pub.s.chol_fail != 0;
+  // Ceres' default min_reciprocal_condition_number; the estimate is the pivot ratio, see include/ctvio.h
+  if (failed || !(rc_value >= 1e-14)) {
+    char msg[128];
+    std::snprintf(msg, sizeof(msg), "%s: rank deficient (rcond %.3e%s)", who, rc_value, failed ? ", non-positive pivot" : "");
+    *why = msg;
+    return CTVIO_ERR_STATE;
+  }
+  return CTVIO_OK;
+}
+
+bool times_inside(const SplineParams& sp, int n, const int64_t* t) {
+  int32_t s;
+  double u;
+  for (int i = 0; i < n; ++i)
+    if (!spline_index(sp, t[i], s, u)) return false;
+  return true;
+}
+
+bool held_frames_inside(ctvio_engine* e) {
+  for (int slot = 0; slot < ctvio_engine::kFrameSlots; ++slot)
+    if ((e->ft.held >> slot & 1u) && !times_inside(e->sp, 1, &e->h_frame_t[slot])) return false;
+  return true;
+}
+
 // the cycle's device workspace cov_out: cov12 (144) | cov6 [15][36] | cov9 [n_landmarks][9]
 constexpr size_t kCycleCov6 = 144, kCycleCov9 = kCycleCov6 + 36 * (kKeyframeMaxSlots - 1);
-
-int covariance_rank_test(const LmPublished& pub, const char* who, std::string* why) { return rank_test(pub, who, why); }
 
 int cycle_covariance_enqueue(ctvio_engine* e, int gauge_knot, bool pose, bool rel, bool points) {
   auto& c = e->cyc;
@@ -861,46 +814,30 @@ int cycle_covariance_enqueue(ctvio_engine* e, int gauge_knot, bool pose, bool re
   CUDA_OK(c.cov_t.reserve(1 + kKeyframeMaxSlots));
   CUDA_OK(c.cov_out.reserve(kCycleCov9 + 9 * size_t(kFeatureTableMaxEntries)));
   CycleCovHost* h = c.cov_host;
-  cudaStream_t st = e->stream;
   const int nf = cv.n_frames, n_pairs = rel ? nf - 1 : 0;
   // the times go up from the mapped block (the last cycle's copy out of it completed before that cycle ended)
   const int n_t = (pose || n_pairs > 0) ? 1 + (n_pairs > 0 ? nf : 0) : 0;
   h->t[0] = cv.pose_t;
   for (int k = 0; k < nf; ++k) h->t[1 + k] = cv.frame_t[k];
   if (n_t) {
-    CUDA_OK(cudaMemcpyAsync(c.cov_t.p, h->t, size_t(n_t) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(c.cov_t.p, h->t, size_t(n_t) * sizeof(int64_t), cudaMemcpyHostToDevice, e->stream));
     e->h2d_bytes += size_t(n_t) * sizeof(int64_t);
   }
   if (const int rc = enqueue_covariance(e, gauge_knot, &h->pub, ++cv.seq)) return rc;
   if (pose) {  // the camera pose and velocity at the TF time: ctvio_pose_covariance(camera_frame = 1)
     PoseCovLaunch a = {};
-    a.st = e->x[e->cur].ptrs();
-    a.sp = e->sp;
-    a.R_CI = e->rig.R_CI;
-    a.p_CI = e->rig.p_CI;
-    a.n = 1; a.np = e->dims().np; a.camera_frame = 1;
+    a.n = 1; a.camera_frame = 1;
     a.t = c.cov_t.p;
-    a.cov = e->cws.cov.p;
-    a.out = c.cov_out.p;
-    e->launches += launch_pose_cov(a, st);
-    CUDA_OK(cudaMemcpyAsync(h->cov12, a.out, 144 * sizeof(double), cudaMemcpyDeviceToHost, st));
-    e->d2h_bytes += 144 * sizeof(double);
+    launch_pose_covariance(e, a, c.cov_out.p);
+    if (const int rc = copy_to_host(e, h->cov12, a.out, 144)) return rc;
   }
   if (n_pairs > 0) {  // the odometry edges (t[i], t[i + 1]): ctvio_relative_pose_covariance(camera_frame = 1)
     RelativePoseCovLaunch a = {};
-    a.st = e->x[e->cur].ptrs();
-    a.sp = e->sp;
-    a.R_CI = e->rig.R_CI;
-    a.p_CI = e->rig.p_CI;
-    a.n = n_pairs; a.np = e->dims().np; a.camera_frame = 1;
+    a.n = n_pairs; a.camera_frame = 1;
     a.t_a = c.cov_t.p + 1;
     a.t_b = c.cov_t.p + 2;
-    a.cov = e->cws.cov.p;
-    a.out = c.cov_out.p + kCycleCov6;
-    a.cross = nullptr;
-    e->launches += launch_relative_pose_cov(a, st);
-    CUDA_OK(cudaMemcpyAsync(h->cov6, a.out, 36 * size_t(n_pairs) * sizeof(double), cudaMemcpyDeviceToHost, st));
-    e->d2h_bytes += 36 * size_t(n_pairs) * sizeof(double);
+    launch_relative_pose_covariance(e, a, c.cov_out.p + kCycleCov6);
+    if (const int rc = copy_to_host(e, h->cov6, a.out, 36 * size_t(n_pairs))) return rc;
   }
   if (points && cv.n_lm > 0) {  // the window landmarks' world points, anchored as the table holds them: stay on the
                                 // device until the map kernel gathers them

@@ -388,6 +388,22 @@ struct ArenaScope {
   ~ArenaScope() { g_arena = prev; }
 };
 
+// n elements from the device to the host on the engine stream, counted in d2h_bytes; no synchronisation
+template <class T>
+int copy_to_host(ctvio_engine* e, T* dst, const T* src, size_t n = 1) {
+  CUDA_OK(cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyDeviceToHost, e->stream));
+  e->d2h_bytes += n * sizeof(T);
+  return CTVIO_OK;
+}
+
+// n elements of a kernel's small result, back to the host at the end of the call
+template <class T>
+int read_result(ctvio_engine* e, T* dst, const T* src, size_t n = 1) {
+  if (const int rc = copy_to_host(e, dst, src, n)) return rc;
+  CUDA_OK(stream_sync(e->stream));
+  return CTVIO_OK;
+}
+
 inline int ensure_table(ctvio_engine* e) {
   if (!e->table_valid) {
     e->launches += launch_knot_table(e->x[e->cur].ptrs(), e->nK, e->stream);
@@ -435,11 +451,16 @@ int feature_table_map_body(ctvio_engine* e, int32_t n_frames, const int32_t* fra
                            double* point_cov9);
 // covariance.cu, for the odometry cycle: Sigma with the knots <= gauge_knot held constant and its projections enqueued
 // on the engine stream without a host wait, the rank test's inputs published to e->cyc.cov_host->pub (the cycle reads
-// them after its next synchronisation, cycle_covariance_rank_test).  pose / rel / points: the TF pose at
-// e->cyc.cov.pose_t, the consecutive frame pairs of e->cyc.cov.frame_t, the window's landmarks.
+// them after its next synchronisation, rank_test).  pose / rel / points: the TF pose at e->cyc.cov.pose_t, the
+// consecutive frame pairs of e->cyc.cov.frame_t, the window's landmarks.
 int cycle_covariance_enqueue(ctvio_engine* e, int gauge_knot, bool pose, bool rel, bool points);
 const double* cycle_point_covariances(ctvio_engine* e);  // [n_lm][9] in the solved window's numbering, on the device
-// CTVIO_OK, or the error the separate covariance calls return for the same inputs (message in *why)
-int covariance_rank_test(const LmPublished& pub, const char* who, std::string* why);
+// the rank test of a published block, after a synchronisation: CTVIO_OK, or the error the covariance calls return for
+// the same inputs (the evaluation's, or CTVIO_ERR_STATE "<who>: rank deficient"; message in *why)
+int rank_test(const LmPublished& pub, const char* who, std::string* why);
+// the ranges the covariance calls check (the range ctvio_query_trajectory accepts): the times t[0 .. n) lie inside the
+// spline; every frame time of a slot the feature table holds (the anchors of its landmarks) lies inside the spline
+bool times_inside(const SplineParams& sp, int n, const int64_t* t);
+bool held_frames_inside(ctvio_engine* e);
 
 }  // namespace ctvio::host

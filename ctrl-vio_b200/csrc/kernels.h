@@ -208,6 +208,22 @@ __device__ __forceinline__ void det_ticket_done(int* ticket, int my) {
 // programmatic dependent launch (see launch_chained): both are no-ops in a kernel that was launched without it
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+// reductions over the 32 lanes of a full warp, one fixed xor-shuffle tree: every lane gets the same, reproducible value
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ double warp_min_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+__device__ __forceinline__ double warp_max_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
 #endif
 
 // ---- programmatic dependent launch (PDL) on the pipelined LM driver's main stream ---------------

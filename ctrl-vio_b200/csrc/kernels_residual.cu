@@ -60,12 +60,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t phase) {
   return ok != 0;
 }
 
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // ------------------------------------------------------------------------------------------------
 // K0
 
@@ -437,7 +431,7 @@ __global__ void __launch_bounds__(kVisThreads, 1) visual_kernel(const __grid_con
   // ---- cost + flush ----
   const int n_rounds = (item.count + kVisObsPerRound - 1) / kVisObsPerRound;
   det_ticket_wait(a.det_ticket, blockIdx.x * 1024 + (FULL ? n_rounds : 0));
-  cost_local = warp_sum(cost_local);
+  cost_local = warp_sum_d(cost_local);
   if (lane == 0) sm.cost_part[warp] = cost_local;
   __syncthreads();
   if (tid == 0) {
@@ -695,7 +689,7 @@ __global__ void __launch_bounds__(kImuThreads) imu_kernel(const __grid_constant_
   }
   if (!FULL) det_ticket_wait(a.det_ticket, blockIdx.x);
   if (warp == 0) {  // every warp evaluated the same samples; warp 0's lanes hold them in sample order
-    cost = warp_sum(cost);
+    cost = warp_sum_d(cost);
     if (lane == 0 && cost != 0.0) atomicAdd(a.ne.cost, cost);
   }
   det_ticket_done(a.det_ticket, blockIdx.x);
@@ -805,7 +799,7 @@ __global__ void __launch_bounds__(256) small_factors_kernel(const __grid_constan
       }
     }
   }
-  cost = warp_sum(cost);
+  cost = warp_sum_d(cost);
   if ((tid & 31) == 0) red[tid >> 5] = cost;
   __syncthreads();
   if (tid == 0) {

@@ -155,14 +155,8 @@ int start_covariances(ctvio_engine* e, int64_t max_t, int n_lm) {
   for (int k = 0; k < c.n_frames; ++k) cv.frame_t[k] = c.t[k];
   cv.n_lm = n_lm;
   // the ranges the separate calls check: the query times, and every held slot's frame time (the anchors)
-  bool inside = true;
-  int32_t s;
-  double u;
-  if (pose) inside = spline_index(e->sp, cv.pose_t, s, u);
-  for (int k = 0; rel && k < c.n_frames; ++k) inside = inside && spline_index(e->sp, c.t[k], s, u);
-  for (int slot = 0; points && slot < ctvio_engine::kFrameSlots; ++slot)
-    if (e->ft.held >> slot & 1u) inside = inside && spline_index(e->sp, e->h_frame_t[slot], s, u);
-  if (!inside) {
+  if ((pose && !times_inside(e->sp, 1, &cv.pose_t)) || (rel && !times_inside(e->sp, c.n_frames, c.t)) ||
+      (points && !held_frames_inside(e))) {
     cv.status = CTVIO_ERR_TIME_RANGE;
     cv.why = "a covariance time falls outside the spline";
     return CTVIO_OK;
@@ -182,7 +176,7 @@ int finish_covariances(ctvio_engine* e) {
     return fail(CTVIO_ERR_CUDA, "the window covariance was not published before the cycle's synchronisation");
   std::atomic_thread_fence(std::memory_order_acquire);
   cv.rcond = pub.rcond;
-  cv.status = covariance_rank_test(pub, "window covariance", &cv.why);
+  cv.status = rank_test(pub, "window covariance", &cv.why);
   if (cv.status == CTVIO_OK) cv.available = cv.requested & 3;  // the map's bit comes with the map
   return CTVIO_OK;
 }

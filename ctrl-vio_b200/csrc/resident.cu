@@ -9,15 +9,6 @@ namespace {
 // the inverse depths just written into the other state buffer become the current ones
 void swap_rho(ctvio_engine* e) { swap(e->x[e->cur].rho, e->x[e->cur ^ 1].rho); }
 
-// n elements of a kernel's small result, back to the host at the end of the call
-template <class T>
-int read_result(ctvio_engine* e, T* dst, const T* src, size_t n = 1) {
-  CUDA_OK(cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyDeviceToHost, e->stream));
-  e->d2h_bytes += n * sizeof(T);
-  CUDA_OK(stream_sync(e->stream));
-  return CTVIO_OK;
-}
-
 // the caller's window of 1..kFrameSlots frame slots (n_frames checked by the caller), oldest to newest, each listed once
 int parse_window_slots(int32_t n_frames, const int32_t* frame_slots, ctvio::WindowSlots& w) {
   w.n_frames = n_frames;
