@@ -197,9 +197,6 @@ struct ctvio_engine {
   DevBuf<VisualItem> d_items;
   int n_items = 0;
   std::vector<int32_t> img_order;  // sorted position -> original index
-  std::vector<int32_t> img_li, img_lj;    // ... and the last knot of those windows
-  std::vector<int32_t> img_wi0, img_wj0;  // first knot of the padded anchor / observation window per factor (caller order)
-  std::vector<VisualItem> h_items;        // K1 work items (one per chunk of a frame-pair group)
   std::vector<int32_t> imu_order;
   DevBuf<longlong2> d_imu_t;
   DevBuf<double2> d_imu_ga;
@@ -223,8 +220,8 @@ struct ctvio_engine {
   int n_schur_items = 0, n_schur_entries = 0;
   int64_t w_len = 0;                        // length of the compact W array (woff[nL])
   DevBuf<uint8_t> d_cmask, d_active;
-  std::vector<uint8_t> h_cmask, h_active;
-  // device structure build (structure.cu): scratch, its count block and the knot bitmask of the image factors' windows
+  std::vector<uint8_t> h_cmask, h_active;  // h_active: camera part, then the host build's landmark part
+  // device structure build (structure.cu): scratch, its count block; either build's knot bitmask of the factors' windows
   DevBuf<uint64_t> sb_key;
   DevBuf<int32_t> sb_idx;
   DevBuf<uint32_t> sb_counts;
@@ -412,24 +409,31 @@ inline int ensure_table(ctvio_engine* e) {
   return CTVIO_OK;
 }
 
-// structure.cu: the structure build of a factor set with device-resident descriptors (T: tiles per side of the reduced
-// system).  structure_build_device reads back the one count block; schur_lists_device fills the K4 lists it sized.
 // resident.cu: the resident feature table's arrays, at full size, on first use
 int ensure_feature_table(ctvio_engine* e);
 // odometry.cu: ctvio_odometry_start's option checks (also applied to a checkpoint's options by ctvio_odometry_restore)
 int check_cycle_options(const ctvio_cycle_options* o);
 
+// structure.cu: the structure build of the image-factor set, on the device or on the host (T: tiles per side of the
+// reduced system).  structure_build_device reads back the one count block; schur_lists_device fills the K4 lists it sized.
 int structure_build_device(ctvio_engine* e, int T);
 int schur_lists_device(ctvio_engine* e, int T);
-// ctvio_marginalize's image part: marg_img, pos_lm relative to the first inverse-depth position (offset_pos_lm_device
-// adds it), the knot bitmask of the marginalized factors' windows and the counts, in one read-back
+int structure_build_host(ctvio_engine* e);
+int schur_lists_host(ctvio_engine* e, int T);
+// ctvio_marginalize's image part: knot bitmask, counts, marg_img and the landmarks' ranks (pos_lm, -1: none), the last
+// two in e->mws (device; offset_pos_lm_device adds the base) or in the host vectors
 int marg_discover_device(ctvio_engine* e, std::vector<uint32_t>& knots, int& n_marg, int& n_rho);
 int offset_pos_lm_device(ctvio_engine* e, int base);
+int marg_discover_host(ctvio_engine* e, std::vector<uint32_t>& knots, int& n_marg, int& n_rho,
+                       std::vector<int32_t>& marg_img, std::vector<int32_t>& pos_lm);
 // sharded mode: per-landmark owned flags (hi > 0 of the built structure) into either buffer (may be null)
 int owned_flags_device(ctvio_engine* e, double* as_double, uint8_t* as_byte);
 
 // engine.cu, used by the LM driver in solve.cu
-int prepare(ctvio_engine* e);  // structures of the factor set, built on the host (or by structure.cu) and uploaded
+int prepare(ctvio_engine* e);  // structures of the factor set, built by structure.cu and the stages of engine.cu
+// first knot of the spline segment of an evaluation time; its padded window [first, last] (false: outside the spline)
+int knot_window_first(const ctvio_engine* e, int64_t t);
+bool knot_window(const ctvio_engine* e, int64_t t, int& first, int& last);
 void evaluate(ctvio_engine* e, int xb, int nb, bool full, bool reset_cost = true);
 int read_scalars(ctvio_engine* e, bool published = false);
 LinearLaunch linear_launch(ctvio_engine* e, int nb);

@@ -1,8 +1,9 @@
-// The engine's structure build of an image-factor set whose descriptors live on the device (the factors of
-// ctvio_add_image_features_from_table, and slot-named factors added next to them): frame-pair groups, K1 work items,
-// landmark knot ranges, the compact W layout, the K4 per-tile landmark lists and the image part of the active mask,
-// bit for bit what prepare()'s host build makes of the same factors in the same caller order.  Also the image part of
-// ctvio_marginalize's block discovery, the sharded mode's owned flags and the structure probe.
+// The engine's two structure builds of an image-factor set, bit for bit the same arrays of the same factors in the same
+// caller order: frame-pair groups, K1 work items, landmark knot ranges, the compact W layout, the K4 per-tile landmark
+// lists, the landmark part of the active mask and the knot bitmask of the factors' padded windows.  The device build
+// takes a set whose descriptors live on the device (ctvio_add_image_features_from_table, and slot-named factors added
+// next to them), the host build a set of host records.  Each has its half of ctvio_marginalize's block discovery.
+// Also the sharded mode's owned flags and the structure probe.
 //
 // structure_kernel runs as ONE CTA: a table window has at most 15 x 1024 factors and 16 distinct frame times, and every
 // step is a scan, a stable radix sort or an order-independent atomic min / max / or, so the result does not depend on
@@ -446,6 +447,17 @@ __global__ void owned_flags_kernel(const int32_t* hi, int nL, double* as_double,
 
 namespace ctvio::host {
 
+// the SoA payload of the n sorted descriptors in d_img_desc, gathered from the resident frame tables
+int gather_factors(ctvio_engine* e, int n) {
+  CUDA_OK(e->d_img_t.reserve(n)); CUDA_OK(e->d_img_pi.reserve(n)); CUDA_OK(e->d_img_pj.reserve(n)); CUDA_OK(e->d_img_meta.reserve(n));
+  ctvio::GatherFactorsArgs ga;
+  ga.n = n; ga.desc = e->d_img_desc.p; ga.table = e->d_frames.p; ga.frame_t = e->d_frame_t.p;
+  ga.frame_cap = ctvio_engine::kFrameCap;
+  ga.t = e->d_img_t.p; ga.pi = e->d_img_pi.p; ga.pj = e->d_img_pj.p; ga.meta = e->d_img_meta.p;
+  e->launches += ctvio::launch_gather_factors(ga, e->stream);
+  return CTVIO_OK;
+}
+
 int structure_build_device(ctvio_engine* e, int T) {
   cudaStream_t st = e->stream;
   const int n = e->n_img_dev, nL = e->nL, nK = e->nK;
@@ -485,13 +497,8 @@ int structure_build_device(ctvio_engine* e, int T) {
   e->n_schur_entries = int(c[kEntries]);
   e->w_len = int64_t(uint64_t(c[kWLenLo]) | (uint64_t(c[kWLenHi]) << 32));
   e->img_knots.assign(c.begin() + kHdrWords, c.end());
-  ctvio::GatherFactorsArgs ga;
-  ga.n = n; ga.desc = e->d_img_desc.p; ga.table = e->d_frames.p; ga.frame_t = e->d_frame_t.p;
-  ga.frame_cap = ctvio_engine::kFrameCap;
-  CUDA_OK(e->d_img_t.reserve(n)); CUDA_OK(e->d_img_pi.reserve(n)); CUDA_OK(e->d_img_pj.reserve(n)); CUDA_OK(e->d_img_meta.reserve(n));
-  ga.t = e->d_img_t.p; ga.pi = e->d_img_pi.p; ga.pj = e->d_img_pj.p; ga.meta = e->d_img_meta.p;
-  e->launches += ctvio::launch_gather_factors(ga, st);
-  return CTVIO_OK;
+  e->h_active.assign(d.np, 0);  // the landmark part of the active mask is in d_active already
+  return gather_factors(e, n);
 }
 
 int schur_lists_device(ctvio_engine* e, int T) {
@@ -508,6 +515,204 @@ int schur_lists_device(ctvio_engine* e, int T) {
     schur_lists_kernel<<<n_tiles, kListThreads, 0, e->stream>>>(a);
     e->launches += 1;
   }
+  return CTVIO_OK;
+}
+
+int structure_build_host(ctvio_engine* e) {
+  cudaStream_t st = e->stream;
+  const ProblemDims d = e->dims();
+  // ---- image factors: padded knot windows, landmark knot ranges, the knot bitmask ----
+  const int n = int(e->img.size());
+  std::vector<int32_t> wi0(n), wj0(n);
+  e->h_lo.assign(e->nL, INT32_MAX);
+  e->h_hi.assign(e->nL, 0);
+  e->img_knots.assign((size_t(e->nK) + 31) / 32, 0u);
+  // the image factors of a window carry a dozen distinct frame times: the padded knot window of a time (two 64-bit
+  // divisions) is looked up in a small direct-mapped cache.  Every window handed out was computed by a fill, so the
+  // fills mark the bitmask.
+  struct WinCache { int64_t t = INT64_MIN; int f = 0, l = 0; bool ok = false; } wc[64];
+  auto window_of = [&](int64_t t, int& f, int& l) {
+    WinCache& c = wc[size_t(uint64_t(t) * 0x9E3779B97F4A7C15ull >> 58)];
+    if (c.t != t) {
+      c.t = t;
+      c.ok = knot_window(e, t, c.f, c.l);
+      for (int k = c.f; c.ok && k <= c.l; ++k) e->img_knots[size_t(k) / 32] |= 1u << (k % 32);
+    }
+    f = c.f; l = c.l;
+    return c.ok;
+  };
+  for (int k = 0; k < n; ++k) {
+    const HostImage& o = e->img[k];
+    int f0, l0, f1, l1;
+    if (!window_of(o.ti, f0, l0) || !window_of(o.tj, f1, l1))
+      return fail(CTVIO_ERR_TIME_RANGE, "image factor time (+ rolling-shutter padding) outside the spline");
+    if (o.lm < 0 || o.lm >= e->nL) return fail(CTVIO_ERR_INVALID, "landmark index out of range");
+    wi0[k] = f0; wj0[k] = f1;
+    e->h_lo[o.lm] = std::min(e->h_lo[o.lm], 6 * std::min(f0, f1));
+    e->h_hi[o.lm] = std::max(e->h_hi[o.lm], 6 * (std::max(l0, l1) + 1));
+  }
+  e->img_order.resize(n);
+  // order: (frame-pair group, landmark, position).  The reference's feature loop hands the factors over landmark by
+  // landmark (trajectory_manager.cpp:360-385), so they usually arrive sorted by landmark already: then a STABLE
+  // counting sort by group is the whole job (O(n), this runs once per window inside the end-to-end time); any other
+  // input order takes the general key sort.
+  bool lm_sorted = true;
+  for (int k = 1; k < n && lm_sorted; ++k) lm_sorted = e->img[k - 1].lm <= e->img[k].lm;
+  const size_t nKk = size_t(e->nK) + 1;
+  if (lm_sorted && nKk * nKk <= (size_t(1) << 22)) {
+    std::vector<int32_t> start(nKk * nKk + 1, 0);
+    for (int k = 0; k < n; ++k) ++start[size_t(wi0[k]) * nKk + size_t(wj0[k]) + 1];
+    for (size_t g = 1; g < start.size(); ++g) start[g] += start[g - 1];
+    for (int k = 0; k < n; ++k) e->img_order[start[size_t(wi0[k]) * nKk + size_t(wj0[k])]++] = k;
+  } else {
+    std::vector<uint64_t> key(n);
+    const uint64_t nLl = uint64_t(std::max(e->nL, 1));
+    if (uint64_t(nKk) * nKk * nLl < (uint64_t(1) << 40) && uint64_t(n) < (uint64_t(1) << 24)) {
+      for (int k = 0; k < n; ++k)
+        key[k] = (((uint64_t(wi0[k]) * nKk + uint64_t(wj0[k])) * nLl + uint64_t(e->img[k].lm)) << 24) | uint64_t(k);
+      std::sort(key.begin(), key.end());
+      for (int k = 0; k < n; ++k) e->img_order[k] = int32_t(key[k] & 0xffffffu);
+    } else {
+      for (int k = 0; k < n; ++k) e->img_order[k] = k;
+      std::stable_sort(e->img_order.begin(), e->img_order.end(), [&](int a, int b) {
+        if (wi0[a] != wi0[b]) return wi0[a] < wi0[b];
+        if (wj0[a] != wj0[b]) return wj0[a] < wj0[b];
+        return e->img[a].lm < e->img[b].lm;
+      });
+    }
+  }
+  std::vector<longlong2> ht(n);
+  std::vector<double2> hpi(n), hpj(n);
+  std::vector<int4> hm(n);
+  for (int k = 0; k < n; ++k) {
+    const HostImage& o = e->img[e->img_order[k]];
+    ht[k] = make_longlong2(o.ti, o.tj);
+    hpi[k] = make_double2(o.pi[0], o.pi[1]);
+    hpj[k] = make_double2(o.pj[0], o.pj[1]);
+    hm[k] = make_int4(o.rowi, o.rowj, o.lm, o.marg);
+  }
+  // work items: chunks of one group, one evaluation round (<= 128 observations, a lane pair each) per CTA.  The
+  // round is latency bound whatever its fill, so a group is cut into EQUAL chunks (263 observations -> 3 x 88, not
+  // 128 + 128 + 7) and every chunk gets its own CTA.  A window with fewer chunks than SMs has its groups cut finer
+  // (the cap halved down to kVisMinChunk) as long as all chunks still run at once: each CTA then has fewer rows to
+  // evaluate and to reduce in its SYRK, on SMs that would otherwise idle.  A window that fills the SMs keeps full
+  // rounds (finer chunks would only add flushes).
+  std::vector<int2> groups;  // [first, end) in sorted order
+  for (int k = 0; k < n;) {
+    const int a = e->img_order[k];
+    int end = k;
+    while (end < n && wi0[e->img_order[end]] == wi0[a] && wj0[e->img_order[end]] == wj0[a]) ++end;
+    groups.push_back(make_int2(k, end));
+    k = end;
+  }
+  auto n_chunks = [&](int c) {
+    size_t m = 0;
+    for (const int2& g : groups) m += (g.y - g.x + c - 1) / c;
+    return m;
+  };
+  int cap = kVisObsPerRound;
+  const size_t n_sm = size_t(device_sm_count());
+  while (cap / 2 >= kVisMinChunk && n_chunks(cap / 2) <= n_sm) cap /= 2;
+  std::vector<VisualItem> items;
+  for (const int2& g : groups) {
+    const int a = e->img_order[g.x];
+    const int cnt = g.y - g.x;
+    const int nchunks = (cnt + cap - 1) / cap;
+    const int per = (cnt + nchunks - 1) / nchunks;
+    for (int s = g.x; s < g.y; s += per) items.push_back(VisualItem{s, std::min(per, g.y - s), wi0[a], wj0[a]});
+  }
+  e->n_items = int(items.size());
+  if (!e->img_desc.empty()) {
+    // slot-named factors: only the sorted 16-byte descriptors go up, the SoA payload is gathered on the device
+    std::vector<ctvio::FactorDesc> sd(n);
+    for (int k = 0; k < n; ++k) sd[k] = e->img_desc[e->img_order[k]];
+    CUDA_OK(e->d_img_desc.upload(sd, st));
+    if (const int rc = gather_factors(e, n)) return rc;
+  } else {
+    CUDA_OK(e->d_img_t.upload(ht, st));
+    CUDA_OK(e->d_img_pi.upload(hpi, st));
+    CUDA_OK(e->d_img_pj.upload(hpj, st));
+    CUDA_OK(e->d_img_meta.upload(hm, st));
+  }
+  CUDA_OK(e->d_img_orig.upload(e->img_order, st));
+  CUDA_OK(e->d_items.upload(items, st));
+
+  // ---- landmark layout; a landmark with a factor is active (the landmark part of the active mask) ----
+  e->h_woff.assign(e->nL + 1, 0);
+  e->h_active.assign(size_t(d.np) + e->nL, 0);
+  for (int l = 0; l < e->nL; ++l) {
+    if (e->h_hi[l] == 0) e->h_lo[l] = 0;
+    e->h_woff[l + 1] = e->h_woff[l] + (e->h_hi[l] - e->h_lo[l]);
+    e->h_active[d.np + l] = e->h_hi[l] > 0 ? 1 : 0;
+  }
+  CUDA_OK(e->d_lo.upload(e->h_lo, st));
+  CUDA_OK(e->d_hi.upload(e->h_hi, st));
+  CUDA_OK(e->d_woff.upload(e->h_woff, st));
+  e->w_len = e->h_woff[e->nL];
+  return CTVIO_OK;
+}
+
+int schur_lists_host(ctvio_engine* e, int T) {
+  // per 64x64 tile (ti >= tj) of the reduced system the landmarks whose knot-dim range [lo, hi) touches both blocks,
+  // cut into parts of `part` landmarks so that about two waves of CTAs exist whatever the window size (the line-delay
+  // row / column is a matrix-vector product done by the diagonal tiles)
+  std::vector<std::vector<int32_t>> lists(size_t(T) * (T + 1) / 2);
+  std::vector<int32_t> order;
+  for (int l = 0; l < e->nL; ++l)
+    if (e->h_hi[l] > 0) order.push_back(l);
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) {
+    if (e->h_lo[a] != e->h_lo[b]) return e->h_lo[a] < e->h_lo[b];
+    return e->h_hi[a] < e->h_hi[b];
+  });
+  size_t total = 0;
+  for (int l : order) {
+    int blocks[64], nbk = 0;
+    const int b0 = e->h_lo[l] / kCholNB, b1 = (e->h_hi[l] - 1) / kCholNB;
+    for (int b = b0; b <= b1 && nbk < 63; ++b) blocks[nbk++] = b;
+    for (int x = 0; x < nbk; ++x)
+      for (int y = 0; y <= x; ++y) {
+        lists[size_t(blocks[x]) * (blocks[x] + 1) / 2 + blocks[y]].push_back(l);
+        ++total;
+      }
+  }
+  const int part = std::max(32, int((total / size_t(2 * device_sm_count()) + 31) / 32) * 32);
+  std::vector<SchurTileItem> items;
+  std::vector<SchurEntry> flat;
+  flat.reserve(total);
+  for (int ti = 0; ti < T; ++ti)
+    for (int tj = 0; tj <= ti; ++tj) {
+      const std::vector<int32_t>& v = lists[size_t(ti) * (ti + 1) / 2 + tj];
+      for (size_t s0 = 0; s0 < v.size(); s0 += part)
+        items.push_back(SchurTileItem{ti, tj, int32_t(flat.size() + s0), int32_t(std::min(v.size() - s0, size_t(part)))});
+      for (int32_t l : v) flat.push_back(SchurEntry{l, e->h_lo[l], e->h_hi[l], 0, e->h_woff[l]});
+    }
+  e->n_schur_items = int(items.size());
+  e->n_schur_entries = int(flat.size());
+  CUDA_OK(e->d_schur_list.upload(flat, e->stream));
+  CUDA_OK(e->d_schur_items.upload(items, e->stream));
+  return CTVIO_OK;
+}
+
+int marg_discover_host(ctvio_engine* e, std::vector<uint32_t>& knots, int& n_marg, int& n_rho,
+                       std::vector<int32_t>& marg_img, std::vector<int32_t>& pos_lm) {
+  knots.assign((size_t(e->nK) + 31) / 32, 0u);
+  marg_img.clear();
+  pos_lm.assign(size_t(std::max(e->nL, 1)), -1);
+  for (size_t k = 0; k < e->img_order.size(); ++k) {
+    const HostImage& o = e->img[e->img_order[k]];
+    if (!o.marg) continue;
+    marg_img.push_back(int32_t(k));
+    pos_lm[o.lm] = 0;
+    for (const int64_t t : {o.ti, o.tj}) {
+      int f = 0, l = -1;
+      knot_window(e, t, f, l);  // checked by the structure build
+      for (int kk = f; kk <= l; ++kk) knots[size_t(kk) / 32] |= 1u << (kk % 32);
+    }
+  }
+  n_marg = int(marg_img.size());
+  n_rho = 0;
+  for (int32_t& p : pos_lm)
+    if (p == 0) p = n_rho++;
   return CTVIO_OK;
 }
 
