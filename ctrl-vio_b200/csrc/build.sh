@@ -5,7 +5,7 @@
 set -euo pipefail
 cd "$(dirname "$0")"
 OUT=libctvio_b200.so
-SRCS="engine.cu resident.cu odometry.cu checkpoint.cu solve.cu covariance.cu structure.cu kernels_residual.cu kernels_linear.cu chol_coop.cu chol_dag.cu misc_kernels.cu marginalize.cu jacobi_blocked.cu frontend.cu comm.cu"
+SRCS="engine.cu prior.cu resident.cu odometry.cu checkpoint.cu solve.cu covariance.cu structure.cu kernels_residual.cu kernels_linear.cu chol_coop.cu chol_dag.cu misc_kernels.cu marginalize.cu jacobi_blocked.cu frontend.cu comm.cu"
 HDRS="$(ls *.h *.cuh) ../../include/ctvio.h build.sh"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 # NCCL: only <nccl.h> (types) is needed at build time; the library is dlopen'ed by comm.cu on first use.

@@ -433,24 +433,13 @@ int parse_blob(const ctvio_engine* e, const unsigned char* b, int64_t len, CkptH
   for (int k = 0; k < kSections; ++k)
     if (h.section[k].offset != L.off[k] || h.section[k].bytes != L.bytes[k]) return bad("bad section table");
   // the prior's blocks: types, indices and columns as ctvio_set_prior and the solve's preparation check them
-  const int32_t* blk = reinterpret_cast<const int32_t*>(b + L.off[ctvio::kPriorBlocks]);
-  std::vector<uint8_t> covered(size_t(m.prior_n), 0);
-  for (int k = 0; k < m.prior_nb; ++k) {
-    int32_t type, index, col;
-    std::memcpy(&type, blk + k, 4);
-    std::memcpy(&index, blk + m.prior_nb + k, 4);
-    std::memcpy(&col, blk + 2 * m.prior_nb + k, 4);
-    if (type < CTVIO_BLK_ROT || type > CTVIO_BLK_LD) return bad("bad prior block");
-    if (type != CTVIO_BLK_LD && ctvio::prior_block_base(type, index, m.nK, m.nB) < 0) return bad("bad prior block");
-    const int ls = type == CTVIO_BLK_LD ? 1 : 3;
-    if (col < 0 || col + ls > m.prior_n) return bad("bad prior block");
-    for (int c = 0; c < ls; ++c) {
-      if (covered[size_t(col + c)]) return bad("bad prior block");
-      covered[size_t(col + c)] = 1;
-    }
-  }
-  for (uint8_t c : covered)
-    if (!c) return bad("bad prior block");
+  // (a prior never holds an inverse depth: block_base rejects it with the out-of-range types and indices)
+  std::vector<int32_t> blk(3 * size_t(m.prior_nb));  // type | index | col
+  if (!blk.empty()) std::memcpy(blk.data(), b + L.off[ctvio::kPriorBlocks], blk.size() * sizeof(int32_t));
+  const int32_t *type = blk.data(), *index = type + m.prior_nb, *col = index + m.prior_nb;
+  for (int k = 0; k < m.prior_nb; ++k)
+    if (ctvio::block_base(type[k], index[k], m.nK, m.nB) < 0) return bad("bad prior block");
+  if (ctvio::prior_tiling_error(m.prior_n, m.prior_nb, type, col)) return bad("bad prior block");
   return CTVIO_OK;
 }
 

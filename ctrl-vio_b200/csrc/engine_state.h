@@ -429,6 +429,10 @@ int marg_discover_host(ctvio_engine* e, std::vector<uint32_t>& knots, int& n_mar
 // sharded mode: per-landmark owned flags (hi > 0 of the built structure) into either buffer (may be null)
 int owned_flags_device(ctvio_engine* e, double* as_double, uint8_t* as_byte);
 
+// prior.cu: prepare()'s prior stage, and the active prior as the factor kernels see it
+int prepare_prior(ctvio_engine* e);
+PriorPtrs prior_ptrs(ctvio_engine* e);
+
 // engine.cu, used by the LM driver in solve.cu
 int prepare(ctvio_engine* e);  // structures of the factor set, built by structure.cu and the stages of engine.cu
 // first knot of the spline segment of an evaluation time; its padded window [first, last] (false: outside the spline)

@@ -7,6 +7,7 @@
 #include <cstdint>
 #include <utility>
 
+#include "param_blocks.h"
 #include "spline_eval.cuh"
 
 namespace ctvio {
@@ -32,6 +33,37 @@ struct StatePtrs {
   double* ld;      // [1]
   KnotPair* tab;   // [nK-1] knot-pair table of this state
 };
+
+// the state of a parameter block (param_blocks.h): a knot's quaternion or position, a bias node's gyro or accel bias,
+// the line delay, an inverse depth
+__device__ __forceinline__ const double* block_state(const StatePtrs& st, int type, int index) {
+  switch (type) {
+    case CTVIO_BLK_ROT: return st.q + 4 * index;
+    case CTVIO_BLK_POS: return st.p + kPStride * index;
+    case CTVIO_BLK_BG: return st.bias + 6 * index;
+    case CTVIO_BLK_BA: return st.bias + 6 * index + 3;
+    case CTVIO_BLK_LD: return st.ld;
+    default: return st.rho + index;
+  }
+}
+
+// dx = x [-] x0 of a prior block at state x, linearised at x0 (marginalization_factor.cpp:326-373): the rotation's
+// quaternion box-minus, a plain difference otherwise
+__device__ __forceinline__ void prior_block_dx(int type, const double* x, const double* x0, double* dx) {
+  if (type == CTVIO_BLK_ROT) {
+    const double n2 = x0[0] * x0[0] + x0[1] * x0[1] + x0[2] * x0[2] + x0[3] * x0[3];
+    const double ax = -x0[0] / n2, ay = -x0[1] / n2, az = -x0[2] / n2, aw = x0[3] / n2;
+    const double bx = x[0], by = x[1], bz = x[2], bw = x[3];
+    const double qx = aw * bx + ax * bw + ay * bz - az * by;
+    const double qy = aw * by + ay * bw + az * bx - ax * bz;
+    const double qz = aw * bz + az * bw + ax * by - ay * bx;
+    const double qw = aw * bw - ax * bx - ay * by - az * bz;
+    const double sg = (qw >= 0) ? 2.0 : -2.0;
+    dx[0] = sg * qx; dx[1] = sg * qy; dx[2] = sg * qz;
+  } else {
+    for (int d = 0; d < block_dim(type); ++d) dx[d] = x[d] - x0[d];
+  }
+}
 
 // ---- Schur-form normal equations at one linearisation point -------------------------------------
 struct NormalEqPtrs {

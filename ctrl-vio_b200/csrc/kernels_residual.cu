@@ -721,17 +721,6 @@ struct SmallArgs {
   int deterministic;
 };
 
-__device__ __forceinline__ const double* block_data(const StatePtrs& st, int type, int index) {
-  switch (type) {
-    case 0: return st.q + 4 * index;
-    case 1: return st.p + kPStride * index;
-    case 2: return st.bias + 6 * index;
-    case 3: return st.bias + 6 * index + 3;
-    case 4: return st.ld;
-    default: return st.rho + index;
-  }
-}
-
 template <bool FULL>
 __global__ void __launch_bounds__(256) small_factors_kernel(const __grid_constant__ SmallArgs a) {
   __shared__ double red[8];
@@ -762,23 +751,7 @@ __global__ void __launch_bounds__(256) small_factors_kernel(const __grid_constan
   if (n > 0) {
     for (int b = tid; b < a.prior.n_blocks; b += blockDim.x) {
       const int type = a.prior.type[b];
-      const double* x = block_data(a.st, type, a.prior.index[b]);
-      const double* x0 = a.prior.x0 + 4 * b;
-      double* dx = a.prior.dx + a.prior.col[b];
-      if (type == 0) {
-        const double n2 = x0[0] * x0[0] + x0[1] * x0[1] + x0[2] * x0[2] + x0[3] * x0[3];
-        const double ax = -x0[0] / n2, ay = -x0[1] / n2, az = -x0[2] / n2, aw = x0[3] / n2;
-        const double bx = x[0], by = x[1], bz = x[2], bw = x[3];
-        const double qx = aw * bx + ax * bw + ay * bz - az * by;
-        const double qy = aw * by + ay * bw + az * bx - ax * bz;
-        const double qz = aw * bz + az * bw + ax * by - ay * bx;
-        const double qw = aw * bw - ax * bx - ay * by - az * bz;
-        const double sg = (qw >= 0) ? 2.0 : -2.0;
-        dx[0] = sg * qx; dx[1] = sg * qy; dx[2] = sg * qz;
-      } else {
-        const int sz = (type == 4 || type == 5) ? 1 : 3;
-        for (int d = 0; d < sz; ++d) dx[d] = x[d] - x0[d];
-      }
+      prior_block_dx(type, block_state(a.st, type, a.prior.index[b]), a.prior.x0 + 4 * b, a.prior.dx + a.prior.col[b]);
     }
     __syncthreads();
     for (int i = tid; i < n; i += blockDim.x) {

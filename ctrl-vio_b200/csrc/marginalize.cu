@@ -126,24 +126,7 @@ __global__ void marg_small_kernel(MargSmallArgs a) {
   // residual of the old prior at the current state (dx / res scratch as in small_factors_kernel)
   for (int b = tid; b < a.prior.n_blocks; b += blockDim.x) {
     const int type = a.prior.type[b];
-    const int index = a.prior.index[b];
-    const double* x = type == 0 ? a.st.q + 4 * index : type == 1 ? a.st.p + kPStride * index
-                    : type == 2 ? a.st.bias + 6 * index : type == 3 ? a.st.bias + 6 * index + 3 : a.st.ld;
-    const double* x0 = a.prior.x0 + 4 * b;
-    double* dx = a.prior.dx + a.prior.col[b];
-    if (type == 0) {
-      const double n2 = x0[0] * x0[0] + x0[1] * x0[1] + x0[2] * x0[2] + x0[3] * x0[3];
-      const double ax = -x0[0] / n2, ay = -x0[1] / n2, az = -x0[2] / n2, aw = x0[3] / n2;
-      const double qx = aw * x[0] + ax * x[3] + ay * x[2] - az * x[1];
-      const double qy = aw * x[1] + ay * x[3] + az * x[0] - ax * x[2];
-      const double qz = aw * x[2] + az * x[3] + ax * x[1] - ay * x[0];
-      const double qw = aw * x[3] - ax * x[0] - ay * x[1] - az * x[2];
-      const double sg = (qw >= 0) ? 2.0 : -2.0;
-      dx[0] = sg * qx; dx[1] = sg * qy; dx[2] = sg * qz;
-    } else {
-      const int sz = type == 4 ? 1 : 3;
-      for (int d = 0; d < sz; ++d) dx[d] = x[d] - x0[d];
-    }
+    prior_block_dx(type, block_state(a.st, type, a.prior.index[b]), a.prior.x0 + 4 * b, a.prior.dx + a.prior.col[b]);
   }
   __syncthreads();
   for (int i = tid; i < n; i += blockDim.x) {

@@ -1,5 +1,5 @@
-// Small host/device helpers shared by engine.cu: prior bookkeeping, Gram kernel, gradient dot product,
-// NCCL communicator wrappers.
+// Small host/device helpers shared by the engine's host code: the prior's host form (prior.cu), Gram kernel, gradient
+// dot product, NCCL communicator wrappers.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -17,18 +17,6 @@ struct PriorHost {
   std::vector<double> J, r, x0;            // n x n row-major, n, n_blocks x 4
   std::vector<int32_t> type, index, col;   // per kept block
 };
-
-// first camera dim of a parameter block, -1 if it has none / is out of range
-inline int prior_block_base(int type, int index, int nK, int nB) {
-  switch (type) {
-    case 0: return (index >= 0 && index < nK) ? 6 * index : -1;
-    case 1: return (index >= 0 && index < nK) ? 6 * index + 3 : -1;
-    case 2: return (index >= 0 && index < nB) ? 6 * nK + 6 * index : -1;
-    case 3: return (index >= 0 && index < nB) ? 6 * nK + 6 * index + 3 : -1;
-    case 4: return 6 * nK + 6 * nB;
-    default: return -1;
-  }
-}
 
 // G = J' J for a row-major rows x cols matrix (G: cols x cols)
 int launch_gram(const double* J, int rows, int cols, double* G, cudaStream_t s);

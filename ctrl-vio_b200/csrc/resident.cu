@@ -263,9 +263,9 @@ int ctvio_slide_window(ctvio_handle e, int32_t drop_knots, int32_t drop_bias, in
   // the active prior's blocks follow the window: knot / bias-node indices are window relative
   for (size_t b = 0; b < e->prior.type.size(); ++b) {
     const int t = e->prior.type[b];
-    if (t == CTVIO_BLK_ROT || t == CTVIO_BLK_POS) e->prior.index[b] -= drop_knots;
-    else if (t == CTVIO_BLK_BG || t == CTVIO_BLK_BA) e->prior.index[b] -= drop_bias;
-    if ((t <= CTVIO_BLK_BA) && e->prior.index[b] < 0) return fail(CTVIO_ERR_STATE, "a block of the active prior left the window");
+    if (!ctvio::block_is_knot(t) && !ctvio::block_is_bias(t)) continue;
+    e->prior.index[b] -= ctvio::block_is_knot(t) ? drop_knots : drop_bias;
+    if (e->prior.index[b] < 0) return fail(CTVIO_ERR_STATE, "a block of the active prior left the window");
   }
   e->prior_dirty = true;
   e->masks_dirty = true;
@@ -650,11 +650,9 @@ int ctvio_slide_window_second_new(ctvio_handle e) {
   if (e->nB < 2) return fail(CTVIO_ERR_STATE, "the window has fewer than 2 bias nodes");
   const int gone = e->nB - 2;
   // the prior is kept as it is (trajectory_manager.cpp:270-280), so none of its blocks may belong to the leaving node
-  for (size_t b = 0; b < e->prior.type.size(); ++b) {
-    const int t = e->prior.type[b];
-    if ((t == CTVIO_BLK_BG || t == CTVIO_BLK_BA) && e->prior.index[b] == gone)
+  for (size_t b = 0; b < e->prior.type.size(); ++b)
+    if (ctvio::block_is_bias(e->prior.type[b]) && e->prior.index[b] == gone)
       return fail(CTVIO_ERR_STATE, "the active prior holds a block of the second-newest bias node");
-  }
   cudaSetDevice(e->cfg.device);
   // Bgs_/Bas_[WINDOW_SIZE - 1] = [WINDOW_SIZE] (visual_odometry.cpp:253-278); node nB-1 keeps its value and stands for the
   // next image, as the node ctvio_slide_window appends does.  Knots, time origin and prior block indices do not move.

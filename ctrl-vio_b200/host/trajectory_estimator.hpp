@@ -190,7 +190,7 @@ class TrajectoryEstimator {
   // PrepareMarginalizationInfo(RType_Prior, factor, NULL, parameter_blocks, drop_set) (trajectory_estimator.cpp:143-151,
   // trajectory_manager.cpp:166-203): the old prior takes part in the marginalization with an explicit drop set (indices
   // into its block list).  The engine derives the same drop set from options.ctrl_to_be_opt_now / _later and bias node 0
-  // (engine.cu: ctvio_marginalize [1]); here the caller's set is CHECKED against that rule so that a divergence is loud.
+  // (prior.cu: ctvio_marginalize [1]); here the caller's set is CHECKED against that rule so that a divergence is loud.
   void PrepareMarginalizationInfo(ResidualType r_type, const MarginalizationInfo::Ptr& prior, const std::vector<int>& drop_set) {
     if (r_type != RType_Prior || !prior) throw Error(CTVIO_ERR_INVALID, "PrepareMarginalizationInfo: only the prior is recorded explicitly");
     std::vector<int> expect;
